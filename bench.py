@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Headline benchmark: ResNet-18/CIFAR-10 steps/sec at r=3 under s adversaries on N B200s (BASELINE.json metric).
+"""Headline benchmark: ResNet-18/CIFAR-10 steps/sec at r=3 under s adversaries on N H100s.
 
     python bench.py --gpus 1 --steps 20 --warmup 5
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 --master-port 29500 \
@@ -15,10 +15,10 @@ every N (strong scaling): with N < 8 the logical ranks are packed onto the GPUs 
            pinned host memory to the device and reads the loss back to the host.
 --impl reference : the unmodified reference cannot be installed here (Python 2.7 / torch 0.3 / mpi4py, no setup.py) ->
            prints {"impl": "reference", "unavailable": ...}.
---impl nccl      : our reference-faithful NCCL baseline (per-tensor messages, library-op decode; BASELINE.md section 4).
+--impl nccl      : our reference-faithful NCCL baseline (per-tensor messages, library-op decode).
 --impl nccl_flat : the honest library comparator (flat arenas, ONE broadcast + ONE message per worker, vectorised torch vote,
            CUDA graphs, cuDNN / ATen model compute): parallel/flat_engine.py.  `vs_baseline` divides by the FASTER of the two
-           library arms recorded in baseline/measured_nccl.json.
+           library arms when their rates are recorded in baseline/measured_nccl.json (null otherwise).
 """
 from __future__ import annotations
 
@@ -29,9 +29,8 @@ import sys
 import time
 
 METRIC = "ResNet-18/CIFAR-10 steps/sec at r=3 under s adversaries"
-REF_UNAVAILABLE = ("hwang595/Draco is Python-2.7/PyTorch-0.3/mpi4py code with no setup.py or pyproject.toml: "
-                   "`pip install --no-index --target baseline/_ref /root/reference` fails with 'Neither setup.py nor "
-                   "pyproject.toml found'; mpi4py, blosc, hdmedians and Eigen are not in the offline wheelhouse")
+REF_UNAVAILABLE = ("hwang595/Draco is Python-2.7/PyTorch-0.3/mpi4py code with no setup.py or pyproject.toml: it cannot be "
+                   "installed as a package ('Neither setup.py nor pyproject.toml found') and needs mpi4py, blosc, hdmedians and Eigen")
 
 
 def parse():
@@ -42,7 +41,7 @@ def parse():
     ap.add_argument("--impl", type=str, default="ours", choices=("ours", "reference", "nccl", "nccl_flat"))
     ap.add_argument("--network", type=str, default="ResNet18")
     ap.add_argument("--dataset", type=str, default="Cifar10", help="Cifar10 (3x32x32) | ImageNet (synthetic 3x224x224, 1000 classes: "
-                    "ResNets get the 7x7/s2 stem + max-pool, BASELINE.json config 5) | MNIST")
+                    "ResNets get the 7x7/s2 stem + max-pool) | MNIST")
     ap.add_argument("--synthetic-size", type=int, default=None)
     ap.add_argument("--approach", type=str, default="maj_vote")
     ap.add_argument("--mode", type=str, default="maj_vote")
@@ -70,7 +69,29 @@ def parse():
                     help="like --timeline but for 3 steps of the end-to-end loop (Trainer.train_step_pipelined, pinned H2D + D2H)")
     ap.add_argument("--worker-streams", type=int, default=None,
                     help="concurrent CUDA streams for logical workers sharing a GPU (default: the JobConfig default)")
+    ap.add_argument("--dump-outputs", type=str, default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step produced as DIR/<name>.npy: params.npy (the fp32 "
+                         "parameter arena; a fixed, seeded sample when it exceeds 60 MB) and metrics.npy (loss, Prec@1, Prec@5, float64)")
     return ap.parse_args()
+
+
+DUMP_MAX_ELEMS = 60 * 2 ** 20 // 4
+
+
+def _dump_outputs(path, params, metrics):
+    """Outputs of the timed path for comparing two builds: the same arguments give the same inputs (seeded model, data and
+    adversaries), so two builds can be compared array by array."""
+    import numpy as np
+    import torch
+    os.makedirs(path, exist_ok=True)
+    flat = params.detach().reshape(-1)
+    if flat.numel() > DUMP_MAX_ELEMS:
+        g = torch.Generator().manual_seed(0)
+        idx = torch.randperm(flat.numel(), generator=g)[:DUMP_MAX_ELEMS].sort().values
+        flat = flat[idx.to(flat.device)]
+    np.save(os.path.join(path, "params.npy"), flat.float().cpu().numpy())
+    np.save(os.path.join(path, "metrics.npy"), np.array([metrics.get(k, float("nan")) for k in ("loss", "prec1", "prec5")],
+                                                        dtype=np.float64))
 
 
 def _write_timeline(path, trainer, rank, barrier, pipelined=False):
@@ -236,6 +257,8 @@ def main() -> int:
                  "worker_wait_for_params_ms_mean": sum(ww) / len(ww) if ww else None,
                  "worker_wait_for_params_ms_min": min(ww) if ww else None} if traces and any(traces) else None
     m = eng.read_metrics()
+    if a.dump_outputs and rank == 0:
+        _dump_outputs(a.dump_outputs, eng.master_params(), m)
     if a.timeline:
         _write_timeline(a.timeline, trainer, rank, barrier)
     trainer.close()
@@ -297,7 +320,7 @@ def main() -> int:
                        "placement": eng.place.describe(), "code": f"repetition r={a.group_size} majority-vote" if a.approach == "maj_vote" else a.approach,
                        "adversaries_per_step": a.worker_fail, "err_mode": a.err_mode, "transport": transport,
                        "cuda_graphs": bool(cfg.cuda_graphs), "wgrad_stream": a.wgrad_stream, "worker_streams": len(getattr(eng, "worker_streams", None) or getattr(eng, "streams", None) or []) or 1, "nvls_multicast": bool(getattr(eng, "mc_params", None)),
-                       "l2": "per-step working set (7x44.7 MB gradient slab + activations) exceeds the 126 MB L2; no explicit flush",
+                       "l2": "per-step working set (7x44.7 MB gradient slab + activations) exceeds the 50 MB L2; no explicit flush",
                        "images_per_s": value * a.batch_size * a.num_workers,
                        "note": ("adversaries are drawn over all workers each step like the reference (src/util.py:100-103), so "
                                 "with r=3 and 3 liars a group can be out-voted and the loss may diverge; throughput is "

@@ -1,6 +1,6 @@
 // K10 (normalisation part): fused training-mode BatchNorm + residual add + ReLU for NHWC bf16 activations (third iteration).
 //
-// What changed against round 1 (profiles/ncu_bn.md: 10-14 us per launch at 14-35 % of HBM, four launches per layer):
+// Design (a plain statistics + apply implementation costs four launches per layer, each far from HBM bandwidth):
 //   * the forward statistics normally come out of the producing convolution's epilogue (conv_epilogue.cuh), so a layer's
 //     forward is ONE streaming kernel: bn_apply_kernel (x, mean, invstd, residual -> y, ReLU fused).  bn_stats_kernel remains
 //     for producers that are not ours (GEMM-served 1x1 convolutions, library fallbacks);

@@ -1,4 +1,4 @@
-// Shared device-side definitions for the draco_b200 step-path kernels (sm_100a only).
+// Shared device-side definitions for the draco_b200 step-path kernels (sm_90a only).
 //
 // Arena model: every rank keeps its parameters / gradients / momentum in flat arenas that share one
 // element layout.  A tensor starts at a multiple of TILE elements and owns ceil(numel / TILE) tiles, so a

@@ -1,6 +1,7 @@
-// Epilogue shared by the tcgen05 convolution kernels (conv_tap_tcgen05.cu, conv_halo_tcgen05.cu).
+// Epilogue shared by the wgmma convolution kernels (conv_tap_wgmma.cu, conv_halo_wgmma.cu).
 //
-// A finished 128-pixel x BLOCK_N accumulator tile leaves TMEM through the four epilogue warps (thread = pixel row) and is
+// A finished 128-pixel x BLOCK_N accumulator tile leaves the registers of the MMA warpgroup (handed over thread = pixel row,
+// tc::acc_row32) and is
 //   1. converted to bf16 (+ bias) and written into a shared-memory staging tile in the 128B-swizzled layout TMA expects
 //      (row = pixel, 16-byte chunk j of row r at chunk j ^ (r & 7): conflict-free 16-byte stores);
 //   2. handed to ONE TMA tensor store per 64-channel half (cp.async.bulk.tensor...global.shared::cta, SASS UTMASTG) -- the
@@ -21,11 +22,11 @@
 //
 // Reference counterpart: nn.Conv2d followed by nn.BatchNorm2d in src/model_ops/resnet.py:19-24, vgg.py:46-59.
 #pragma once
-#include "tcgen05_common.cuh"
+#include "wgmma_common.cuh"
 
 namespace convepi {
 
-constexpr int EPI_THREADS = 128;          // warps 4..7
+constexpr int EPI_THREADS = 128;          // warps 4..7 (the MMA warpgroup)
 constexpr int EPI_BAR_ID = 1;
 constexpr int STAT_MAX_C = 512;
 
@@ -52,30 +53,25 @@ struct BnStatArgs {
 __host__ __device__ constexpr int staging_bytes(int block_n) { return block_n * 128 * 2; }          // 128 rows x block_n bf16
 __host__ __device__ constexpr int stat_bytes() { return 4 * 2 * STAT_MAX_C * 4; }                   // [4 warps][2][512] fp32
 
-// Drain one accumulator tile.  Called by all 128 epilogue threads (et = 0..127 = tile row).
-//   tmem_acc : TMEM address of column 0 of this accumulator (lane field 0)
+// Drain one accumulator tile.  Called by all 128 threads of the MMA warpgroup (et = 0..127 = tile row).
+//   acc      : the tile's accumulators (wgmma fragment of this thread), scratch: tc::SCRATCH_BYTES of shared memory
 //   sbuf     : staging tile (1024-byte aligned), s_stat: statistics accumulators or null
 //   valid_rows: rows of the tile that are real pixels (partial batch tiles), col0: first output channel of the tile
 template <int BLOCK_N>
-__device__ __forceinline__ void drain_tile(uint32_t tmem_acc, uint8_t* sbuf, float* s_stat, int et, int valid_rows, int col0, int Cn,
-                                           const float* bias_f32, const __nv_bfloat16* bias_bf16, uint64_t* tmem_empty_bar,
-                                           uint32_t remote_empty_bar = 0, const __nv_bfloat16* resid_row = nullptr,
-                                           const __nv_bfloat16* mask_row = nullptr) {
+__device__ __forceinline__ void drain_tile(const float (&acc)[2][BLOCK_N / 2], float* scratch, uint8_t* sbuf, float* s_stat, int et,
+                                           int valid_rows, int col0, int Cn, const float* bias_f32, const __nv_bfloat16* bias_bf16,
+                                           const __nv_bfloat16* resid_row = nullptr, const __nv_bfloat16* mask_row = nullptr) {
   // mask_row: channel 0 of this thread's pixel in a tensor of the output's shape; the output is zeroed where it is <= 0 (ReLU
   // backward of the BatchNorm output that fed this convolution), after the residual add
   // resid_row: channel 0 of THIS thread's output pixel in a tensor of the output's shape that is added to the tile before rounding
   // (dgrad: the gradient arriving over the other branch of a fork, e.g. the residual shortcut); null = nothing to add / row invalid
-  const int q = et >> 5, lane = et & 31;
   // the previous tile's TMA store must have finished READING the staging tile before it is overwritten
   if (et == 0) tc::tma_store_wait_read<0>();
   tc::named_bar_sync(EPI_BAR_ID, EPI_THREADS);
-#pragma unroll 1
-  for (int c = 0; c < BLOCK_N; c += 32) {
-    uint32_t v[32];
-    tc::tmem_ld_32x32b_x32(tmem_acc + ((uint32_t)(q * 32) << 16) + (uint32_t)c, v);
-    float f[32];
 #pragma unroll
-    for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
+  for (int c = 0; c < BLOCK_N; c += 32) {
+    float f[32];
+    tc::acc_row32<BLOCK_N>(acc, c, scratch, et, f, EPI_BAR_ID);
     if (bias_f32 || bias_bf16) {
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
@@ -118,13 +114,6 @@ __device__ __forceinline__ void drain_tile(uint32_t tmem_acc, uint8_t* sbuf, flo
       const int phys = (lc0 + jj) ^ (et & 7);
       *reinterpret_cast<uint4*>(row + phys * 16) = tc::pack8(f + jj * 8);
     }
-  }
-  // TMEM fully read by this warp -> the MMA warp may reuse the accumulator
-  tc::tcgen05_fence_before();
-  __syncwarp();
-  if (lane == 0) {
-    if (remote_empty_bar) tc::remote_arrive(remote_empty_bar);     // CTA pair: the barrier lives in the leader CTA
-    else tc::mbar_arrive(tmem_empty_bar);
   }
   tc::fence_async_smem();                          // generic-proxy writes -> visible to the TMA store
   tc::named_bar_sync(EPI_BAR_ID, EPI_THREADS);

@@ -1,9 +1,8 @@
 // K10 (convolution part, continued): the 3-channel stem convolution (3x3 / stride 1 / pad 1, Cin = 3, Cout = 64) on CUDA cores.
 //
-// K = 27 is far too small for the tensor-core path (a UMMA K-step is 16 and a TMA row must be a multiple of 16 bytes; a
+// K = 27 is far too small for the tensor-core path (a wgmma K-step is 16 and a TMA row must be a multiple of 16 bytes; a
 // 3-channel bf16 pixel is 6 bytes), and the work is tiny: 0.45 GFLOP per ResNet-18 step at B = 128, but the output / dy
-// tensors are the largest of the network (16.8 MB).  cuDNN serves the layer with legacy kernels (35 us fprop, 47 us wgrad);
-// the first version of this file took 65 / 76 us because every FMA was paired with a shared-memory load.  Second version:
+// tensors are the largest of the network (16.8 MB).  Pairing every FMA with a shared-memory load makes such a kernel slow, hence this layout:
 //
 //   stem_fprop_kernel : persistent CTAs over 256-pixel tiles.  The (rows+2) x (W+2) input halo patch sits in shared memory as
 //                       fp32 float4 per pixel (3 channels + pad), the 27 x 64 weights as fp32.  A thread computes 4 consecutive

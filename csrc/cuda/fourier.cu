@@ -100,8 +100,8 @@ struct LocateArgs {
 };
 
 // One CTA per tensor: the locator is a serial O(n^3) fp64 computation per tensor, so the only parallelism is ACROSS tensors -- and
-// fp64 throughput per SM is tiny on this part, so the tensors are spread over as many SMs as there are tensors (62 CTAs for
-// ResNet-18) instead of sharing the fp64 pipe of two SMs (one warp per 32 tensors: 63 us in profiles/ncu_cyclic.md).
+// the chain is latency-bound, so the tensors are spread over as many SMs as there are tensors (62 CTAs for ResNet-18) instead of
+// sharing the fp64 pipe of two SMs (one warp per 32 tensors).
 __global__ void __launch_bounds__(32) cyclic_locate_kernel(const __grid_constant__ LocateArgs a) {
   const int t = blockIdx.x;
   if (threadIdx.x != 0 || t >= a.T) return;

@@ -2,7 +2,7 @@
 //
 // The worker's loss tail -- logits.float(), log_softmax, nll_loss, their two backward kernels, the cast of the gradient
 // back to bf16, topk, eq, the reductions and the three scalar updates of the metrics tensor -- is a chain of ~20 dependent
-// 2-3 us launches on a [B, 10] tensor (profiles/worker_profile_ResNet18_fused.txt).  This kernel reads the logits once and
+// short launches on a [B, 10] tensor.  This kernel reads the logits once and
 // produces everything: mean loss, d(loss)/d(logits) = (softmax - onehot) / B in the logits' dtype, and the Prec@k counts,
 // accumulated straight into the worker's metrics tensor (loss, prec1, prec5).  One warp per row, rows distributed over the
 // 32 warps of ONE CTA, all cross-row sums folded in a fixed order (bit-deterministic, as the exact-equality vote needs).

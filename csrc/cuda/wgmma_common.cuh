@@ -1,0 +1,299 @@
+// Shared sm_90a building blocks of every tensor-core kernel in this tree (GEMM, tap-table / halo convolutions, wgrad):
+// mbarrier + TMA (load, multicast load, store) wrappers, the wgmma shared-memory descriptor and warpgroup MMA wrappers, the
+// register-accumulator -> row hand-over the epilogues use, and the host-side cuTensorMapEncodeTiled lookup.  One copy instead of
+// one per .cu file.
+//
+// Kernel shape shared by the tensor-core kernels: warp 0 is the TMA producer (one elected lane), warpgroup 1 (warps 4-7) issues
+// wgmma on a 128-row tile (two m64 halves, fp32 accumulators in registers) and then runs the epilogue of that tile while the
+// producer already fills the stages of the next one.
+//
+// Every shared-memory operand starts on a 1024-byte boundary of a 128B-swizzled tile or at +32 / +64 / +96 bytes (K steps inside
+// a swizzle row) or +2048 bytes (16 K rows of an MN-major tile), so the descriptor base-offset field is always 0.
+//
+// Every blocking wait carries a watchdog: a wait that does not complete within ~2 s of spinning traps the kernel (a CUDA error
+// the host sees) instead of hanging the GPU.
+#pragma once
+#include <cuda.h>
+#include <cuda_bf16.h>
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+namespace tc {
+
+constexpr int MMA_K = 16;             // K per wgmma for 16-bit operands
+
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
+// ------------------------------------------------------------------------------------------------------------- mbarrier
+__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_fence_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+  const uint32_t addr = smem_u32(bar);
+  uint32_t done = 0, spins = 0;
+  while (true) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}"
+        : "=r"(done) : "r"(addr), "r"(parity) : "memory");
+    if (done) break;
+    if (++spins > (1u << 24)) __trap();            // try_wait suspends for ~1 us per failed poll: seconds, not a hang
+  }
+}
+__device__ __forceinline__ bool elect_one() {
+  uint32_t pred;
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t.reg .b32 r;\n\t"
+      "elect.sync r|p, 0xffffffff;\n\t"
+      "selp.u32 %0, 1, 0, p;\n\t}"
+      : "=r"(pred));
+  return pred != 0;
+}
+// named barrier among `count` threads (count % 32 == 0); id 1..15 (0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
+
+// ------------------------------------------------------------------------------------------------------------------ TMA
+__device__ __forceinline__ void prefetch_tmap(const CUtensorMap* t) { asm volatile("prefetch.tensormap [%0];" ::"l"(t) : "memory"); }
+__device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* tmap, int c0, int c1, uint64_t* bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+      ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(c0), "r"(c1), "r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* tmap, int c0, int c1, int c2, int c3, uint64_t* bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
+      ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(smem_u32(bar)) : "memory");
+}
+// multicast: the box lands at the same shared-memory offset in every CTA of `mask`, each CTA's barrier (same offset) gets the bytes
+__device__ __forceinline__ void tma_load_2d_mc(void* smem_dst, const CUtensorMap* tmap, int c0, int c1, uint64_t* bar, uint16_t mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%2, %3}], [%4], %5;"
+      ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(c0), "r"(c1), "r"(smem_u32(bar)), "h"(mask) : "memory");
+}
+__device__ __forceinline__ void tma_load_4d_mc(void* smem_dst, const CUtensorMap* tmap, int c0, int c1, int c2, int c3, uint64_t* bar,
+                                               uint16_t mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%2, %3, %4, %5}], [%6], %7;"
+      ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(smem_u32(bar)), "h"(mask) : "memory");
+}
+// shared -> global tile stores (bulk async-group completion)
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* tmap, const void* smem_src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+               ::"l"(tmap), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+}
+__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+template <int N>
+__device__ __forceinline__ void tma_store_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+// generic-proxy writes to shared memory -> visible to the async proxy (TMA store)
+__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// ------------------------------------------------------------------------------------------------------------- clusters
+__device__ __forceinline__ uint32_t cluster_rank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
+  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// arrive on the barrier at the same shared-memory offset in CTA `cta_rank` of this cluster
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta_rank) {
+  uint32_t remote;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(cta_rank));
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+}
+
+// ---------------------------------------------------------------------------------------------------------------- wgmma
+// 64-bit shared-memory matrix descriptor (sm_90 GMMA layout), SWIZZLE_128B:
+//   K-major  tile [rows][64 k]        : 8-row groups `sbo_bytes` apart (1024 for a dense tile); LBO unused (= 1 like CUTLASS)
+//   MN-major tile [64 k][64 mn] boxes : 8-k-row groups `sbo_bytes` apart; 64-wide MN atoms `lbo_bytes` apart
+__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t sbo_bytes, uint32_t lbo_field) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr >> 4) & 0x3fff);
+  d |= (uint64_t)(lbo_field & 0x3fff) << 16;
+  d |= (uint64_t)((sbo_bytes >> 4) & 0x3fff) << 32;
+  d |= 1ull << 62;                    // layout type 1: 128-byte swizzle
+  return d;
+}
+__device__ __forceinline__ uint64_t desc_kmajor(uint32_t smem_addr, uint32_t sbo_bytes = 1024) { return make_desc(smem_addr, sbo_bytes, 1); }
+__device__ __forceinline__ uint64_t desc_mnmajor(uint32_t smem_addr, uint32_t atom_pitch_bytes, uint32_t sbo_bytes = 1024) {
+  return make_desc(smem_addr, sbo_bytes, atom_pitch_bytes >> 4);
+}
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across a wgmma wait
+template <int N>
+__device__ __forceinline__ void fence_acc(float* d) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D[64 x N] (+)= A[64 x 16] * B[16 x N], bf16 operands from shared memory, fp32 accumulators in registers.
+// TA / TB: 0 = K-major, 1 = MN-major operand.  `accumulate` = 0 overwrites D.
+template <int N, int TA, int TB>
+struct Wgmma;
+template <int TA, int TB>
+struct Wgmma<32, TA, TB> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+  }
+};
+template <int TA, int TB>
+struct Wgmma<64, TA, TB> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+  }
+};
+template <int TA, int TB>
+struct Wgmma<128, TA, TB> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+  }
+};
+template <int TA, int TB>
+struct Wgmma<192, TA, TB> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %98, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n192k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95}, %96, %97, p, 1, 1, %99, %100;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95])
+        : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+  }
+};
+
+// One K block (64) of a 128 x BN tile on one warpgroup: A rows 64..127 start 8 KB after rows 0..63 (K-major: 64 rows of 128 B;
+// MN-major: the second 64-wide atom), B is K-major [BN rows][64 k] or MN-major [64 k][64 n] atoms 8 KB apart.
+template <int BN, bool A_MN, bool B_MN>
+__device__ __forceinline__ void mma_kblock(float (&acc)[2][BN / 2], uint32_t sa, uint32_t sb, bool first) {
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < 64 / MMA_K; ++k) {
+    const uint32_t adv_a = A_MN ? k * MMA_K * 128 : k * MMA_K * 2;
+    const uint32_t adv_b = B_MN ? k * MMA_K * 128 : k * MMA_K * 2;
+    const uint64_t db = B_MN ? desc_mnmajor(sb + adv_b, 64 * 128) : desc_kmajor(sb + adv_b);
+    const uint32_t accum = (first && k == 0) ? 0u : 1u;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint32_t a = sa + h * 8192 + adv_a;
+      Wgmma<BN, A_MN, B_MN>::mma(acc[h], A_MN ? desc_mnmajor(a, 64 * 128) : desc_kmajor(a), db, accum);
+    }
+  }
+  wgmma_commit();
+}
+
+// Accumulator -> rows.  Thread t of warp w (in the warpgroup) holds, for half h, rows 64h + 16w + t/4 (+8) and columns
+// 8j + 2(t%4) (+1) at acc[h][4j + {0,1,2,3}].  The epilogues work thread-per-row (thread et owns tile row et): acc_row32 hands
+// columns [c, c + 32) of row et to thread et through `scratch` (128 x 17 floats), 16 columns at a time.  All 128 threads of the
+// warpgroup call it with the same compile-time c.
+constexpr int SCRATCH_PITCH = 17;
+constexpr int SCRATCH_BYTES = 128 * SCRATCH_PITCH * 4;
+template <int BN>
+__device__ __forceinline__ void acc_row32(const float (&acc)[2][BN / 2], int c, float* scratch, int et, float* f, int bar_id) {
+  const int w = et >> 5, l = et & 31;
+#pragma unroll
+  for (int q = 0; q < 2; ++q) {
+    named_bar_sync(bar_id, 128);                    // the previous chunk has been read by every row
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int jj = 0; jj < 2; ++jj) {
+        const int j = (c >> 3) + 2 * q + jj;
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+          const int row = 64 * h + 16 * w + (l >> 2) + 8 * (r >> 1);
+          scratch[row * SCRATCH_PITCH + 8 * jj + 2 * (l & 3) + (r & 1)] = acc[h][4 * j + r];
+        }
+      }
+    }
+    named_bar_sync(bar_id, 128);
+#pragma unroll
+    for (int k = 0; k < 16; ++k) f[16 * q + k] = scratch[et * SCRATCH_PITCH + k];
+  }
+}
+
+// pack 8 floats -> 8 bf16 (16 bytes)
+__device__ __forceinline__ uint4 pack8(const float* f) {
+  __nv_bfloat162 p0 = __floats2bfloat162_rn(f[0], f[1]), p1 = __floats2bfloat162_rn(f[2], f[3]);
+  __nv_bfloat162 p2 = __floats2bfloat162_rn(f[4], f[5]), p3 = __floats2bfloat162_rn(f[6], f[7]);
+  uint4 o;
+  o.x = *reinterpret_cast<uint32_t*>(&p0); o.y = *reinterpret_cast<uint32_t*>(&p1);
+  o.z = *reinterpret_cast<uint32_t*>(&p2); o.w = *reinterpret_cast<uint32_t*>(&p3);
+  return o;
+}
+
+// ------------------------------------------------------------------------------------------------------------ host side
+typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+inline PFN_encodeTiled get_encode() {
+  static PFN_encodeTiled fn = nullptr;
+  if (!fn) {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
+      fn = reinterpret_cast<PFN_encodeTiled>(p);
+  }
+  return fn;
+}
+
+// NHWC bf16 activation [N][H][W][C] as a 4-D map with 64-channel boxes of bw x bh x bn pixels (every `estride`-th pixel)
+inline int encode_act(CUtensorMap* tm, const void* base, int C, int W, int H, int N, int bw, int bh, int bn, int estride) {
+  PFN_encodeTiled enc = get_encode();
+  if (!enc) return -2;
+  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
+  cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
+  cuuint32_t box[4] = {64, (cuuint32_t)(bw * estride), (cuuint32_t)(bh * estride), (cuuint32_t)bn};
+  cuuint32_t estr[4] = {1, (cuuint32_t)estride, (cuuint32_t)estride, 1};
+  return (int)enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+}
+// row-major bf16 matrix [rows][cols] with 64-column x box_rows boxes
+inline int encode_mat(CUtensorMap* tm, const void* base, long long rows, long long cols, long long ld_elems, int box_rows) {
+  PFN_encodeTiled enc = get_encode();
+  if (!enc) return -2;
+  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  cuuint64_t strides[1] = {(cuuint64_t)ld_elems * 2};
+  cuuint32_t box[2] = {64, (cuuint32_t)box_rows};
+  cuuint32_t estr[2] = {1, 1};
+  return (int)enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+}
+
+}  // namespace tc

@@ -1,9 +1,9 @@
-"""draco_b200: a Blackwell-native Byzantine-resilient data-parallel trainer with Draco's capabilities.
+"""draco_b200: a Hopper-native (H100) Byzantine-resilient data-parallel trainer with Draco's capabilities.
 
 Layout
   codes/     repetition + cyclic (Fourier) gradient codes, adversary model, fp64 oracles
   models/    LeNet, FC, ResNet-18..152, VGG-11..19 (+ *Split layer-wise backward drivers)
-  ops/       launchers for the sm_100a kernels (push/encode, vote, decode, robust aggregators, tcgen05 GEMM)
+  ops/       launchers for the sm_90a kernels (push/encode, vote, decode, robust aggregators, wgmma GEMM)
   optim/     SGDModified / AdamModified (external-gradient optimizers)
   parallel/  arenas, symmetric memory, placement, PS / worker roles, fused (nvl) and collective (nccl/gloo) engines, Trainer
   data/      datasets + identical-batch plans

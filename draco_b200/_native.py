@@ -1,7 +1,7 @@
 """ctypes bindings for the in-tree native libraries (see ``draco_b200/build.py``).
 
 ``host()`` loads ``libdraco_host.so`` (pure C++, works everywhere).  ``cuda()`` loads ``libdraco_cuda.so`` (every
-sm_100a kernel + the symmetric-memory runtime); it raises loudly when CUDA is present but the library is missing,
+sm_90a kernel + the symmetric-memory runtime); it raises loudly when CUDA is present but the library is missing,
 because silently falling back to PyTorch ops on a GPU box would hide that the product path is not running.
 
 The ``Structure`` classes mirror, field for field, the argument structs in ``csrc/cuda/*.cu``.
@@ -174,7 +174,7 @@ def cuda_available() -> bool:
 
 
 def cuda() -> C.CDLL:
-    """The sm_100a kernel library.  Never falls back: a missing library on a GPU box is an error."""
+    """The sm_90a kernel library.  Never falls back: a missing library on a GPU box is an error."""
     global _cuda
     if _cuda is None:
         path = LIB_DIR / "libdraco_cuda.so"

@@ -1,10 +1,10 @@
 """In-tree native build: ``python -m draco_b200.build``.
 
-Two shared libraries are produced under ``draco_b200/_lib`` (git-ignored, shipped to GPU boxes by gpurun):
+Two shared libraries are produced under ``draco_b200/_lib`` (git-ignored build products):
 
 * ``libdraco_host.so``  -- pure C++17 (locator, codec, host aggregators); loads on CPU-only machines.
-* ``libdraco_cuda.so``  -- every CUDA kernel + the symmetric-memory runtime, compiled for sm_100a only
-  (``-gencode arch=compute_100a,code=sm_100a -lineinfo``).  nvcc cross-compiles without a GPU.
+* ``libdraco_cuda.so``  -- every CUDA kernel + the symmetric-memory runtime, compiled for sm_90a (H100) only
+  (``-gencode arch=compute_90a,code=sm_90a -lineinfo``).  nvcc cross-compiles without a GPU.
 
 Both expose a plain C ABI and are loaded with ctypes (``draco_b200._native``) -- no torch headers involved, so a
 full rebuild takes seconds and does not depend on the torch ABI.
@@ -24,7 +24,7 @@ CSRC = ROOT / "csrc"
 LIB_DIR = Path(__file__).resolve().parent / "_lib"
 OBJ_DIR = ROOT / "build" / "obj"
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 CXX_FLAGS = ["-O3", "-std=c++17", "-fPIC", "-Wall", "-pthread"]
 
@@ -84,7 +84,7 @@ def build_cuda(force: bool = False, verbose: bool = False, ptxas_info: bool = Fa
         with cf.ThreadPoolExecutor(max_workers=min(8, len(jobs))) as ex:
             list(ex.map(lambda c: _run(c, verbose or ptxas_info), jobs))
     if jobs or force or _newer(objs, out):
-        _run([nvcc, "-shared", "-o", str(out), *map(str, objs), "-gencode", "arch=compute_100a,code=sm_100a"], verbose)
+        _run([nvcc, "-shared", "-o", str(out), *map(str, objs), "-gencode", "arch=compute_90a,code=sm_90a"], verbose)
     return out
 
 

@@ -19,7 +19,7 @@ values are interpolated against the dict itself, :12-20).  What survives here:
                                requests + terminate (reference :128-257, :370-372, :905-926).  Needs boto3 (not in this image; the
                                logic is exercised in tests/test_misc_cpu.py against a stub client).
 
-One B200 node hosts the whole 1 PS + 7 workers job.  ``run`` starts ONE job: on the first node, or -- with ``--nnodes`` > 1 --
+One 8-GPU H100 node hosts the whole 1 PS + 7 workers job.  ``run`` starts ONE job: on the first node, or -- with ``--nnodes`` > 1 --
 spanning that many nodes through torchrun's rendezvous (the *collective* transports are used across nodes, peer memory is
 intra-node).  ``run --all-nodes`` starts an independent copy on every node (sweeps), each with its own log / train_dir suffix.
 """
@@ -63,7 +63,7 @@ DEFAULT_CFG = Cfg({
     "master_port": 29500,
     "state_file": ".cluster_state.json",
     # EC2 fields (Ec2Fleet)
-    "region": "us-west-2", "availability_zone": "us-west-2b", "instance_type": "p6-b200.48xlarge", "image_id": "", "key_name": "",
+    "region": "us-west-2", "availability_zone": "us-west-2b", "instance_type": "p5.48xlarge", "image_id": "", "key_name": "",
     "n_instances": 1, "spot_price": "", "security_group": [], "subnet_id": "", "efs_id": "", "nfs_dir": "%(remote_dir)s/output",
     "launch_timeout_s": 900, "poll_s": 5,
 })

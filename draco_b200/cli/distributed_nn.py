@@ -22,7 +22,7 @@ from ..config import add_fit_args, config_from_args
 
 
 def main(argv=None) -> int:
-    ap = add_fit_args(argparse.ArgumentParser(description="Draco on B200 (draco_b200)"))
+    ap = add_fit_args(argparse.ArgumentParser(description="Draco on H100 (draco_b200)"))
     ap.add_argument("--launch", type=int, default=0, help="spawn this many local processes with torchrun semantics")
     ap.add_argument("--master-port", type=int, default=29511)
     args = ap.parse_args(argv)

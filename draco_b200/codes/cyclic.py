@@ -166,8 +166,7 @@ def encode(code: CyclicCode, worker: int, grads_by_batch: np.ndarray) -> np.ndar
 
 def decode_ifft(code: CyclicCode, R: np.ndarray, f: Optional[np.ndarray] = None) -> np.ndarray:
     """Alternative decoder: estimate the error matrix and subtract it (the reference's earlier, now dead, decoder --
-    ``_obtain_E`` / ``_obtain_epsilon`` in src/master/cyclic_master.py:175-188 and the orphan Cython ``decoding`` module,
-    SURVEY N3).
+    ``_obtain_E`` / ``_obtain_epsilon`` in src/master/cyclic_master.py:175-188 and the orphan Cython ``decoding`` module).
 
     The syndrome ``C2^H R`` holds the last 2s DFT coefficients of every error column.  The locator polynomial (from the
     projected syndrome, as in :func:`decode`) gives a linear recurrence that extends them cyclically to all n

@@ -44,7 +44,7 @@ class JobConfig:
     checkpoint_step: int = 0
     # ---- additions --------------------------------------------------------------------------
     num_workers: int = 0            # logical workers P (0: world_size - 1, like `mpirun -n P+1`)
-    transport: str = "nvl"          # nvl: fused sm_100a kernels over peer memory | nccl: baseline | gloo: CPU
+    transport: str = "nvl"          # nvl: fused sm_90a kernels over peer memory | nccl: baseline | gloo: CPU
     dtype: str = "bf16"             # compute dtype on workers (bf16 | fp32)
     cuda_graphs: bool = True
     weight_decay: float = 0.0

@@ -7,7 +7,7 @@ ResNet18 62 / 11,173,962; ResNet34 110 / 21,282,122; ResNet50 161 / 23,520,842; 
 ResNet152 467 / 58,156,618.
 
 ``num_classes`` is an extension (the reference hard-codes 10); ``imagenet_stem=True`` swaps the 3x3 CIFAR stem for the
-7x7 / stride-2 convolution + 3x3 / stride-2 max-pool of the ImageNet ResNets and pools adaptively (BASELINE.json config 5:
+7x7 / stride-2 convolution + 3x3 / stride-2 max-pool of the ImageNet ResNets and pools adaptively (used for
 ResNet-50 on synthetic 224x224 ImageNet-shaped data).  The defaults reproduce the reference exactly.
 """
 from __future__ import annotations
@@ -26,7 +26,7 @@ from .split import make_split
 
 
 def _conv(cin: int, cout: int, k: int, stride: int = 1) -> nn.Conv2d:
-    # ops.conv.Conv2d is nn.Conv2d whose 1x1 / stride-1 case runs on the tcgen05 GEMM (bottleneck conv1 / conv3)
+    # ops.conv.Conv2d is nn.Conv2d whose 1x1 / stride-1 case runs on the wgmma GEMM (bottleneck conv1 / conv3)
     return Conv2d(cin, cout, kernel_size=k, stride=stride, padding=k // 2, bias=False)
 
 

@@ -6,7 +6,7 @@ remaining layers are still back-propagating (src/model_ops/resnet_split.py:431-6
 :760-860 ``backward_coded``, :739-758 ``backward_single``; lenet.py:114-218; fc_nn.py:94-199) -- with MPI
 calls, the adversary and the compressor living *inside the model*.
 
-The B200 design keeps the capability (gradients become visible to the transport in reverse layer order
+This design keeps the capability (gradients become visible to the transport in reverse layer order
 while backward is still running, so the push overlaps backprop) but not the layering violation: a
 ``SplitBackwardMixin`` model exposes the same three drivers, implemented with autograd's
 post-accumulate-grad hooks; what happens to a finished gradient is a callback supplied by the worker

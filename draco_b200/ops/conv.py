@@ -1,6 +1,6 @@
-"""Convolution layer served by this repository's sm_100a kernels (see ``Conv2d``): tcgen05 tap-table / halo-reuse implicit GEMM
-for 3x3 and 1x1 convolutions with stride 1 or 2 (fprop, dgrad, split-K wgrad; csrc/cuda/conv_tap_tcgen05.cu,
-conv_halo_tcgen05.cu), the tcgen05 GEMM for the remaining pointwise layers (csrc/cuda/gemm_tcgen05.cu) and CUDA-core kernels
+"""Convolution layer served by this repository's sm_90a kernels (see ``Conv2d``): wgmma tap-table / halo-reuse implicit GEMM
+for 3x3 and 1x1 convolutions with stride 1 or 2 (fprop, dgrad, split-K wgrad; csrc/cuda/conv_tap_wgmma.cu,
+conv_halo_wgmma.cu), the wgmma GEMM for the remaining pointwise layers (csrc/cuda/gemm_wgmma.cu) and CUDA-core kernels
 for the 3-channel stem (csrc/cuda/conv_stem.cu).  In NHWC a 1x1 convolution *is* a GEMM:
 ``y[N*H*W, Cout] = x[N*H*W, Cin] @ W[Cout, Cin]^T`` -- both operands K-major, no im2col, no layout change (weights live in the
 arena as ``[Cout, kH, kW, Cin]``).  The convolution epilogue can also produce the BatchNorm statistics of its output
@@ -176,7 +176,7 @@ def _bwd_args(link, mask: torch.Tensor, c: int, slots: int, device):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# tap-table implicit-GEMM kernels (csrc/cuda/conv_tap_tcgen05.cu): stride 1 or 2, 1x1 or 3x3, fprop / dgrad / split-K wgrad
+# tap-table implicit-GEMM kernels (csrc/cuda/conv_tap_wgmma.cu): stride 1 or 2, 1x1 or 3x3, fprop / dgrad / split-K wgrad
 # ---------------------------------------------------------------------------------------------------------------------
 def convg_tcgen05(act: torch.Tensor, weight: torch.Tensor, in_hw, stride: int, dgrad: bool = False,
                   bias: torch.Tensor = None, bn_stats: "BnStatRequest" = None, residual: torch.Tensor = None,
@@ -218,9 +218,9 @@ def convg_tcgen05(act: torch.Tensor, weight: torch.Tensor, in_hw, stride: int, d
     return out
 
 
-def convg_plan(n: int, h: int, w: int, cin: int, cout: int, ks: int, stride: int, dgrad: int, num_sms: int = 148):
+def convg_plan(n: int, h: int, w: int, cin: int, cout: int, ks: int, stride: int, dgrad: int, num_sms: int = 132):
     """[block_n, cm, cn, grid, mode] the tap-convolution launcher picks for this layer (mode 0 = one CTA per tile, 1 = multicast
-    cluster, 2 = CTA pair / cta_group::2); host-side planning only, no GPU needed."""
+    cluster); host-side planning only, no GPU needed.  ``num_sms`` defaults to an H100 SXM."""
     import ctypes as C
     out = (C.c_int * 5)()
     if _lib().drc_convg_plan(n, h, w, cin, cout, ks, stride, int(dgrad), num_sms, out) != 0:
@@ -248,7 +248,7 @@ def convg_wgrad_tcgen05(dy: torch.Tensor, x: torch.Tensor, ks: int, stride: int)
 
 
 def halo_supported(h: int, w: int, cin: int, cout: int) -> bool:
-    """Halo-reuse kernel (csrc/cuda/conv_halo_tcgen05.cu): 3x3 / stride 1, 64 -> 64 channels, H % 16 == 0, W % 8 == 0."""
+    """Halo-reuse kernel (csrc/cuda/conv_halo_wgmma.cu): 3x3 / stride 1, 64 -> 64 channels, H % 16 == 0, W % 8 == 0."""
     return os.environ.get("DRACO_CONV_HALO", "1") != "0" and bool(_lib().drc_conv_halo_supported(h, w, cin, cout))
 
 
@@ -317,7 +317,7 @@ def conv_stem_wgrad(dy: torch.Tensor, x: torch.Tensor) -> torch.Tensor:
 
 def conv3x3_halo_wgrad(dy: torch.Tensor, x: torch.Tensor) -> torch.Tensor:
     """Weight gradient [64, 64, 3, 3] (stored [Cout, 3, 3, Cin]) of the 64 -> 64 3x3 / stride-1 layers: all nine taps from one resident
-    halo patch per 128-pixel tile (csrc/cuda/conv_halo_tcgen05.cu: wgrad_halo_tcgen05_kernel)."""
+    halo per 128-pixel tile (csrc/cuda/conv_halo_wgmma.cu: wgrad_halo_wgmma_kernel)."""
     from .. import _native as N
     from . import kernels as K
     lib = _lib()
@@ -357,7 +357,7 @@ class _ConvStemFn(torch.autograd.Function):
 
 
 class _ConvGFn(torch.autograd.Function):
-    """3x3 / 1x1, stride 1 / 2 convolution on the tcgen05 kernels.  Returns (y, mean, invstd, x_fork); mean / invstd are the
+    """3x3 / 1x1, stride 1 / 2 convolution on the wgmma kernels.  Returns (y, mean, invstd, x_fork); mean / invstd are the
     fused BatchNorm statistics when ``bn_req`` is given (empty tensors otherwise) and carry no gradient.  ``x_fork`` (``fork=True``)
     is x again, for the OTHER consumer of x (the residual shortcut): its gradient comes back into this function and is added to dx
     inside the dgrad kernel's epilogue instead of by a separate elementwise kernel of autograd."""
@@ -370,8 +370,8 @@ class _ConvGFn(torch.autograd.Function):
         ctx.in_link = in_link if (in_link is not None and stride == 1 and weight.shape[1] <= 512
                                   and os.environ.get("DRACO_CONV_EPI", "tma") != "direct"
                                   and os.environ.get("DRACO_BN_BWD_FUSE", "0") == "1" and in_link.x.shape == x.shape) else None
-        # OPT-IN: measured on B200 (profiles/README.md, "what did not work") the fused epilogue costs 8-9 us per tile (row-offset
-        # integer divisions + exposed loads of y / x) against the 11 us reduce kernel it removes: the step gets 6 % slower
+        # OPT-IN: the fused epilogue adds row-offset integer divisions and exposed loads of y / x to every tile, against the one
+        # reduce kernel it removes; it is not the default
         ctx.stride, ctx.has_bias = stride, bias is not None
         ctx.set_materialize_grads(False)          # no zero-filled "gradients" for the statistics outputs
         h, w = x.shape[2], x.shape[3]
@@ -436,8 +436,8 @@ class _ConvGFn(torch.autograd.Function):
 class Conv2d(nn.Conv2d):
     """``nn.Conv2d`` (same parameters / state_dict) whose CUDA bf16 channels-last forms run on this repository's kernels:
 
-    * 3x3 and 1x1, stride 1 or 2, channel counts that are multiples of 64 -> tap-table / halo-reuse tcgen05 implicit GEMM;
-    * 1x1 / stride 1 with other channel counts (multiples of 8, >= 64) -> the tcgen05 GEMM on NHWC rows;
+    * 3x3 and 1x1, stride 1 or 2, channel counts that are multiples of 64 -> tap-table / halo-reuse wgmma implicit GEMM;
+    * 1x1 / stride 1 with other channel counts (multiples of 8, >= 64) -> the wgmma GEMM on NHWC rows;
     * the 3-channel 3x3 stem -> CUDA-core kernels of conv_stem.cu;
     * everything else (CPU, fp32, exotic geometry) -> ``nn.Conv2d`` (counted in ``backend_counters["cudnn"]``).
 
@@ -471,7 +471,7 @@ class Conv2d(nn.Conv2d):
 
     def forward(self, x: torch.Tensor, bn: nn.Module = None, fork: bool = False):
         """``fork=True`` returns ``(y, x_fork)``: ``x_fork`` is x for the second consumer of x (the shortcut branch of a residual
-        block); on the tcgen05 path the gradient that comes back through it is added inside this layer's dgrad epilogue."""
+        block); on the native path the gradient that comes back through it is added inside this layer's dgrad epilogue."""
         if fork:
             if self._tap_ok(x) and x.requires_grad and os.environ.get("DRACO_CONV_FORK", "1") != "0":
                 backend_counters["tcgen05"] += 1

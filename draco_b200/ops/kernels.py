@@ -1,4 +1,4 @@
-"""Python launchers for the sm_100a step-path kernels (thin: build the argument struct, launch on the current stream).
+"""Python launchers for the sm_90a step-path kernels (thin: build the argument struct, launch on the current stream).
 
 Every function takes either torch CUDA tensors or raw device addresses (``int``) -- peer-mapped and multicast pointers
 coming from the symmetric-memory runtime are plain integers.  Nothing here falls back to PyTorch ops: if the CUDA
@@ -308,11 +308,13 @@ def krum_select(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, s:
 # ------------------------------------------------------------------------------------------------ GEMM (K10)
 def gemm_bf16(A: torch.Tensor, B: torch.Tensor, *, a_mn: bool = False, b_mn: bool = False, out: Optional[torch.Tensor] = None,
               out_dtype: torch.dtype = torch.bfloat16, bias: Optional[torch.Tensor] = None, relu: bool = False,
-              accumulate: bool = False, block_n: int = 0, cta_pair: Optional[bool] = None) -> torch.Tensor:
-    """``C[M, N] = op(A) op(B)^T`` on tcgen05 tensor cores (``cta_pair``: force / forbid the cta_group::2 kernel; None = by size).
+              accumulate: bool = False, block_n: int = 0) -> torch.Tensor:
+    """``C[M, N] = op(A) op(B)^T`` on the wgmma tensor cores (csrc/cuda/gemm_wgmma.cu).
 
     K-major operands (default) are ``A[M, K]`` / ``B[N, K]``; with ``a_mn`` / ``b_mn`` the tensor passed is the
     transposed storage ``A[K, M]`` / ``B[K, N]`` (MN contiguous), so no transpose copy is ever needed.
+    ``block_n``: tile width, 0 = chosen by size, else 32 / 64 / 128.  256 is accepted and runs 128-wide tiles: one warpgroup's
+    registers hold at most a 128 x 128 fp32 accumulator, so results are those of ``block_n=128``.
     """
     assert A.dtype == torch.bfloat16 and B.dtype == torch.bfloat16 and A.is_cuda and B.is_cuda
     assert A.dim() == 2 and B.dim() == 2 and A.stride(1) == 1 and B.stride(1) == 1
@@ -324,37 +326,10 @@ def gemm_bf16(A: torch.Tensor, B: torch.Tensor, *, a_mn: bool = False, b_mn: boo
     assert out.shape == (M, Nn) and out.stride(1) == 1
     bias_f32 = bias.data_ptr() if bias is not None and bias.dtype == torch.float32 else None
     bias_b16 = bias.data_ptr() if bias is not None and bias.dtype == torch.bfloat16 else None
-    # large K-major problems go to the CTA-pair kernel (tcgen05.mma.cta_group::2): measured 1.04x cuBLAS at 4096^3, 0.95x at
-    # 16384 x 512 x 4608 vs 0.87x / 0.82x for the single-CTA kernel (profiles/gemm_bench_r2.json); small ones lose to it
-    pair = os.environ.get("DRACO_GEMM_2CTA", "auto") if cta_pair is None else ("1" if cta_pair else "0")
-    if (not a_mn and not b_mn and block_n in (0, 128, 256) and M >= 256 and Nn >= 128
-            and (pair == "1" or (pair == "auto" and M >= 2048 and Nn >= 512 and K >= 1024))):
-        return gemm2_bf16(A, B, out=out, bias=bias, relu=relu, accumulate=accumulate, block_n=block_n)
     code = N.cuda().drc_gemm_bf16(A.data_ptr(), A.stride(0), int(a_mn), B.data_ptr(), B.stride(0), int(b_mn), out.data_ptr(),
                                   out.stride(0), int(out.dtype == torch.float32), M, Nn, K, bias_f32, bias_b16, int(relu),
                                   int(accumulate), block_n, sm_count(A.device), A.device.index, _stream())
     N.check(code, "gemm_bf16")
-    return out
-
-
-def gemm2_bf16(A: torch.Tensor, B: torch.Tensor, *, out: Optional[torch.Tensor] = None, out_dtype: torch.dtype = torch.bfloat16,
-               bias: Optional[torch.Tensor] = None, relu: bool = False, accumulate: bool = False, block_n: int = 0) -> torch.Tensor:
-    """``C[M, N] = A[M, K] B[N, K]^T`` on CTA PAIRS (tcgen05.mma.cta_group::2, 256 x block_n tiles, csrc/cuda/gemm2_tcgen05.cu)."""
-    assert A.dtype == torch.bfloat16 and B.dtype == torch.bfloat16 and A.is_cuda and A.dim() == 2 and B.dim() == 2
-    assert A.stride(1) == 1 and B.stride(1) == 1 and A.shape[1] == B.shape[1]
-    M, Kd, Nn = A.shape[0], A.shape[1], B.shape[0]
-    if out is None:
-        out = torch.empty(M, Nn, dtype=out_dtype, device=A.device)
-    lib = N.cuda()
-    if not getattr(lib, "_gemm2_ready", False):
-        lib.drc_gemm2_bf16.argtypes = [N.ptr, N.i64, N.ptr, N.i64, N.ptr, N.i64] + [C.c_int] * 4 + [N.ptr, N.ptr] + [C.c_int] * 5 + [N.ptr]
-        lib.drc_gemm2_bf16.restype = C.c_int
-        lib._gemm2_ready = True
-    bias_f32 = bias.data_ptr() if bias is not None and bias.dtype == torch.float32 else None
-    bias_b16 = bias.data_ptr() if bias is not None and bias.dtype == torch.bfloat16 else None
-    N.check(lib.drc_gemm2_bf16(A.data_ptr(), A.stride(0), B.data_ptr(), B.stride(0), out.data_ptr(), out.stride(0),
-                               int(out.dtype == torch.float32), M, Nn, Kd, bias_f32, bias_b16, int(relu), int(accumulate), block_n,
-                               sm_count(A.device), A.device.index, _stream()), "gemm2_bf16")
     return out
 
 

@@ -1,7 +1,7 @@
-"""Linear layer backed by the hand-written tcgen05 GEMM (``csrc/cuda/gemm_tcgen05.cu``).
+"""Linear layer backed by the hand-written wgmma GEMM (``csrc/cuda/gemm_wgmma.cu``).
 
 All three products of a linear layer run on the same kernel without transpose copies, by describing operands to TMA
-/ UMMA as K-major or MN-major:
+/ wgmma as K-major or MN-major:
 
     y  = x  W^T   A = x  (K-major)   B = W  (K-major)     + fused bias (+ReLU) epilogue
     dx = dy W     A = dy (K-major)   B = W  (MN-major)
@@ -81,7 +81,7 @@ class _LinearFn(torch.autograd.Function):
 
 
 class Linear(nn.Module):
-    """Drop-in ``nn.Linear`` (same parameter names / init) whose CUDA bf16 path is the tcgen05 GEMM."""
+    """Drop-in ``nn.Linear`` (same parameter names / init) whose CUDA bf16 path is the wgmma GEMM."""
 
     def __init__(self, in_features: int, out_features: int, bias: bool = True) -> None:
         super().__init__()

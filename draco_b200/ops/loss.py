@@ -1,4 +1,4 @@
-"""Classifier-head loss: softmax cross-entropy + Prec@1 / Prec@5, optionally as ONE sm_100a kernel.
+"""Classifier-head loss: softmax cross-entropy + Prec@1 / Prec@5, optionally as ONE sm_90a kernel.
 
 ``cross_entropy_with_metrics(logits, labels, metrics, scale)`` returns the mean loss (differentiable w.r.t. ``logits``) and
 adds ``scale * (loss, prec1 %, prec5 %)`` to the 3-element ``metrics`` tensor.  Default path: the PyTorch ops the reference

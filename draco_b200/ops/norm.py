@@ -1,4 +1,4 @@
-"""BatchNorm2d with fused residual-add + ReLU on the sm_100a kernels of ``csrc/cuda/bn_fused.cu``.
+"""BatchNorm2d with fused residual-add + ReLU on the sm_90a kernels of ``csrc/cuda/bn_fused.cu``.
 
 ``FusedBatchNorm2d`` *is* an ``nn.BatchNorm2d`` (same parameters, buffers and state_dict keys as the reference's models,
 src/model_ops/resnet.py:19-24) whose ``forward(x, residual=None, relu=False)`` computes
@@ -46,8 +46,7 @@ def _lib():
 UPDATE_RUNNING_STATS = True
 
 
-# ``num_batches_tracked += 1`` is a kernel launch per BatchNorm layer per forward (20 launches, 35 us of a 2.0 ms ResNet-18
-# step, profiles/worker_profile_ResNet18_fused.txt).  Inside ``deferred_batch_counts()`` the fused path only remembers the
+# ``num_batches_tracked += 1`` is a kernel launch per BatchNorm layer per forward (20 launches per ResNet-18 step).  Inside ``deferred_batch_counts()`` the fused path only remembers the
 # counters and the context exit bumps all of them with ONE multi-tensor kernel.
 _defer_counts = False
 _pending_counts: list = []
@@ -116,8 +115,8 @@ class _BnActFn(torch.autograd.Function):
                                M, c, float(eps), float(momentum), int(relu), _sms(dev), int(have_stats),
                                torch.cuda.current_stream().cuda_stream), "bn_fwd")
         # ReLU mask in backward: the saved output y.  DRACO_BN_MASK=x recomputes it from x with the forward's own arithmetic for
-        # layers without a residual input (one saved activation less per layer: memory for large models); measured A/B in one
-        # process it is ~1.5 % slower on the ResNet-18/CIFAR step (the activations are L2-resident there), so it is opt-in.
+        # layers without a residual input (one saved activation less per layer: memory for large models); it adds arithmetic to
+        # every backward and the ResNet-18/CIFAR activations are small, so it is opt-in.
         mask_from_x = residual is None and os.environ.get("DRACO_BN_MASK", "y") == "x"
         ctx.save_for_backward(x, y if (relu and not mask_from_x) else None, gamma, beta, mean, invstd)
         ctx.relu, ctx.has_res = bool(relu), residual is not None

@@ -1,7 +1,7 @@
 """Library-collective transports: ``--transport nccl`` (the measured baseline) and ``--transport gloo`` (CPU plumbing).
 
 This engine keeps the *structure* of the reference's step on purpose, so that it can serve as the reference-faithful
-baseline BASELINE.md asks for -- the unmodified reference cannot run here (Python 2.7 / torch 0.3 / mpi4py):
+baseline -- the unmodified reference cannot run here (Python 2.7 / torch 0.3 / mpi4py):
 
 * one broadcast per parameter tensor per step        (reference: ``comm.Bcast`` per layer, baseline_master.py:180-186)
 * one message per (worker, parameter tensor) upward  (reference: ``isend`` tag 88+layer, baseline_worker.py:258-273)

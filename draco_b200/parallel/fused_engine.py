@@ -1,4 +1,4 @@
-"""The product transport (``--transport nvl``): every byte of a training step moves through sm_100a kernels.
+"""The product transport (``--transport nvl``): every byte of a training step moves through sm_90a kernels.
 
 Step anatomy (one PS + P logical workers hosted by ``nprocs`` GPU processes; see placement.py):
 
@@ -20,7 +20,7 @@ workers that share a GPU run on concurrent streams inside that graph (``--worker
 streams overlapped with the rest of the backward pass, and the PS consumes buckets as they complete (pipelined PS).
 
 Reference counterparts: master loops src/master/{baseline,rep,cyclic}_master.py ``start()``; worker loops
-src/worker/*_worker.py ``train()``; all mpi4py traffic listed in SURVEY.md section 2.3 "Collective / message call sites".
+src/worker/*_worker.py ``train()``; all of their mpi4py traffic.
 """
 from __future__ import annotations
 
@@ -184,7 +184,7 @@ class FusedEngine:
                          if self.debug_checksum and self.local_workers else None)
         self._initial_broadcast()
 
-    # ------------------------------------------------------------------ transport self-check (SURVEY 5.2)
+    # ------------------------------------------------------------------ transport self-check
     def _dbg_loopback(self, w: int, g32, g16, push_kw) -> None:
         """Re-run the worker's encode + adversary into a LOCAL buffer and keep its 64-bit checksum (sum of the 32-bit
         words): what the PS must find in slot ``w`` if every peer store of the real push landed."""
@@ -272,7 +272,7 @@ class FusedEngine:
                 order.sort(key=lambda r: self.schedule.is_adversary(r, step_host))
             if self.worker_streams:
                 # Logical workers sharing this GPU are issued round-robin on concurrent streams: the late layers of a
-                # CIFAR ResNet launch 16-128 CTAs on 148 SMs, so kernels of different workers fill each other's gaps.
+                # CIFAR ResNet launch 16-128 CTAs on 132 SMs, so kernels of different workers fill each other's gaps.
                 # Every worker's kernel sequence is unchanged => its gradient stays bit-identical to the serial run.
                 from ..ops import norm as _norm
                 main = torch.cuda.current_stream()

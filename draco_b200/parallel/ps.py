@@ -3,7 +3,7 @@
 Two implementations of the same semantics (reference: ``SyncReplicasMaster_NN`` / ``CodedMaster`` / ``CyclicMaster`` in
 src/master/*.py):
 
-* ``FusedPS``  -- the product path.  Decode + SGD + parameter broadcast are sm_100a kernels working on the flat
+* ``FusedPS``  -- the product path.  Decode + SGD + parameter broadcast are sm_90a kernels working on the flat
   ``grad_in`` slab that workers filled through peer stores (ops/kernels.py); nothing returns to the host.
 * ``TorchPS``  -- reference-faithful structure: per-tensor decode with library ops, a separate optimizer step, used by
   the NCCL baseline transport and the CPU/Gloo transport (where the small dense solves go through the C++ host

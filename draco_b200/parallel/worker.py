@@ -62,7 +62,7 @@ def make_model(cfg: JobConfig) -> torch.nn.Module:
     if cfg.num_classes != 10 and (cfg.network.startswith("ResNet") or cfg.network.startswith("VGG")):
         kwargs["num_classes"] = cfg.num_classes
     if cfg.dataset == "ImageNet" and cfg.network.startswith("ResNet"):
-        # BASELINE.json config 5: ImageNet-shaped ResNets (7x7 / stride-2 stem + max-pool, 224 x 224 inputs, 1000 classes)
+        # ImageNet-shaped ResNets (7x7 / stride-2 stem + max-pool, 224 x 224 inputs, 1000 classes)
         kwargs.update(num_classes=1000, imagenet_stem=True)
     return build_model(cfg.network, **kwargs)
 
@@ -197,7 +197,7 @@ class WorkerCompute:
         if self.device.type == "cuda":
             # The PCIe transfer runs on a COPY STREAM into device staging buffers while the compute stream still executes the
             # step that was enqueued before this call; the compute stream then only does a device-to-device copy (a few us)
-            # into the buffers the captured step reads.  In-stream H2D copies cost ~40 us of idle GPU per step.
+            # into the buffers the captured step reads.  In-stream H2D copies would leave the GPU idle for the transfer.
             main = torch.cuda.current_stream(self.device)
             if getattr(self, "_copy_stream", None) is None:
                 self._copy_stream = torch.cuda.Stream(device=self.device)

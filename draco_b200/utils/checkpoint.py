@@ -1,6 +1,6 @@
 """Checkpoint / resume.
 
-Reference behaviour (SURVEY 5.4): the PS pickles the whole module to ``train_dir + "model_step_" + step`` every
+Reference behaviour: the PS pickles the whole module to ``train_dir + "model_step_" + step`` every
 ``eval_freq`` steps (src/master/baseline_master.py:237-243), worker 1 saves a state_dict for ResNets
 (src/worker/baseline_worker.py:298-302), and resume exists only for the baseline approach from a hard-coded path without
 optimizer state (baseline_master.py:54-57).

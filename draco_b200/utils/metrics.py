@@ -19,9 +19,9 @@ import torch
 
 def wait_event(event) -> None:
     """Host wait for a CUDA event created with ``blocking=True`` (cudaEventBlockingSync): the thread sleeps instead of
-    spinning.  Measured on the B200 boxes (`tools/diag_e2e.py`): a host that burns CPU while the GPU works -- a spinning
-    sync plus idle OpenMP workers spinning after every `index_select` of the input staging -- runs into the container's
-    CPU quota and is descheduled for ~50 ms every ~100 ms, which idles the GPU in any loop that reads results per step."""
+    spinning.  A host that burns CPU while the GPU works -- a spinning sync plus idle OpenMP workers spinning after every
+    `index_select` of the input staging -- can run into a container's CPU quota and be descheduled for tens of milliseconds,
+    which idles the GPU in any loop that reads results per step (`tools/diag_e2e.py` shows the effect)."""
     event.synchronize()
 
 

@@ -1,4 +1,4 @@
-"""Coding-theory layer + oracles (CPU, fp64).  SURVEY section 4 blueprint item 1."""
+"""Coding-theory layer + oracles (CPU, fp64)."""
 import itertools
 
 import numpy as np

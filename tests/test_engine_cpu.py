@@ -1,4 +1,4 @@
-"""CPU runtime tests: single-process collective engine for every approach, multi-process Gloo job (BASELINE config #1),
+"""CPU runtime tests: single-process collective engine for every approach, multi-process Gloo job (LeNet/MNIST),
 checkpoint / resume / evaluator, CLI flag surface."""
 import argparse
 import os
@@ -163,7 +163,7 @@ def test_compressed_wire_roundtrip_single_proc():
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# multi-process Gloo: BASELINE.json config #1 -- LeNet/MNIST, repetition r=1, 1 PS + 2 workers, no adversary
+# multi-process Gloo: LeNet/MNIST, repetition r=1, 1 PS + 2 workers, no adversary
 # ---------------------------------------------------------------------------------------------------------------
 def _free_port():
     s = socket.socket()

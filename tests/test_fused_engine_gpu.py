@@ -39,8 +39,11 @@ def test_fused_vote_tolerates_adversaries_bitwise():
     assert not torch.allclose(clean.engine.master_params(), mean.engine.master_params(), atol=1e-3)
 
 
-def test_fused_matches_library_op_engine():
-    """Same job through the kernels and through the torch-op PS (nccl transport on one process = no collectives)."""
+def test_fused_matches_library_op_engine(monkeypatch):
+    """Same job through the kernels and through the torch-op PS (nccl transport on one process = no collectives).  The fp32
+    model runs in true fp32: TF32 convolutions would round the two runs' worker gradients differently."""
+    monkeypatch.setattr(torch.backends.cudnn, "allow_tf32", False)
+    monkeypatch.setattr(torch.backends.cuda.matmul, "allow_tf32", False)
     for kw in (dict(approach="maj_vote", mode="maj_vote", group_size=3, worker_fail=1, err_mode="rev_grad"),
                dict(approach="baseline", mode="normal", worker_fail=0, err_mode="none"),
                dict(approach="baseline", mode="krum", worker_fail=2, err_mode="constant"),
@@ -246,7 +249,7 @@ def test_multigpu_job_trains_under_attack():
 
 
 def test_resnet50_bottlenecks_train_on_the_fused_path():
-    """ResNet-50 (BASELINE config 5 model): pointwise convs on the tcgen05 GEMM, fused BN, r=5 vote, graph replay."""
+    """ResNet-50 (ImageNet-shaped model): pointwise convs on the wgmma GEMM, fused BN, r=5 vote, graph replay."""
     from draco_b200.ops.conv import backend_counters as conv_c
     from draco_b200.ops.norm import backend_counters as bn_c
     c0, b0 = conv_c["tcgen05"], bn_c["fused"]
@@ -263,7 +266,7 @@ def test_resnet50_bottlenecks_train_on_the_fused_path():
                                 dict(approach="cyclic", worker_fail=1, err_mode="constant"),
                                 dict(approach="baseline", mode="geometric_median", worker_fail=2, err_mode="rev_grad")])
 def test_debug_checksum_verifies_every_pushed_gradient(kw):
-    """--debug-checksum (SURVEY 5.2): loopback re-encode on the worker vs the words that landed in the PS slot."""
+    """--debug-checksum: loopback re-encode on the worker vs the words that landed in the PS slot."""
     t, losses = _run(_cfg(debug_checksum=True, **kw), 4)
     log = t.engine.checksum_log
     assert [r["step"] for r in log] == [1, 2, 3, 4]

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM (csrc/cuda/gemm_tcgen05.cu) and the Linear layer built on it, against fp32 PyTorch references."""
+"""wgmma GEMM (csrc/cuda/gemm_wgmma.cu) and the Linear layer built on it, against fp32 PyTorch references."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -98,28 +98,6 @@ def test_linear_layer_forward_backward(batch, fin, fout):
     assert _rel_err(lin.bias.grad, b32.grad) < 2e-2
 
 
-@pytest.mark.timeout(300)
-@pytest.mark.parametrize("M,N,Kd,bn", [(256, 256, 64, 256), (512, 256, 512, 128), (1024, 768, 1024, 0), (4096, 512, 4608, 256),
-                                        (300, 264, 200, 128), (8192, 256, 2304, 0), (257, 130, 72, 0)])
-def test_gemm_cta_pair_kernel(K, M, N, Kd, bn):
-    """tcgen05.mma.cta_group::2: two CTAs of a cluster share one 256 x BLOCK_N MMA (csrc/cuda/gemm2_tcgen05.cu); ragged M / N / K,
-    bias + ReLU epilogue, fp32 output and accumulate mode, vs fp32 torch."""
-    dev = torch.device("cuda", 0)
-    torch.manual_seed(M + N + Kd)
-    A = torch.randn(M, Kd, device=dev).to(torch.bfloat16)
-    B = torch.randn(N, Kd, device=dev).to(torch.bfloat16)
-    bias = torch.randn(N, device=dev)
-    ref = A.float() @ B.float().t()
-    c = K.gemm2_bf16(A, B, block_n=bn)
-    assert _rel_err(c, ref) < 1e-2, _rel_err(c, ref)
-    c2 = K.gemm2_bf16(A, B, out_dtype=torch.float32, bias=bias, relu=True, block_n=bn)
-    assert _rel_err(c2, torch.relu(ref + bias)) < 1e-2
-    acc = torch.ones(M, N, device=dev, dtype=torch.float32)
-    K.gemm2_bf16(A, B, out=acc, accumulate=True, block_n=bn)
-    assert _rel_err(acc, ref + 1.0) < 1e-2
-    assert torch.equal(K.gemm2_bf16(A, B, block_n=bn), c)
-
-
 @pytest.mark.parametrize("n,cin,cout,hw", [(32, 64, 256, 16), (16, 256, 64, 8), (8, 512, 2048, 4), (128, 64, 64, 32)])
 def test_pointwise_conv_on_tcgen05(n, cin, cout, hw):
     from draco_b200.ops.conv import Conv2d, backend_counters
@@ -176,7 +154,7 @@ TAP_SHAPES = [(128, 64, 128, 32, 3, 2), (128, 128, 256, 16, 3, 2), (128, 256, 51
 @pytest.mark.parametrize("epi", ["tma", "direct"])
 @pytest.mark.parametrize("n,cin,cout,hw,ks,stride", TAP_SHAPES)
 def test_convg_tap_table_kernels(n, cin, cout, hw, ks, stride, epi, monkeypatch):
-    """Tap-table tcgen05 implicit GEMM (csrc/cuda/conv_tap_tcgen05.cu): fprop / dgrad / split-K wgrad for 3x3 and 1x1, stride 1 and
+    """Tap-table wgmma implicit GEMM (csrc/cuda/conv_tap_wgmma.cu): fprop / dgrad / split-K wgrad for 3x3 and 1x1, stride 1 and
     2, with the staged TMA-store epilogue and with the direct-store epilogue, against fp32 references."""
     from draco_b200.ops.conv import convg_tcgen05, convg_wgrad_tcgen05
     monkeypatch.setenv("DRACO_CONV_EPI", epi)
@@ -235,12 +213,12 @@ def test_conv_dgrad_epilogue_adds_fork_gradient(n, cin, cout, hw, ks, stride):
 
 
 @pytest.mark.timeout(300)
-@pytest.mark.parametrize("cfg", ["pair", "2,1,128", "1,2,128", "2,2,128", "4,2,128", "2,4,64", "8,1,64", "1,8,64", "4,1,128", "1,4,64"])
+@pytest.mark.parametrize("cfg", ["2,1,128", "1,2,128", "2,2,128", "4,2,128", "2,4,64", "8,1,64", "1,8,64", "4,1,128", "1,4,64",
+                                 "2,1,64", "1,2,64", "2,2,64", "4,2,64"])
 @pytest.mark.parametrize("n,cin,cout,hw,ks,stride", [(128, 256, 256, 8, 3, 1), (128, 512, 512, 4, 3, 1), (128, 128, 256, 16, 3, 2),
                                                      (24, 64, 512, 14, 1, 1)])
 def test_convg_cluster_multicast_shapes(n, cin, cout, hw, ks, stride, cfg, monkeypatch):
-    """Cluster variants of the tap convolution.  "pair": two CTAs execute one tcgen05.mma.cta_group::2 of M = 256 (each stages its
-    own activation tile and half of the weight tile).  "cm,cn,bn": every CTA loads 1/cn of the activation tile and 1/cm of the
+    """Cluster variants of the tap convolution.  "cm,cn,bn": every CTA loads 1/cn of the activation tile and 1/cm of the
     weight tile and TMA-multicasts them to its cluster row / column.  Each forced shape must reproduce the one-CTA-per-tile kernel
     (same k order per output element) for fprop (with fused BatchNorm statistics), dense dgrad and the one-launch stride-2 dgrad."""
     from draco_b200.ops.conv import BnStatRequest, convg_plan, convg_tcgen05
@@ -258,8 +236,6 @@ def test_convg_cluster_multicast_shapes(n, cin, cout, hw, ks, stride, cfg, monke
     monkeypatch.setenv("DRACO_CONV_CLUSTER", cfg)
     def forced(dgrad):
         plan = convg_plan(n, hw, hw, cin, cout, ks, stride, dgrad)
-        if cfg == "pair":
-            return plan[4] == 2
         cm, cn, bn = (int(v) for v in cfg.split(","))
         return plan[:3] == [bn, cm, cn] and plan[4] == 1
 
@@ -305,8 +281,8 @@ def test_conv_epilogue_batchnorm_statistics(n, cin, cout, hw, ks, stride):
 @pytest.mark.timeout(300)
 @pytest.mark.parametrize("n,hw", [(4, 32), (128, 32), (3, 16), (16, 64)])
 def test_conv3x3_halo_reuse_kernels(n, hw):
-    """Halo patch loaded once per tile, nine taps through row-shifted UMMA descriptors (64 -> 64 channels), resident weights, staged
-    TMA-store epilogue with fused BatchNorm statistics (csrc/cuda/conv_halo_tcgen05.cu)."""
+    """Halo loaded once per tile as three column-shifted boxes, tap (r, s) = box s from row r on (64 -> 64 channels), resident weights, staged
+    TMA-store epilogue with fused BatchNorm statistics (csrc/cuda/conv_halo_wgmma.cu)."""
     from draco_b200.ops.conv import BnStatRequest, conv3x3_halo
     dev = torch.device("cuda", 0)
     torch.manual_seed(n + hw)
@@ -418,7 +394,7 @@ def test_batchnorm_backward_reduction_inside_the_dgrad_epilogue(planes, hw, n, m
     """Two stacked BasicBlocks: the BatchNorm backward reductions (sum dz, sum dz * xhat) of the layers whose output feeds a
     stride-1 convolution can ride on that convolution's dgrad epilogue (DRACO_BN_BWD_FUSE=1; halo and tap kernels, with the
     residual-fork gradient added first), so those BatchNorms only run their apply kernel.  Same result as the standalone reduce
-    kernels up to summation order; deterministic; the counter proves the fused path ran.  (Opt-in: measured slower.)"""
+    kernels up to summation order; deterministic; the counter proves the fused path ran.  (Opt-in.)"""
     from draco_b200.models.resnet import BasicBlock
     from draco_b200.ops import norm
     dev = torch.device("cuda", 0)

@@ -1,4 +1,4 @@
-"""sm_100a kernel numerics against plain PyTorch fp32 / numpy fp64 references ("loopback ranks": every peer buffer is a
+"""sm_90a kernel numerics against plain PyTorch fp32 / numpy fp64 references ("loopback ranks": every peer buffer is a
 distinct buffer on the same device, so push / decode+update / broadcast semantics are checked without NVSwitch)."""
 import numpy as np
 import pytest

@@ -1,4 +1,4 @@
-"""Model zoo parity (tensor counts / parameter counts from SURVEY 2.2), split drivers, arenas."""
+"""Model zoo parity (tensor counts / parameter counts of the reference models), split drivers, arenas."""
 import numpy as np
 import pytest
 import torch

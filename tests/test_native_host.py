@@ -138,7 +138,7 @@ def test_native_loader_thread_pool_overlapping_jobs():
 # ------------------------------------------------------------------------------------------------ tap-table convolution algebra
 @pytest.mark.parametrize("ks,stride", [(3, 1), (3, 2), (1, 2), (1, 1)])
 def test_conv_tap_tables_reproduce_fprop_and_parity_class_dgrad(ks, stride):
-    """The host-side tables that drive the tap-table tcgen05 convolutions (csrc/cuda/conv_tap_tcgen05.cu), checked by
+    """The host-side tables that drive the tap-table wgmma convolutions (csrc/cuda/conv_tap_wgmma.cu), checked by
     emulating the kernel's loads on the CPU: input pixel = patch origin * in_mul + tap offset (out-of-range reads as zero, as
     the TMA unit fills), one weight column block per tap; strided dgrad assembled from its parity classes."""
     import torch
@@ -200,8 +200,9 @@ def test_conv_tap_tables_reproduce_fprop_and_parity_class_dgrad(ks, stride):
 
 
 def test_tap_convolution_launch_plans(monkeypatch):
-    """Host-side planning of the tap convolution (drc_convg_plan): one CTA per tile by default (the multicast-cluster and CTA-pair
-    variants measured slower on B200), the forced shapes honour divisibility, grids are whole clusters within the SM count."""
+    """Host-side planning of the tap convolution (drc_convg_plan): one CTA per tile by default (the multicast-cluster variant is
+    opt-in), a forced shape needs two real tiles along each dimension it multicasts over, grids are whole clusters within the SM
+    count (132 on an H100 SXM)."""
     if not N.cuda_available():
         pytest.skip("libdraco_cuda.so not built")
     from draco_b200.ops.conv import convg_plan
@@ -211,11 +212,8 @@ def test_tap_convolution_launch_plans(monkeypatch):
     for (n, h, w, cin, cout, ks, st) in layers:
         for dgrad in (0, 1):
             bn, cm, cn, grid, mode = convg_plan(n, h, w, cin, cout, ks, st, dgrad)
-            assert (cm, cn, mode) == (1, 1, 0) and 0 < grid <= 148
+            assert (cm, cn, mode) == (1, 1, 0) and 0 < grid <= 132
             assert bn == (128 if (cin if dgrad else cout) >= 128 else 64)
-    monkeypatch.setenv("DRACO_CONV_CLUSTER", "pair")
-    bn, cm, cn, grid, mode = convg_plan(128, 8, 8, 256, 256, 3, 1, 0)
-    assert (bn, cm, cn, mode) == (128, 2, 1, 2) and grid % 2 == 0 and grid <= 148
     monkeypatch.setenv("DRACO_CONV_CLUSTER", "2,2,128")
     bn, cm, cn, grid, mode = convg_plan(128, 8, 8, 256, 256, 3, 1, 1)
     assert (bn, cm, cn, mode) == (128, 2, 2, 1) and grid % 4 == 0

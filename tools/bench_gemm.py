@@ -1,4 +1,4 @@
-"""tcgen05 GEMM throughput vs cuBLAS (torch.matmul), CUDA-event timed, L2 flushed between iterations.
+"""wgmma GEMM (csrc/cuda/gemm_wgmma.cu) throughput vs cuBLAS (torch.matmul), CUDA-event timed, L2 flushed between iterations.
     python tools/bench_gemm.py [--json gpurun_out/gemm_bench.json]
 """
 import argparse
@@ -42,20 +42,13 @@ def main():
         B = torch.randn(N, Kd, device=dev).to(torch.bfloat16)
         out = torch.empty(M, N, dtype=torch.bfloat16, device=dev)
         t_ours = timeit(lambda: K.gemm_bf16(A, B, out=out), flush)
-        t_128 = timeit(lambda: K.gemm_bf16(A, B, out=out, block_n=128, cta_pair=False), flush) if N >= 128 else None
-        t_256 = timeit(lambda: K.gemm_bf16(A, B, out=out, block_n=256, cta_pair=False), flush) if N >= 256 else None
-        t_2cta = None
-        if M >= 256 and N >= 128 and os.environ.get("BENCH_2CTA", "1") == "1":
-            try:
-                t_2cta = timeit(lambda: K.gemm2_bf16(A, B, out=out), flush)
-            except Exception as e:  # noqa: BLE001
-                print("2-CTA kernel failed:", e, flush=True)
+        t_64 = timeit(lambda: K.gemm_bf16(A, B, out=out, block_n=64), flush) if N >= 64 else None
+        t_128 = timeit(lambda: K.gemm_bf16(A, B, out=out, block_n=128), flush) if N >= 128 else None
         t_cublas = timeit(lambda: torch.matmul(A, B.t(), out=out), flush)
         fl = 2.0 * M * N * Kd
         rows.append({"M": M, "N": N, "K": Kd, "ours_ms": t_ours, "cublas_ms": t_cublas, "ours_tflops": fl / t_ours / 1e9,
                      "cublas_tflops": fl / t_cublas / 1e9, "ratio": t_cublas / t_ours,
-                     "bn128_tflops": fl / t_128 / 1e9 if t_128 else None, "bn256_tflops": fl / t_256 / 1e9 if t_256 else None,
-                     "cta_pair_tflops": fl / t_2cta / 1e9 if t_2cta else None, "cta_pair_ratio": t_cublas / t_2cta if t_2cta else None})
+                     "bn64_tflops": fl / t_64 / 1e9 if t_64 else None, "bn128_tflops": fl / t_128 / 1e9 if t_128 else None})
         print(rows[-1], flush=True)
     if a.json:
         with open(a.json, "w") as fh:

@@ -1,4 +1,4 @@
-"""NVLink roofline sweep of the fused communication paths (BASELINE.json config 5: "encode/decode GB/s sweep vs NVLink roofline").
+"""NVLink roofline sweep of the fused communication paths (encode / decode GB/s vs the NVLink roofline).
 
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 --master-port 29510 tools/bench_push.py
 
@@ -34,7 +34,7 @@ from draco_b200.parallel.placement import Placement  # noqa: E402
 from draco_b200.parallel.symm import SymmContext  # noqa: E402
 from draco_b200.parallel.trainer import init_distributed  # noqa: E402
 
-LINK_GBS = 770.0          # measured peer copy per direction (B200_PROFILING.md); nominal 900
+LINK_GBS = 450.0          # H100 SXM NVLink 4, data-sheet rate per direction (900 GB/s bidirectional); not a measured rate
 FLAG_BYTES = 1 << 16
 REPS = int(os.environ.get("PUSH_REPS", "10"))
 

@@ -1,7 +1,7 @@
 #!/bin/bash
 # Round-end benchmark sweep:  gpurun --gpus N -- bash tools/final_sweep.sh N [headline|extra|all] [steps]
 #   headline : ResNet-18 / r=3 vote / 3 sign-flip adversaries, fused path and the NCCL reference-faithful baseline
-#   extra    : the other BASELINE.json configs (VGG-11 cyclic, ResNet-18 geometric median / krum, ResNet-50 r=5) on the fused path
+#   extra    : the other configurations (VGG-11 cyclic, ResNet-18 geometric median / krum, ResNet-50 r=5) on the fused path
 # Every run writes its JSON line to gpurun_out/sweep/<name>_N<N>.log; copy the ones to be judged into profiles/bench/.
 cd "${GRAFT_REPO_ROOT:-$(dirname "$0")/..}"
 N=${1:-1}; WHAT=${2:-all}; STEPS=${3:-60}

@@ -21,7 +21,7 @@ for s in "$@"; do
     tests_quick) timeout -k 10 900 python -m pytest tests/test_fused_engine_gpu.py -q -m multigpu -p no:cacheprovider -k "peer_memory_matches or nvls" > $OUT/t_multigpu_quick.log 2>&1; echo "tests_quick rc=$?" ;;
     nvlink)     timeout -k 10 600 python tools/prof_nvlink.py > $OUT/nvlink_timing.log 2>&1; echo "nvlink timing rc=$?"
                 timeout -k 10 900 ncu --clock-control none --metrics gpu__time_duration.sum,nvltx__bytes.sum,nvlrx__bytes.sum,dram__bytes_read.sum,dram__bytes_write.sum,lts__t_bytes.sum -k regex:"push_encode|aggregate_update" -s 12 -c 6 --csv --log-file $OUT/nvlink_counters.csv python tools/prof_nvlink.py > $OUT/nvlink_ncu.log 2>&1; echo "nvlink ncu rc=$?" ;;
-    sweep148)   PUSH_CTAS=148 timeout -k 10 900 $TR --master-port 29620 tools/bench_push.py > $OUT/push_sweep_148cta.log 2> $OUT/push_sweep_148cta.err; echo "sweep148 rc=$?" ;;
+    sweep132)   PUSH_CTAS=132 timeout -k 10 900 $TR --master-port 29620 tools/bench_push.py > $OUT/push_sweep_132cta.log 2> $OUT/push_sweep_132cta.err; echo "sweep132 rc=$?" ;;
     test_equiv) timeout -k 10 1500 python -m pytest tests/test_fused_engine_gpu.py -q -m multigpu -p no:cacheprovider -k "equals_nccl" > $OUT/t_multigpu_equiv.log 2>&1; echo "test_equiv rc=$?" ;;
     geomed)     timeout -k 10 900 $TR --master-port 29616 bench.py --gpus $N --steps 30 --warmup 5 --approach baseline --mode geometric_median --sanity-steps 0 > $OUT/bench_geomed.log 2> $OUT/bench_geomed.err; echo "geomed rc=$?" ;;
     vgg_cyclic) timeout -k 10 900 $TR --master-port 29617 bench.py --gpus $N --steps 30 --warmup 5 --network VGG11 --approach cyclic --worker-fail 1 --err-mode constant --sanity-steps 0 > $OUT/bench_vgg_cyclic.log 2> $OUT/bench_vgg_cyclic.err; echo "vgg_cyclic rc=$?" ;;

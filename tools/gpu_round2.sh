@@ -20,7 +20,6 @@ for s in "$@"; do
     bench1_flat) timeout -k 10 600 python bench.py --gpus 1 --steps 20 --warmup 5 --impl nccl_flat > gpurun_out/bench1_flat.log 2>&1; echo "bench1_flat rc=$?" ;;
     bench1_ps) CUDA_DEVICE_MAX_CONNECTIONS=32 timeout -k 10 600 python bench.py --gpus 1 --steps 20 --warmup 5 --ps-stream > gpurun_out/bench1_psstream.log 2>&1; echo "bench1_ps rc=$?" ;;
     ncu_small) timeout -k 10 900 ncu --set full --clock-control none --import-source on -k regex:"convg_tcgen05|conv_halo|wgrad_halo|bn_bwd|bn_apply|stem_" -s 10 -c 14 -f -o gpurun_out/prof_conv python tools/prof_conv.py > gpurun_out/ncu_conv.log 2>&1; echo "ncu_small rc=$?" ;;
-    ncu_gemm2) DRACO_GEMM_2CTA=1 timeout -k 10 600 ncu --set full --clock-control none --import-source on -k regex:"gemm2_bf16|gemm_bf16" -s 4 -c 4 -f -o gpurun_out/prof_gemm2 python tools/bench_gemm.py --quick > gpurun_out/ncu_gemm2.log 2>&1; echo "ncu_gemm2 rc=$?" ;;
     launches) timeout -k 10 900 ncu --metrics gpu__time_duration.sum --clock-control none --csv --log-file gpurun_out/launches.csv python -c "import __graft_entry__ as g; g.smoke()" > gpurun_out/launches.log 2>&1; echo "launches rc=$?" ;;
   esac
 done

@@ -1,6 +1,6 @@
 // Micro-benchmark: what does programmatic dependent launch buy for a chain of short dependent kernels inside a CUDA graph?
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o pdl_chain pdl_chain.cu && ./pdl_chain
-// Kernel = 148 CTAs x 256 threads, SMEM bytes of dynamic shared memory (1 CTA / SM when large), prologue (barrier-init stand-in),
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o pdl_chain pdl_chain.cu && ./pdl_chain
+// Kernel = one CTA per SM x 256 threads, SMEM bytes of dynamic shared memory (1 CTA / SM when large), prologue (barrier-init stand-in),
 // then a streaming read-modify-write of `elems` floats (dependent on the previous kernel's output).
 #include <cuda_runtime.h>
 #include <cstdio>
@@ -56,12 +56,14 @@ static float run(int n_kernels, int smem, int elems, int pdl, int threads_grid) 
 }
 
 int main() {
+  int sms = 0;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
   const int smems[2] = {1024, 200 * 1024};
   const int elems[3] = {1 << 16, 1 << 21, 1 << 23};       // 0.25 MB, 8 MB, 32 MB per tensor
   for (int si = 0; si < 2; ++si)
     for (int ei = 0; ei < 3; ++ei) {
-      float t0 = run(200, smems[si], elems[ei], 0, 148);
-      float t1 = run(200, smems[si], elems[ei], 1, 148);
+      float t0 = run(200, smems[si], elems[ei], 0, sms);
+      float t1 = run(200, smems[si], elems[ei], 1, sms);
       printf("smem %6d B  tensor %5.2f MB : %.2f us/kernel plain, %.2f us/kernel PDL\n", smems[si], elems[ei] * 4 / 1e6, t0, t1);
     }
   return 0;

@@ -29,7 +29,7 @@ def main(rep, out, title):
     hdr, units, data = rows[0], rows[1], rows[2:]
     col = {h: i for i, h in enumerate(hdr)}
     with open(out, "w") as fh:
-        fh.write(f"# {title}\n\nsource: `{rep}` (`ncu --set full --clock-control none --import-source on`, one B200)\n\n")
+        fh.write(f"# {title}\n\nsource: `{rep}` (`ncu --set full --clock-control none --import-source on`, one H100)\n\n")
         names = [lab for k, lab in KEYS if k in col]
         fh.write("| kernel | " + " | ".join(names) + " |\n|---|" + "---:|" * len(names) + "\n")
         for r in data:

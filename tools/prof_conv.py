@@ -1,4 +1,4 @@
-"""Launch each tcgen05 convolution kernel (fprop with fused BatchNorm statistics / dgrad / wgrad) and the BatchNorm kernels a few
+"""Launch each wgmma convolution kernel (fprop with fused BatchNorm statistics / dgrad / wgrad) and the BatchNorm kernels a few
 times on ResNet-18 layer shapes -- the ncu target (`tools/gpu_ci.sh ncu_conv`)."""
 import os
 import sys

@@ -1,6 +1,6 @@
 """Where do the microseconds of a tap-convolution launch go?  Per-CTA clock64 stamps written by the kernel itself
-(drc_convg_set_timeline): setup (barriers, TMEM allocation) -> first operands landed -> last MMA issued -> accumulator complete ->
-tile stored -> exit, averaged over the CTAs, plus the spread of CTA start times (globaltimer).  Not a timed number: the stamps
+(drc_convg_set_timeline): setup (barrier initialisation) -> first operands landed -> last wgmma issued -> accumulator complete ->
+last tile stored -> exit, averaged over the CTAs, plus the spread of CTA start times (globaltimer).  Not a timed number: the stamps
 cost a few stores; the point is the breakdown."""
 import ctypes as C
 import json
@@ -16,7 +16,8 @@ dev = torch.device("cuda", 0)
 lib = CV._lib()
 lib.drc_convg_set_timeline.argtypes = [C.c_void_p]
 lib.drc_convg_set_timeline.restype = None
-MHZ = 1965.0
+MHZ = 1980.0                 # H100 SXM maximum SM clock (nvidia-smi clocks.max.sm); the stamps are clock64 cycles
+SMS = torch.cuda.get_device_properties(dev).multi_processor_count   # the launch grid never exceeds one CTA per SM
 
 
 def cl(t):
@@ -44,13 +45,13 @@ for (c, k, hw, ks, st) in [(128, 128, 16, 3, 1), (256, 256, 8, 3, 1), (512, 512,
             continue
         for _ in range(3):
             fn()
-        buf = torch.zeros(148 * 8, dtype=torch.int64, device=dev)
+        buf = torch.zeros(SMS * 8, dtype=torch.int64, device=dev)
         torch.cuda.synchronize()
         lib.drc_convg_set_timeline(buf.data_ptr())
         fn()
         torch.cuda.synchronize()
         lib.drc_convg_set_timeline(None)
-        t = buf.view(148, 8).cpu()
+        t = buf.view(SMS, 8).cpu()
         t = t[t[:, 1] != 0]
         rel = (t[:, 1:7] - t[:, 1:2]).double() / MHZ           # us since CTA entry
         g0 = (t[:, 0] - t[:, 0].min()).double() / 1e3
@@ -61,7 +62,7 @@ for (c, k, hw, ks, st) in [(128, 128, 16, 3, 1), (256, 256, 8, 3, 1), (512, 512,
                "tile_stored_us": round(float(m[5]), 2),
                "span_first_entry_to_last_exit_us": round(float((t[:, 7].max() - t[:, 0].min())) / 1e3, 2)}
         # the same launch five times back to back inside a CUDA graph: kernel period vs the time no CTA of either kernel is alive
-        bufs = [torch.zeros(148 * 8, dtype=torch.int64, device=dev) for _ in range(5)]
+        bufs = [torch.zeros(SMS * 8, dtype=torch.int64, device=dev) for _ in range(5)]
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
             for b in bufs:
@@ -70,7 +71,7 @@ for (c, k, hw, ks, st) in [(128, 128, 16, 3, 1), (256, 256, 8, 3, 1), (512, 512,
         lib.drc_convg_set_timeline(None)
         g.replay()
         torch.cuda.synchronize()
-        tt = [b.view(148, 8).cpu() for b in bufs]
+        tt = [b.view(SMS, 8).cpu() for b in bufs]
         tt = [x[x[:, 1] != 0] for x in tt]
         starts = [int(x[:, 0].min()) for x in tt]
         ends = [int(x[:, 7].max()) for x in tt]

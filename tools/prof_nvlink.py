@@ -48,7 +48,7 @@ def main():
     out = {}
     for name, fn, nbytes in (
             ("push_encode_16cta", lambda: K.push_encode(layout, grad, [None], slot_remote[0], step_ptr=step, worker=0, done_counter=cnt[0:1], grid=16), D * 4),
-            ("push_encode_148cta", lambda: K.push_encode(layout, grad, [None], slot_remote[1], step_ptr=step, worker=0, done_counter=cnt[1:2], grid=148), D * 4),
+            ("push_encode_full_grid", lambda: K.push_encode(layout, grad, [None], slot_remote[1], step_ptr=step, worker=0, done_counter=cnt[1:2], grid=K.sm_count()), D * 4),
             ("aggregate_update_unicast", lambda: K.aggregate_update(layout, grad_in, D, K=2, scale=0.5, params=params, momentum=mom, hp=hp, step_ptr=step,
                                                                    done_counter=cnt[2:3], dst=[params_remote.data_ptr()]), D * 4)):
         for _ in range(3):

@@ -1,6 +1,6 @@
 #!/bin/bash
 # Run on the parameter-server node: install the cluster key, make every node reachable by its alias (node0 = PS, node1..), and
-# replicate the repository (sources only; each node builds its own sm_100a extensions) to all workers.
+# replicate the repository (sources only; each node builds its own sm_90a extensions) to all workers.
 # Idempotent: the ssh settings live in their own file (used with `ssh -F`), /etc/hosts entries are replaced, never duplicated.
 # (role of the reference's tools/remote_script.sh:1-18)
 set -euo pipefail

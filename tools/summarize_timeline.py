@@ -1,7 +1,7 @@
 """Summarise a `bench.py --timeline` kernel timeline (one rank): step period, busy time per stream, time per kernel class, and
 the forward / backward / tail split of the middle one of the three recorded steps.
 
-    python tools/summarize_timeline.py gpurun_out/multi_N8/timeline.rank1.txt > profiles/step_timeline_N8_worker.md
+    python tools/summarize_timeline.py timeline.rank1.txt > step_timeline_worker.md
 """
 import collections
 import re
@@ -24,14 +24,14 @@ period = rows[b][0] - t0 if b < len(rows) else step[-1][0] + step[-1][1] - t0
 
 def cls(n):
     n = n.replace("(anonymous namespace)::", "").replace("void ", "")
-    for pat, c in (("conv_halo_tcgen05_kernel<false>|conv_halo_tcgen05_kernel<0>", "conv fprop (halo, tcgen05)"),
-                   ("conv_halo_tcgen05_kernel", "conv dgrad (halo, tcgen05)"),
-                   ("wgrad_halo|convg_wgrad|wgradg_reduce|stem_wgrad", "conv wgrad (tcgen05 / stem) + split-K fold"),
-                   (r"convg_tcgen05_kernel<\d+, \d+, false|convg_tcgen05_kernel<\d+, \d+, 0", "conv fprop (tap, tcgen05)"),
-                   ("convg_tcgen05_kernel", "conv dgrad (tap, tcgen05)"),
+    for pat, c in (("conv_halo_wgmma_kernel<false>|conv_halo_wgmma_kernel<0>", "conv fprop (halo, wgmma)"),
+                   ("conv_halo_wgmma_kernel", "conv dgrad (halo, wgmma)"),
+                   ("wgrad_halo|convg_wgrad|wgradg_reduce|stem_wgrad", "conv wgrad (wgmma / stem) + split-K fold"),
+                   (r"convg_wgmma_kernel<\d+, \d+, false|convg_wgmma_kernel<\d+, \d+, 0", "conv fprop (tap, wgmma)"),
+                   ("convg_wgmma_kernel", "conv dgrad (tap, wgmma)"),
                    ("stem_fprop", "stem fprop"),
                    ("bn_apply", "BatchNorm apply (+res +ReLU)"), ("bn_bwd", "BatchNorm backward"), ("bn_stats", "BatchNorm statistics"),
-                   ("gemm_bf16|gemm2_bf16", "linear (tcgen05 GEMM)"), ("push_encode", "push_encode (gradient -> PS slot)"),
+                   ("gemm_bf16", "linear (wgmma GEMM)"), ("push_encode", "push_encode (gradient -> PS slot)"),
                    ("ce_fused|prep_input|gap_|head_prep|cast_params|wait_flags|stamp|step_add|dropout", "loss / prep / pool / flags (ours)"),
                    ("Memcpy|memset|Memset", "memcpy / memset")):
         if re.search(pat, n):

@@ -1,4 +1,4 @@
-"""Cluster-shape sweep of the tap convolution (csrc/cuda/conv_tap_tcgen05.cu): for the ResNet-18/CIFAR layers at B=128, time
+"""Cluster-shape sweep of the tap convolution (csrc/cuda/conv_tap_wgmma.cu): for the ResNet-18/CIFAR layers at B=128, time
 fprop (with fused BatchNorm statistics) and dgrad for every cluster shape cm x cn and tile width the kernel supports
 (DRACO_CONV_CLUSTER override), with the same CUDA-graph timing as tools/bench_conv.py, and check each variant against the
 no-cluster result (bit-exact: same MMA order per tile).  Writes gpurun_out/conv_cluster_sweep.json; the planner
@@ -47,7 +47,7 @@ N = 128
 SHAPES = [(128, 128, 16, 3, 1), (256, 256, 8, 3, 1), (512, 512, 4, 3, 1), (64, 128, 32, 3, 2), (128, 256, 16, 3, 2),
           (256, 512, 8, 3, 2), (64, 128, 32, 1, 2), (256, 512, 8, 1, 2), (64, 64, 32, 3, 1)]
 CONFIGS = os.environ["SWEEP_CONFIGS"].split(";") if os.environ.get("SWEEP_CONFIGS") else ["1,1,128", "1,1,64", "2,1,128", "4,1,128", "8,1,128", "1,2,128", "2,2,128", "4,2,128", "2,4,128", "1,2,64", "2,2,64",
-           "4,2,64", "2,4,64", "1,4,64", "1,8,64", "4,1,64", "8,1,64", "auto", "pair"]
+           "4,2,64", "2,4,64", "1,4,64", "1,8,64", "4,1,64", "8,1,64", "auto"]
 rows = []
 for (c, k, hw, ks, st) in SHAPES:
     x = cl(torch.randn(N, c, hw, hw, device=dev))
@@ -61,8 +61,8 @@ for (c, k, hw, ks, st) in SHAPES:
         row = {"Cin": c, "Cout": k, "HW": hw, "ks": ks, "stride": st, "cfg": cfg}
         for name, dg in (("fprop", 0), ("dgrad", 1)):
             plan = C.convg_plan(N, hw, hw, c, k, ks, st, dg)
-            want = None if cfg in ("auto", "pair") else [int(v) for v in cfg.split(",")]
-            if (want is not None and [plan[1], plan[2], plan[0]] != want) or (cfg == "pair" and plan[4] != 2):
+            want = None if cfg == "auto" else [int(v) for v in cfg.split(",")]
+            if want is not None and [plan[1], plan[2], plan[0]] != want:
                 row[name + "_us"] = None                      # shape not realisable for this layer
                 continue
             row[name + "_plan"] = plan
