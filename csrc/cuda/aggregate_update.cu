@@ -13,12 +13,13 @@
 
 struct UpdateArgs {
   // gradient source ---------------------------------------------------------------------------
-  int mode;                       // 0: select-sum over `select` table; 1: cyclic recombination; 2: real per-tensor weights
+  int mode;                       // 0: select-sum over `select` table; 1: cyclic recombination; 2: real per-tensor weights;
+                                  // 3: coordinate-wise trimmed mean over rows 0..K-1 (see `trim`)
   const float* grad_in;           // mode 0: [P][slot_stride] fp32 ; mode 1: [n][2*slot_stride] complex64
   long long slot_stride;          // elements (fp32 words for mode 0, complex elements for mode 1)
   const int* select;              // mode 0: [K][T] worker slot to read for (k, tensor); null -> rows 0..K-1 for all tensors
   int K;                          // mode 0: rows summed per tensor ; mode 1: n workers
-  float scale;                    // 1/K (mean, vote), 1 (krum, median vector), 1/n (cyclic)
+  float scale;                    // 1/K (mean, vote, multi-Krum), 1 (krum, median vector), 1/n (cyclic), 1/(K - 2 trim) (mode 3)
   const float2* recomb;           // mode 1: [T][n] recombination vector v (float2 = complex64); mode 2: float [T][K] weights
   TileView tv;
   // optimizer ---------------------------------------------------------------------------------
@@ -37,9 +38,79 @@ struct UpdateArgs {
   unsigned int* done_counter;
   FlagList flags;                 // params_ready flags (peer pointers); value written = step + 1
   int tile_begin, tile_end;       // bucket of tiles to update + broadcast (tile_end == 0: whole arena)
+  int trim;                       // mode 3: values dropped at each end of every coordinate (K = P <= TRIM_MAXP rows,
+                                  // scale = 1 / (P - 2 * trim)); coordinate median: trim = (P - 1) / 2
 };
 
-template <int MODE>
+// ---------------------------------------------------------------------------------------------
+// Mode 3: coordinate-wise trimmed mean (Yin et al., ICML 2018) and coordinate-wise median.
+//
+// Every thread sorts the P values of each of its 4 coordinates in registers with Batcher's odd-even merge network (N = 4,
+// 8 or 16 inputs, padded with a sentinel), on order-preserving uint32 keys so that compare-exchange is an integer min/max:
+// -Inf < finite < +Inf < NaN < padding.  NaN (any sign or payload) becomes the largest non-sentinel key, so up to `trim`
+// NaN / +-Inf values per coordinate land in the trimmed tails.  The kept values are summed in ascending order in fp32:
+// the result depends only on the P values of the coordinate, not on the grid or on the bucketing.
+// ---------------------------------------------------------------------------------------------
+#define TRIM_MAXP 16
+
+__device__ __forceinline__ unsigned int float_key(float f) {
+  const unsigned int u = __float_as_uint(f);
+  if (f != f) return 0xFFFFFFFEu;
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float key_float(unsigned int k) {
+  return __uint_as_float((k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k);
+}
+
+// Batcher's odd-even merge sort written out comparator by comparator (5 / 19 / 63 compare-exchanges), so that every index
+// is a constant and the keys never leave registers
+#define CX(i, j) { const unsigned int lo_ = min(k[i], k[j]); k[j] = max(k[i], k[j]); k[i] = lo_; }
+template <int N> __device__ __forceinline__ void sort_net(unsigned int (&k)[N]);
+template <> __device__ __forceinline__ void sort_net<4>(unsigned int (&k)[4]) {
+  CX(0, 1) CX(2, 3) CX(0, 2) CX(1, 3) CX(1, 2)
+}
+template <> __device__ __forceinline__ void sort_net<8>(unsigned int (&k)[8]) {
+  CX(0, 1) CX(2, 3) CX(4, 5) CX(6, 7) CX(0, 2) CX(1, 3) CX(4, 6) CX(5, 7) CX(1, 2) CX(5, 6) CX(0, 4) CX(1, 5) CX(2, 6)
+  CX(3, 7) CX(2, 4) CX(3, 5) CX(1, 2) CX(3, 4) CX(5, 6)
+}
+template <> __device__ __forceinline__ void sort_net<16>(unsigned int (&k)[16]) {
+  CX(0, 1) CX(2, 3) CX(4, 5) CX(6, 7) CX(8, 9) CX(10, 11) CX(12, 13) CX(14, 15) CX(0, 2) CX(1, 3) CX(4, 6) CX(5, 7)
+  CX(8, 10) CX(9, 11) CX(12, 14) CX(13, 15) CX(1, 2) CX(5, 6) CX(9, 10) CX(13, 14) CX(0, 4) CX(1, 5) CX(2, 6) CX(3, 7)
+  CX(8, 12) CX(9, 13) CX(10, 14) CX(11, 15) CX(2, 4) CX(3, 5) CX(10, 12) CX(11, 13) CX(1, 2) CX(3, 4) CX(5, 6)
+  CX(9, 10) CX(11, 12) CX(13, 14) CX(0, 8) CX(1, 9) CX(2, 10) CX(3, 11) CX(4, 12) CX(5, 13) CX(6, 14) CX(7, 15)
+  CX(4, 8) CX(5, 9) CX(6, 10) CX(7, 11) CX(2, 4) CX(3, 5) CX(6, 8) CX(7, 9) CX(10, 12) CX(11, 13) CX(1, 2) CX(3, 4)
+  CX(5, 6) CX(7, 8) CX(9, 10) CX(11, 12) CX(13, 14)
+}
+#undef CX
+
+template <int N>
+__device__ __forceinline__ float4 trimmed_mean_f4(const UpdateArgs& a, long long idx) {
+  unsigned int k[4][N];
+#pragma unroll
+  for (int r = 0; r < N; ++r) {
+    if (r < a.K) {
+      const float4 v = ld_f4(reinterpret_cast<const float4*>(a.grad_in + r * a.slot_stride + idx));
+      k[0][r] = float_key(v.x); k[1][r] = float_key(v.y); k[2][r] = float_key(v.z); k[3][r] = float_key(v.w);
+    } else {
+      k[0][r] = k[1][r] = k[2][r] = k[3][r] = 0xFFFFFFFFu;
+    }
+  }
+  float out[4];
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    sort_net<N>(k[e]);
+    float s = 0.f;
+#pragma unroll
+    for (int r = 0; r < N; ++r)
+      if (r >= a.trim && r < a.K - a.trim) s += key_float(k[e][r]);
+    out[e] = s;
+  }
+  return make_float4(out[0], out[1], out[2], out[3]);
+}
+
+// SORT_N: mode 3 only, the sorting-network size (4, 8 or 16 >= K).  Each size is its own instantiation so that a launch pays the
+// registers of its own network (4 x SORT_N keys per thread), not those of the largest one.
+template <int MODE, int SORT_N = 0>
 __global__ void __launch_bounds__(DRC_THREADS) aggregate_update_kernel(const __grid_constant__ UpdateArgs a) {
   const HyperParams hp = *a.hp;
   const unsigned long long step = *a.step_ptr;
@@ -69,6 +140,8 @@ __global__ void __launch_bounds__(DRC_THREADS) aggregate_update_kernel(const __g
         float4 v = ld_f4(reinterpret_cast<const float4*>(a.grad_in + k * a.slot_stride + idx));
         g.x = fmaf(w, v.x, g.x); g.y = fmaf(w, v.y, g.y); g.z = fmaf(w, v.z, g.z); g.w = fmaf(w, v.w, g.w);
       }
+    } else if constexpr (MODE == 3) {
+      g = trimmed_mean_f4<SORT_N>(a, idx);
     } else {
       for (int k = 0; k < a.K; ++k) {
         const float2 v = a.recomb[tensor * a.K + k];
@@ -132,8 +205,13 @@ __global__ void __launch_bounds__(DRC_THREADS) aggregate_update_kernel(const __g
 
 extern "C" int drc_aggregate_update(const UpdateArgs* args, int grid, cudaStream_t stream) {
   if (args->ndst > DRC_MAX_DST || args->flags.n > DRC_MAX_DST) return (int)cudaErrorInvalidValue;
+  if (args->mode == 3 && (args->K < 1 || args->K > TRIM_MAXP || args->trim < 0 || 2 * args->trim >= args->K))
+    return (int)cudaErrorInvalidValue;
   if (args->mode == 0) aggregate_update_kernel<0><<<grid, DRC_THREADS, 0, stream>>>(*args);
   else if (args->mode == 2) aggregate_update_kernel<2><<<grid, DRC_THREADS, 0, stream>>>(*args);
+  else if (args->mode == 3 && args->K <= 4) aggregate_update_kernel<3, 4><<<grid, DRC_THREADS, 0, stream>>>(*args);
+  else if (args->mode == 3 && args->K <= 8) aggregate_update_kernel<3, 8><<<grid, DRC_THREADS, 0, stream>>>(*args);
+  else if (args->mode == 3) aggregate_update_kernel<3, 16><<<grid, DRC_THREADS, 0, stream>>>(*args);
   else aggregate_update_kernel<1><<<grid, DRC_THREADS, 0, stream>>>(*args);
   return (int)cudaGetLastError();
 }

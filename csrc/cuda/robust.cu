@@ -18,7 +18,8 @@
 //
 // Krum -- reference: double Python loop of np.linalg.norm per tensor (baseline_master.py:278-296).  Here one
 // pass produces all P(P-1)/2 squared distances per tensor, a one-thread-per-tensor kernel scores and selects,
-// and the winner row goes through the fused select + SGD + broadcast kernel.
+// and the winner row goes through the fused select + SGD + broadcast kernel.  Multi-Krum (Blanchard et al., NeurIPS 2017)
+// selects the m lowest-scoring rows instead, and the same fused kernel averages them.
 #include "common.cuh"
 
 #define GM_MAXP DRC_MAX_WORKERS
@@ -144,6 +145,7 @@ extern "C" int drc_geomed_prep(const GeoMedPrepArgs* args, cudaStream_t stream) 
 // ---------------------------------------------------------------------------------------------
 #define KRUM_MAXP 16
 #define KRUM_MAXPAIRS (KRUM_MAXP * (KRUM_MAXP - 1) / 2)
+#define KRUM_SELECT_THREADS 64
 
 struct PairDistArgs {
   const float* grad_in;
@@ -193,8 +195,13 @@ __global__ void __launch_bounds__(DRC_THREADS) pair_dist_kernel(const __grid_con
 struct KrumSelectArgs {
   double* pair_d2;                // consumed and zeroed
   int T, P, s;
-  int* select;                    // [T] winning worker slot
+  int m;                          // slots selected per tensor: 1 = Krum, P - s = multi-Krum
+  int* select;                    // [m][T] the m lowest-scoring worker slots, ordered by (score, index)
 };
+
+// Order of distances and scores: ascending with NaN last (what torch.sort / np.sort do), so that a row that sends NaN gets a
+// NaN score and is chosen last, as on the library path; on NaN-free input this is the plain `<`.
+__device__ __forceinline__ bool less_nan_last(double x, double y) { return x < y || (y != y && x == x); }
 
 __global__ void krum_select_kernel(const __grid_constant__ KrumSelectArgs a) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -203,7 +210,8 @@ __global__ void krum_select_kernel(const __grid_constant__ KrumSelectArgs a) {
   double* d2 = a.pair_d2 + (long long)t * npairs;
   int keep = a.P - a.s - 2;
   if (keep < 0) keep = 0;
-  double best = 0.0; int best_i = 0;
+  __shared__ double s_score[KRUM_MAXP][KRUM_SELECT_THREADS];
+  double* sc = &s_score[0][threadIdx.x];                       // score of slot i at sc[i * KRUM_SELECT_THREADS]
   for (int i = 0; i < a.P; ++i) {
     double nb[KRUM_MAXP]; int c = 0;
     for (int j = 0; j < a.P; ++j) {
@@ -211,12 +219,24 @@ __global__ void krum_select_kernel(const __grid_constant__ KrumSelectArgs a) {
       int lo = i < j ? i : j, hi = i < j ? j : i;
       nb[c++] = d2[hi * (hi - 1) / 2 + lo];
     }
-    for (int x = 1; x < c; ++x) { double k = nb[x]; int y = x - 1; while (y >= 0 && nb[y] > k) { nb[y + 1] = nb[y]; --y; } nb[y + 1] = k; }
+    for (int x = 1; x < c; ++x) { double k = nb[x]; int y = x - 1; while (y >= 0 && less_nan_last(k, nb[y])) { nb[y + 1] = nb[y]; --y; } nb[y + 1] = k; }
     double score = 0.0;
     for (int x = 0; x < keep && x < c; ++x) score += nb[x];
-    if (i == 0 || score < best) { best = score; best_i = i; }
+    sc[i * KRUM_SELECT_THREADS] = score;
   }
-  a.select[t] = best_i;
+  // m rounds of selection among the slots not chosen yet: the first one in index order, replaced by any later one with a
+  // strictly lower score (NaN last) -- ties go to the lower index, and m = 1 is the Krum winner
+  unsigned int used = 0;
+  for (int q = 0; q < a.m; ++q) {
+    double best = 0.0; int best_i = -1;
+    for (int i = 0; i < a.P; ++i) {
+      if ((used >> i) & 1u) continue;
+      const double s = sc[i * KRUM_SELECT_THREADS];
+      if (best_i < 0 || less_nan_last(s, best)) { best = s; best_i = i; }
+    }
+    used |= 1u << best_i;
+    a.select[q * a.T + t] = best_i;
+  }
   for (int q = 0; q < npairs; ++q) d2[q] = 0.0;
 }
 
@@ -226,8 +246,8 @@ extern "C" int drc_pair_dist(const PairDistArgs* args, int grid, cudaStream_t st
   return (int)cudaGetLastError();
 }
 extern "C" int drc_krum_select(const KrumSelectArgs* args, cudaStream_t stream) {
-  if (args->P > KRUM_MAXP) return (int)cudaErrorInvalidValue;
-  krum_select_kernel<<<(args->T + 63) / 64, 64, 0, stream>>>(*args);
+  if (args->P > KRUM_MAXP || args->m < 1 || args->m > args->P) return (int)cudaErrorInvalidValue;
+  krum_select_kernel<<<(args->T + KRUM_SELECT_THREADS - 1) / KRUM_SELECT_THREADS, KRUM_SELECT_THREADS, 0, stream>>>(*args);
   return (int)cudaGetLastError();
 }
 

@@ -88,20 +88,50 @@ def geometric_median_weights(slots: np.ndarray, eps: float = 1e-10, max_iter: in
 
 def krum_index(slots: np.ndarray, s: int) -> int:
     """Krum (arXiv:1703.02757) as the reference implements it (baseline_master.py:278-296):
-    score_i = sum of the (P - s - 2) smallest squared distances to the others; argmin wins."""
-    X = np.asarray(slots, dtype=np.float64)
-    P = X.shape[0]
-    keep = max(P - s - 2, 0)
-    d2 = ((X[:, None, :] - X[None, :, :]) ** 2).sum(axis=2)
-    scores = []
-    for i in range(P):
-        others = np.sort(np.delete(d2[i], i))
-        scores.append(others[:keep].sum())
-    return int(np.argmin(scores))
+    score_i = sum of the (P - s - 2) smallest squared distances to the others; argmin wins (the lowest index on ties, and
+    NaN scores -- a row that sent NaN -- rank last, like every sort here)."""
+    return int(np.argsort(krum_scores(slots, s), kind="stable")[0])
 
 
 def krum(slots: np.ndarray, s: int) -> np.ndarray:
     return np.asarray(slots, dtype=np.float64)[krum_index(slots, s)]
+
+
+def krum_scores(slots: np.ndarray, s: int) -> np.ndarray:
+    """score_i of ``krum_index``: the sum of the (P - s - 2) smallest squared distances from row i to the others (NaN
+    distances sort last)."""
+    X = np.asarray(slots, dtype=np.float64)
+    P = X.shape[0]
+    keep = max(P - s - 2, 0)
+    d2 = ((X[:, None, :] - X[None, :, :]) ** 2).sum(axis=2)
+    return np.array([np.sort(np.delete(d2[i], i))[:keep].sum() for i in range(P)])
+
+
+def multi_krum_indices(slots: np.ndarray, s: int, m: int) -> List[int]:
+    """Multi-Krum (Blanchard et al., NeurIPS 2017): the ``m`` rows with the lowest Krum scores, ordered by (score, index).
+    ``m = 1`` is ``[krum_index(slots, s)]``; the trainer averages ``m = P - s`` rows."""
+    return [int(i) for i in np.argsort(krum_scores(slots, s), kind="stable")[:m]]
+
+
+def multi_krum(slots: np.ndarray, s: int, m: int) -> np.ndarray:
+    return np.asarray(slots, dtype=np.float64)[multi_krum_indices(slots, s, m)].mean(axis=0)
+
+
+def trimmed_mean(slots: np.ndarray, b: int) -> np.ndarray:
+    """Coordinate-wise b-trimmed mean (Yin et al., ICML 2018): per coordinate, sort the P values ascending, drop ``b`` at each
+    end and average the remaining P - 2b.  The order is -Inf < finite < +Inf < NaN (``np.sort``), so at most ``b`` non-finite
+    values in a coordinate are always dropped."""
+    X = np.asarray(slots, dtype=np.float64)
+    P = X.shape[0]
+    if not 0 <= 2 * b < P:
+        raise ValueError(f"trim {b} leaves nothing of {P} rows")
+    return np.sort(X, axis=0)[b:P - b].mean(axis=0)
+
+
+def coordinate_median(slots: np.ndarray) -> np.ndarray:
+    """Coordinate-wise median: the trimmed mean with b = (P - 1) // 2 -- the middle value for odd P, the mean of the two
+    middle values for even P (``np.median``; not ``torch.median``, which returns the lower one)."""
+    return trimmed_mean(slots, (np.asarray(slots).shape[0] - 1) // 2)
 
 
 def sgd_momentum_step(p: np.ndarray, buf: np.ndarray, g: np.ndarray, lr: float, momentum: float,

@@ -11,7 +11,8 @@ from dataclasses import asdict, dataclass
 from typing import Optional
 
 APPROACHES = ("baseline", "maj_vote", "cyclic")
-MODES = ("normal", "geometric_median", "krum", "maj_vote")
+MODES = ("normal", "geometric_median", "krum", "maj_vote", "coordinate_median", "trimmed_mean", "multi_krum")
+ROBUST_MAXP = 16                    # workers the fused coordinate-wise / Krum kernels take (TRIM_MAXP, KRUM_MAXP)
 ERR_MODES = ("rev_grad", "constant", "random", "omniscient", "none")
 TRANSPORTS = ("nvl", "nccl", "nccl_flat", "gloo")
 
@@ -101,6 +102,17 @@ class JobConfig:
                                  f"divides num_workers more evenly")
         if self.no_cuda:
             self.transport = "gloo"
+        if self.approach == "baseline" and self.mode in ("coordinate_median", "trimmed_mean", "multi_krum"):
+            P, f = self.num_workers, self.worker_fail
+            if self.mode != "multi_krum" and 2 * f >= P:
+                raise ValueError(f"--mode {self.mode} trims --worker-fail {f} values at each end of every coordinate: it needs "
+                                 f"num_workers > 2*worker_fail (got {P} workers)")
+            if self.mode == "multi_krum" and P <= 2 * f + 2:
+                raise ValueError(f"--mode multi_krum needs num_workers > 2*worker_fail + 2 (Krum's condition; got {P} workers, "
+                                 f"worker_fail {f})")
+            if self.transport == "nvl" and P > ROBUST_MAXP:
+                raise ValueError(f"--mode {self.mode} on the nvl transport handles at most {ROBUST_MAXP} workers (got {P}); "
+                                 f"use --transport nccl for more")
         if self.compress and self.transport == "nvl" and self.err_mode == "omniscient":
             raise ValueError("--err-mode omniscient reads the honest slots in PS memory while they arrive; with --compress-grad "
                              "compress they only exist after the PS unpacked them -- pass --compress-grad None")
@@ -153,7 +165,10 @@ def add_fit_args(parser: argparse.ArgumentParser) -> argparse.ArgumentParser:
     a("--profile-phases", action="store_true", default=d.profile_phases,
       help="time the reference's phases (Comm / Comp / Encode / Method / Update) with CUDA events each step; eager mode")
     a("--network", type=str, default=d.network)
-    a("--mode", type=str, default=d.mode, help="normal | geometric_median | krum (baseline); normal | maj_vote (maj_vote)")
+    a("--mode", type=str, default=d.mode,
+      help="normal | geometric_median | krum | coordinate_median | trimmed_mean | multi_krum (baseline); normal | maj_vote "
+           "(maj_vote).  trimmed_mean drops --worker-fail values at each end of every coordinate; multi_krum averages the "
+           "num_workers - worker_fail workers with the lowest Krum scores")
     a("--dataset", type=str, default=d.dataset)
     a("--comm-type", type=str, default=d.comm_type)
     a("--err-mode", type=str, default=d.err_mode, help="rev_grad | constant | random | omniscient | none")

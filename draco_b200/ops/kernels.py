@@ -134,8 +134,9 @@ def aggregate_update(layout: ArenaLayout, grad_in: Addr, slot_stride: int, *, pa
                      recomb: Addr = None, first_step: int = 1, grad_out: Addr = None, mc_params: Addr = None,
                      dst: Sequence[Addr] = (), flags: Sequence[Addr] = (), grid: Optional[int] = None,
                      tile_range: Optional[tuple] = None, weights: Addr = None, exp_avg_sq: Addr = None,
-                     max_exp_avg_sq: Addr = None) -> None:
-    """Fused aggregate (select-sum, cyclic recombination, or real per-tensor ``weights`` [T, K]) + optimizer step (SGD-momentum, or
+                     max_exp_avg_sq: Addr = None, trim: Optional[int] = None) -> None:
+    """Fused aggregate (select-sum, cyclic recombination, real per-tensor ``weights`` [T, K], or -- with ``trim`` -- the
+    coordinate-wise trimmed mean of rows 0..K-1 that drops ``trim`` values at each end, K <= 16) + optimizer step (SGD-momentum, or
     Adam / AMSGrad when the hyper-parameter block says so: ``momentum`` = first moment, ``exp_avg_sq`` / ``max_exp_avg_sq`` = second
     moment / its running maximum) + parameter broadcast + flags."""
     a = N.UpdateArgs()
@@ -143,6 +144,13 @@ def aggregate_update(layout: ArenaLayout, grad_in: Addr, slot_stride: int, *, pa
     if weights is not None:
         assert recomb is None and select is None
         recomb = weights
+    if trim is not None:
+        assert recomb is None and select is None
+        if not (1 <= K <= 16 and 0 <= 2 * trim < K):
+            raise ValueError(f"trimmed mean: K = {K} rows (at most 16) must exceed 2 * trim = {2 * trim}")
+        if abs(scale * (K - 2 * trim) - 1.0) > 1e-6:
+            raise ValueError(f"trimmed mean: scale must be 1 / (K - 2 * trim) = {1.0 / (K - 2 * trim)}, got {scale}")
+        a.mode, a.trim = 3, int(trim)
     a.grad_in = addr(grad_in)
     a.slot_stride = slot_stride
     a.select = addr(select)
@@ -296,12 +304,14 @@ def geometric_median_weights(layout: ArenaLayout, grad_in: Addr, slot_stride: in
 
 
 def krum_select(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, s: int, pair_d2: torch.Tensor,
-                select: torch.Tensor) -> None:
-    """``pair_d2``: zeroed fp64 [T, P*(P-1)/2] scratch (left zeroed); ``select``: int32 [T] out (winning slot)."""
+                select: torch.Tensor, m: int = 1) -> None:
+    """``pair_d2``: zeroed fp64 [T, P*(P-1)/2] scratch (left zeroed); ``select``: int32 [m, T] out, the ``m`` lowest Krum scores
+    per tensor ordered by (score, slot) -- ``m = 1``: the Krum winner, ``m = P - s``: multi-Krum (int32 [T] is fine for m = 1)."""
+    assert 1 <= m <= P and select.numel() >= m * layout.ntensors
     lib = N.cuda()
     pa = N.PairDistArgs(addr(grad_in), slot_stride, P, layout.tile_view(select.device), pair_d2.data_ptr())
     N.check(lib.drc_pair_dist(C.byref(pa), stream_grid(layout, 4), _stream()), "pair_dist")
-    ka = N.KrumSelectArgs(pair_d2.data_ptr(), layout.ntensors, P, s, select.data_ptr())
+    ka = N.KrumSelectArgs(pair_d2.data_ptr(), layout.ntensors, P, s, m, select.data_ptr())
     N.check(lib.drc_krum_select(C.byref(ka), _stream()), "krum_select")
 
 

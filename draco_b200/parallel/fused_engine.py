@@ -9,8 +9,9 @@ Step anatomy (one PS + P logical workers hosted by ``nprocs`` GPU processes; see
     forward / backward  (x R sub-batches under the cyclic code)
     push_encode: encode + adversary + 16 B peer stores  ------>  grad_in[w]   + release flag grad_ready[w] = t
                                                                  wait_flags(grad_ready[*] >= t)
-                                                                 vote | project+locate | krum | geomedian   (decode)
+                                                                 vote | project+locate | (multi-)krum | geomedian   (decode)
     params arena  <------ multimem.st / peer stores  ----------  aggregate_update: SGD-momentum + broadcast
+                                                                 (coordinate median / trimmed mean: sorted inside it)
     flag params_ready = t+1  <---------------------------------  (last CTA)
 
 There is no NCCL / MPI call and no host synchronisation anywhere in that loop; ordering between GPUs is carried by
@@ -79,7 +80,7 @@ class FusedEngine:
         self.compress = bool(cfg.compress)
         self.overlap_push = cfg.overlap_push and not self.cyclic and not self.compress
         # PS pipelining: decode + apply + broadcast each gradient bucket as soon as all workers pushed it
-        self.pipeline_ps = (self.overlap_push and cfg.pipeline_ps and select_rule(cfg) in ("mean", "vote")
+        self.pipeline_ps = (self.overlap_push and cfg.pipeline_ps and select_rule(cfg) in ("mean", "vote", "median", "trimmed_mean")
                             and cfg.err_mode != "omniscient")
         self.push_stream = torch.cuda.Stream(device=device) if self.overlap_push else None
         ns = min(max(int(cfg.worker_streams), 1), len(self.local_workers))

@@ -26,12 +26,24 @@ from .arena import ArenaLayout
 def select_rule(cfg: JobConfig) -> str:
     """Aggregation rule of a job.  Mirrors the reference's dispatch: cyclic approach -> Fourier decode
     (cyclic_master.py:24); maj_vote approach -> vote only when ``--mode maj_vote``, plain mean for ``--mode normal``
-    (rep_master.py:118-129); baseline approach -> mean / geometric median / Krum by ``--mode`` (baseline_master.py:118-129)."""
+    (rep_master.py:118-129); baseline approach -> mean / geometric median / Krum by ``--mode`` (baseline_master.py:118-129), plus
+    three rules beyond the reference: coordinate-wise median, coordinate-wise trimmed mean and multi-Krum."""
     if cfg.approach == "cyclic":
         return "cyclic"
     if cfg.approach == "maj_vote":
         return "vote" if cfg.mode == "maj_vote" else "mean"
-    return {"normal": "mean", "geometric_median": "geomedian", "krum": "krum"}.get(cfg.mode, "mean")
+    return {"normal": "mean", "geometric_median": "geomedian", "krum": "krum", "coordinate_median": "median",
+            "trimmed_mean": "trimmed_mean", "multi_krum": "multi_krum"}.get(cfg.mode, "mean")
+
+
+def coordinate_trim(cfg: JobConfig) -> int:
+    """Values dropped at each end of every coordinate: (P - 1) // 2 for the median, ``--worker-fail`` for the trimmed mean."""
+    return (cfg.num_workers - 1) // 2 if select_rule(cfg) == "median" else cfg.worker_fail
+
+
+def multi_krum_m(cfg: JobConfig) -> int:
+    """Rows multi-Krum averages: P - f."""
+    return cfg.num_workers - cfg.worker_fail
 
 
 def hyperparams_tensor(cfg: JobConfig, device) -> torch.Tensor:
@@ -72,6 +84,12 @@ class FusedPS:
         elif self.rule == "krum":
             self.pair_d2 = torch.zeros(T, self.P * (self.P - 1) // 2, dtype=torch.float64, device=device)
             self.select = torch.zeros(T, dtype=torch.int32, device=device)
+        elif self.rule == "multi_krum":
+            self.m = multi_krum_m(cfg)
+            self.pair_d2 = torch.zeros(T, self.P * (self.P - 1) // 2, dtype=torch.float64, device=device)
+            self.select = torch.zeros(self.m, T, dtype=torch.int32, device=device)
+        elif self.rule in ("median", "trimmed_mean"):
+            self.trim = coordinate_trim(cfg)
         elif self.rule == "geomedian":
             if self.P <= K.GEOMED_FAST_MAXP:      # weight-space Weiszfeld: 2 passes over the slab in total
                 self.gm = None
@@ -108,7 +126,7 @@ class FusedPS:
                       hp=self.hp, step_ptr=step_ptr,
                       done_counter=self.counters[0:1], first_step=1, grad_out=grad_out, mc_params=mc_params, dst=dst)
         n = 0
-        if buckets is not None and self.rule in ("mean", "vote"):
+        if buckets is not None and self.rule in ("mean", "vote", "median", "trimmed_mean"):
             for bi, (t0, t1, idxs) in enumerate(buckets):
                 n += wait_bucket(bi)
                 fl = flags if bi == len(buckets) - 1 else []
@@ -120,11 +138,16 @@ class FusedPS:
                         n += before_update()
                     K.aggregate_update(L, self.grad_in, self.slot_stride, K=G, scale=1.0 / G, select=self.winner_slot,
                                        tile_range=(t0, t1), flags=fl, **common); n += 1
-                else:
+                elif self.rule == "mean":
                     if bi == len(buckets) - 1:
                         n += before_update()
                     K.aggregate_update(L, self.grad_in, self.slot_stride, K=self.P, scale=1.0 / self.P,
                                        tile_range=(t0, t1), flags=fl, **common); n += 1
+                else:                                      # coordinate-wise rules: element by element, nothing per tensor
+                    if bi == len(buckets) - 1:
+                        n += before_update()
+                    K.aggregate_update(L, self.grad_in, self.slot_stride, K=self.P, scale=1.0 / (self.P - 2 * self.trim),
+                                       trim=self.trim, tile_range=(t0, t1), flags=fl, **common); n += 1
             return n
         common["flags"] = flags
         _agg = K.aggregate_update
@@ -142,6 +165,11 @@ class FusedPS:
         elif self.rule == "krum":
             K.krum_select(L, self.grad_in, self.slot_stride, self.P, self.cfg.worker_fail, self.pair_d2, self.select); n += 2
             _update(L, self.grad_in, self.slot_stride, K=1, scale=1.0, select=self.select, **common); n += 1
+        elif self.rule == "multi_krum":
+            K.krum_select(L, self.grad_in, self.slot_stride, self.P, self.cfg.worker_fail, self.pair_d2, self.select, m=self.m); n += 2
+            _update(L, self.grad_in, self.slot_stride, K=self.m, scale=1.0 / self.m, select=self.select, **common); n += 1
+        elif self.rule in ("median", "trimmed_mean"):
+            _update(L, self.grad_in, self.slot_stride, K=self.P, scale=1.0 / (self.P - 2 * self.trim), trim=self.trim, **common); n += 1
         elif self.rule == "geomedian" and self.gm is None:
             K.geometric_median_weights(L, self.grad_in, self.slot_stride, self.P, self.pair_d2, self.gm_weights); n += 2
             _update(L, self.grad_in, self.slot_stride, K=self.P, scale=1.0, weights=self.gm_weights, **common); n += 1
@@ -182,6 +210,7 @@ class TorchPS:
             g = torch.Generator().manual_seed(cfg.seed + 4242)
             f = (torch.randn(layout.total, generator=g) + 1.0) * torch.from_numpy(layout.valid_mask()).float()
             self.f = f.to(device)
+        self.trim = coordinate_trim(cfg) if self.rule in ("median", "trimmed_mean") else 0
         self.last_info: Dict[str, object] = {}
 
     # --- optimizer state for checkpoints (the reference saves none: src/master/baseline_master.py:237-243) ----------
@@ -263,13 +292,29 @@ class TorchPS:
                 break
         return m
 
-    def _krum_tensor(self, X: torch.Tensor) -> int:
+    def _krum_scores(self, X: torch.Tensor) -> torch.Tensor:
         d2 = torch.cdist(X.double(), X.double()).pow(2)
         P = X.shape[0]
         keep = max(P - self.cfg.worker_fail - 2, 0)
         d2 = d2 + torch.diag(torch.full((P,), float("inf"), dtype=d2.dtype, device=d2.device))
-        scores = d2.sort(dim=1).values[:, :keep].sum(1)
-        return int(scores.argmin())
+        return d2.sort(dim=1).values[:, :keep].sum(1)
+
+    def _krum_tensor(self, X: torch.Tensor) -> int:
+        return int(torch.argsort(self._krum_scores(X), stable=True)[0])      # NaN scores last, like the kernel
+
+    def _multi_krum_tensor(self, X: torch.Tensor) -> torch.Tensor:
+        m = multi_krum_m(self.cfg)
+        best = torch.argsort(self._krum_scores(X), stable=True)[:m]
+        return X[best].sum(0) / m
+
+    def _trimmed_mean_tensor(self, X: torch.Tensor) -> torch.Tensor:
+        """Sort every coordinate (NaN sorts last), drop ``trim`` values at each end, sum the rest in ascending order."""
+        P, b = X.shape[0], self.trim
+        S = X.sort(0).values
+        acc = S[b].clone()
+        for k in range(b + 1, P - b):
+            acc += S[k]
+        return acc * (1.0 / (P - 2 * b))
 
     def _cyclic_tensor(self, R: torch.Tensor, f: torch.Tensor) -> torch.Tensor:
         """R: [n, d] complex64 -> Re(v^T R) / n with v from the C++ locator (N1 replacement)."""
@@ -300,6 +345,10 @@ class TorchPS:
                 g = acc / float(self.groups.num_groups)
             elif self.rule == "krum":
                 g = X[self._krum_tensor(X)]
+            elif self.rule == "multi_krum":
+                g = self._multi_krum_tensor(X)
+            elif self.rule in ("median", "trimmed_mean"):
+                g = self._trimmed_mean_tensor(X)
             elif self.rule == "geomedian":
                 g = self._geomedian_tensor(X)
             elif self.rule == "cyclic":
@@ -313,7 +362,8 @@ class TorchPS:
         self.apply(self.aggregate(slots))
 
     def apply(self, grads: List[torch.Tensor]) -> None:
-        mode = {"mean": "normal", "vote": "maj_vote", "krum": "krum", "geomedian": "geometric_median", "cyclic": "cyclic"}[self.rule]
+        mode = {"mean": "normal", "vote": "maj_vote", "krum": "krum", "geomedian": "geometric_median", "cyclic": "cyclic",
+                "median": "coordinate_median", "trimmed_mean": "trimmed_mean", "multi_krum": "multi_krum"}[self.rule]
         self.optimizer.step(grads=grads, mode=mode)
 
 
