@@ -14,10 +14,11 @@
 struct UpdateArgs {
   // gradient source ---------------------------------------------------------------------------
   int mode;                       // 0: select-sum over `select` table; 1: cyclic recombination; 2: real per-tensor weights;
-                                  // 3: coordinate-wise trimmed mean over rows 0..K-1 (see `trim`)
+                                  // 3: coordinate-wise trimmed mean over K rows (see `trim`)
   const float* grad_in;           // mode 0: [P][slot_stride] fp32 ; mode 1: [n][2*slot_stride] complex64
   long long slot_stride;          // elements (fp32 words for mode 0, complex elements for mode 1)
-  const int* select;              // mode 0: [K][T] worker slot to read for (k, tensor); null -> rows 0..K-1 for all tensors
+  const int* select;              // modes 0, 2, 3: [K][T] worker slot to read for (k, tensor); null -> rows 0..K-1 for all
+                                  // tensors.  DETOX: the vote's winner_slot table, so that the rule runs on the G group winners
   int K;                          // mode 0: rows summed per tensor ; mode 1: n workers
   float scale;                    // 1/K (mean, vote, multi-Krum), 1 (krum, median vector), 1/n (cyclic), 1/(K - 2 trim) (mode 3)
   const float2* recomb;           // mode 1: [T][n] recombination vector v (float2 = complex64); mode 2: float [T][K] weights
@@ -83,13 +84,15 @@ template <> __device__ __forceinline__ void sort_net<16>(unsigned int (&k)[16]) 
 }
 #undef CX
 
-template <int N>
-__device__ __forceinline__ float4 trimmed_mean_f4(const UpdateArgs& a, long long idx) {
+// SEL: row r of `tensor` is worker slot select[r][tensor] instead of slot r
+template <int N, bool SEL>
+__device__ __forceinline__ float4 trimmed_mean_f4(const UpdateArgs& a, long long idx, int tensor) {
   unsigned int k[4][N];
 #pragma unroll
   for (int r = 0; r < N; ++r) {
     if (r < a.K) {
-      const float4 v = ld_f4(reinterpret_cast<const float4*>(a.grad_in + r * a.slot_stride + idx));
+      const int slot = SEL ? a.select[r * a.tv.ntensors + tensor] : r;
+      const float4 v = ld_f4(reinterpret_cast<const float4*>(a.grad_in + slot * a.slot_stride + idx));
       k[0][r] = float_key(v.x); k[1][r] = float_key(v.y); k[2][r] = float_key(v.z); k[3][r] = float_key(v.w);
     } else {
       k[0][r] = k[1][r] = k[2][r] = k[3][r] = 0xFFFFFFFFu;
@@ -109,8 +112,9 @@ __device__ __forceinline__ float4 trimmed_mean_f4(const UpdateArgs& a, long long
 }
 
 // SORT_N: mode 3 only, the sorting-network size (4, 8 or 16 >= K).  Each size is its own instantiation so that a launch pays the
-// registers of its own network (4 x SORT_N keys per thread), not those of the largest one.
-template <int MODE, int SORT_N = 0>
+// registers of its own network (4 x SORT_N keys per thread), not those of the largest one.  SEL: mode 3 only, rows come through
+// the `select` table (DETOX); a separate instantiation, so the launches without a table run the code they always ran.
+template <int MODE, int SORT_N = 0, bool SEL = false>
 __global__ void __launch_bounds__(DRC_THREADS) aggregate_update_kernel(const __grid_constant__ UpdateArgs a) {
   const HyperParams hp = *a.hp;
   const unsigned long long step = *a.step_ptr;
@@ -134,14 +138,15 @@ __global__ void __launch_bounds__(DRC_THREADS) aggregate_update_kernel(const __g
         g.x += v.x; g.y += v.y; g.z += v.z; g.w += v.w;
       }
     } else if (MODE == 2) {
-      const float* wts = reinterpret_cast<const float*>(a.recomb);    // geometric median: sum_k w[tensor][k] * g_k
+      const float* wts = reinterpret_cast<const float*>(a.recomb);    // geometric median: sum_k w[tensor][k] * g_{slot k}
       for (int k = 0; k < a.K; ++k) {
         const float w = wts[tensor * a.K + k];
-        float4 v = ld_f4(reinterpret_cast<const float4*>(a.grad_in + k * a.slot_stride + idx));
+        const int slot = a.select ? a.select[k * a.tv.ntensors + tensor] : k;
+        float4 v = ld_f4(reinterpret_cast<const float4*>(a.grad_in + slot * a.slot_stride + idx));
         g.x = fmaf(w, v.x, g.x); g.y = fmaf(w, v.y, g.y); g.z = fmaf(w, v.z, g.z); g.w = fmaf(w, v.w, g.w);
       }
     } else if constexpr (MODE == 3) {
-      g = trimmed_mean_f4<SORT_N>(a, idx);
+      g = trimmed_mean_f4<SORT_N, SEL>(a, idx, tensor);
     } else {
       for (int k = 0; k < a.K; ++k) {
         const float2 v = a.recomb[tensor * a.K + k];
@@ -203,15 +208,25 @@ __global__ void __launch_bounds__(DRC_THREADS) aggregate_update_kernel(const __g
   }
 }
 
+template <int N>
+static void launch_trimmed_mean(const UpdateArgs* args, int grid, cudaStream_t stream) {
+  if (args->select) aggregate_update_kernel<3, N, true><<<grid, DRC_THREADS, 0, stream>>>(*args);
+  else aggregate_update_kernel<3, N, false><<<grid, DRC_THREADS, 0, stream>>>(*args);
+}
+
 extern "C" int drc_aggregate_update(const UpdateArgs* args, int grid, cudaStream_t stream) {
   if (args->ndst > DRC_MAX_DST || args->flags.n > DRC_MAX_DST) return (int)cudaErrorInvalidValue;
   if (args->mode == 3 && (args->K < 1 || args->K > TRIM_MAXP || args->trim < 0 || 2 * args->trim >= args->K))
     return (int)cudaErrorInvalidValue;
+  // a row table names at most TRIM_MAXP rows under the weighted sum (the weight-space geometric median's limit); the cyclic
+  // recombination reads every worker's slot and has no use for one
+  if (args->select && (args->mode == 1 || (args->mode == 2 && (args->K < 1 || args->K > TRIM_MAXP))))
+    return (int)cudaErrorInvalidValue;
   if (args->mode == 0) aggregate_update_kernel<0><<<grid, DRC_THREADS, 0, stream>>>(*args);
   else if (args->mode == 2) aggregate_update_kernel<2><<<grid, DRC_THREADS, 0, stream>>>(*args);
-  else if (args->mode == 3 && args->K <= 4) aggregate_update_kernel<3, 4><<<grid, DRC_THREADS, 0, stream>>>(*args);
-  else if (args->mode == 3 && args->K <= 8) aggregate_update_kernel<3, 8><<<grid, DRC_THREADS, 0, stream>>>(*args);
-  else if (args->mode == 3) aggregate_update_kernel<3, 16><<<grid, DRC_THREADS, 0, stream>>>(*args);
+  else if (args->mode == 3 && args->K <= 4) launch_trimmed_mean<4>(args, grid, stream);
+  else if (args->mode == 3 && args->K <= 8) launch_trimmed_mean<8>(args, grid, stream);
+  else if (args->mode == 3) launch_trimmed_mean<16>(args, grid, stream);
   else aggregate_update_kernel<1><<<grid, DRC_THREADS, 0, stream>>>(*args);
   return (int)cudaGetLastError();
 }

@@ -150,9 +150,10 @@ extern "C" int drc_geomed_prep(const GeoMedPrepArgs* args, cudaStream_t stream) 
 struct PairDistArgs {
   const float* grad_in;
   long long slot_stride;
-  int P;
+  int P;                          // rows compared per tensor
   TileView tv;
   double* pair_d2;                // [T][P*(P-1)/2] zero on entry; pair (i<j) at j*(j-1)/2 + i
+  const int* rows;                // [P][T] worker slot of row i for tensor t (DETOX: the vote's winner_slot); null -> slot i
 };
 
 __global__ void __launch_bounds__(DRC_THREADS) pair_dist_kernel(const __grid_constant__ PairDistArgs a) {
@@ -167,8 +168,12 @@ __global__ void __launch_bounds__(DRC_THREADS) pair_dist_kernel(const __grid_con
     const bool active = (int)threadIdx.x * 4 < valid;
     float4 v[KRUM_MAXP];
 #pragma unroll
-    for (int i = 0; i < KRUM_MAXP; ++i)
-      if (i < a.P && active) v[i] = ld_f4(reinterpret_cast<const float4*>(a.grad_in + i * a.slot_stride + idx));
+    for (int i = 0; i < KRUM_MAXP; ++i) {
+      if (i < a.P && active) {
+        const int slot = a.rows ? a.rows[i * a.tv.ntensors + tensor] : i;
+        v[i] = ld_f4(reinterpret_cast<const float4*>(a.grad_in + slot * a.slot_stride + idx));
+      }
+    }
 #pragma unroll
     for (int j = 1; j < KRUM_MAXP; ++j) {
 #pragma unroll
@@ -197,6 +202,8 @@ struct KrumSelectArgs {
   int T, P, s;
   int m;                          // slots selected per tensor: 1 = Krum, P - s = multi-Krum
   int* select;                    // [m][T] the m lowest-scoring worker slots, ordered by (score, index)
+  const int* rows;                // [P][T] row -> worker slot (the table pair_dist read) so that `select` holds worker slots;
+                                  // null -> row i is slot i
 };
 
 // Order of distances and scores: ascending with NaN last (what torch.sort / np.sort do), so that a row that sends NaN gets a
@@ -235,12 +242,13 @@ __global__ void krum_select_kernel(const __grid_constant__ KrumSelectArgs a) {
       if (best_i < 0 || less_nan_last(s, best)) { best = s; best_i = i; }
     }
     used |= 1u << best_i;
-    a.select[q * a.T + t] = best_i;
+    a.select[q * a.T + t] = a.rows ? a.rows[best_i * a.T + t] : best_i;
   }
   for (int q = 0; q < npairs; ++q) d2[q] = 0.0;
 }
 
 extern "C" int drc_pair_dist(const PairDistArgs* args, int grid, cudaStream_t stream) {
+  // with or without a row table: at most KRUM_MAXP rows (the pair table of one tensor lives in shared memory)
   if (args->P > KRUM_MAXP) return (int)cudaErrorInvalidValue;
   pair_dist_kernel<<<grid, DRC_THREADS, 0, stream>>>(*args);
   return (int)cudaGetLastError();

@@ -121,11 +121,12 @@ class GeoMedWeightsArgs(C.Structure):
 
 
 class PairDistArgs(C.Structure):
-    _fields_ = [("grad_in", ptr), ("slot_stride", i64), ("P", C.c_int), ("tv", TileView), ("pair_d2", ptr)]
+    _fields_ = [("grad_in", ptr), ("slot_stride", i64), ("P", C.c_int), ("tv", TileView), ("pair_d2", ptr), ("rows", ptr)]
 
 
 class KrumSelectArgs(C.Structure):
-    _fields_ = [("pair_d2", ptr), ("T", C.c_int), ("P", C.c_int), ("s", C.c_int), ("m", C.c_int), ("select", ptr)]
+    _fields_ = [("pair_d2", ptr), ("T", C.c_int), ("P", C.c_int), ("s", C.c_int), ("m", C.c_int), ("select", ptr),
+                ("rows", ptr)]
 
 
 def _maybe_build() -> None:

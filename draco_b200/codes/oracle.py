@@ -134,6 +134,41 @@ def coordinate_median(slots: np.ndarray) -> np.ndarray:
     return trimmed_mean(slots, (np.asarray(slots).shape[0] - 1) // 2)
 
 
+def captured_group_bound(worker_fail: int, group_size: int) -> int:
+    """DETOX's b_G: a group of r >= ``group_size`` members returns a liar's row only when at least (r + 1) // 2 of them lie
+    (fewer leave the honest rows a strict majority, which Boyer-Moore always returns; for even r, r / 2 liars can tie and win),
+    so ``worker_fail`` liars capture at most ``worker_fail // ((group_size + 1) // 2)`` groups."""
+    return worker_fail // ((group_size + 1) // 2)
+
+
+def detox_winner_slots(slots: np.ndarray, groups: Sequence[Sequence[int]]) -> List[int]:
+    """Stage 1 of DETOX: the 0-based worker slot of each group's Boyer-Moore winner (``majority_vote``'s winners)."""
+    _, members = majority_vote(np.asarray(slots), groups)
+    return [int(g[k]) - 1 for g, k in zip(groups, members)]
+
+
+def detox(slots: np.ndarray, groups: Sequence[Sequence[int]], mode: str, b: int) -> np.ndarray:
+    """DETOX (Rajput, Wang, Charles and Papailiopoulos, NeurIPS 2019) on one tensor: majority vote inside every group, then
+    ``mode`` across the G winner rows, with the tolerance b = b_G (``captured_group_bound``) in place of the worker count f:
+
+    * ``coordinate_median``: trim (G - 1) // 2;   * ``trimmed_mean``: trim b;
+    * ``multi_krum``: s = b, averaging G - b rows; * ``geometric_median``: Weiszfeld over the G rows.
+
+    With group size 1 every worker is its own group and this is the baseline rule on the same rows."""
+    X = np.asarray(slots, dtype=np.float64)
+    W = X[detox_winner_slots(slots, groups)]
+    G = W.shape[0]
+    if mode == "coordinate_median":
+        return coordinate_median(W)
+    if mode == "trimmed_mean":
+        return trimmed_mean(W, b)
+    if mode == "multi_krum":
+        return multi_krum(W, b, G - b)
+    if mode == "geometric_median":
+        return geometric_median(W)
+    raise ValueError(f"DETOX has no rule {mode!r}")
+
+
 def sgd_momentum_step(p: np.ndarray, buf: np.ndarray, g: np.ndarray, lr: float, momentum: float,
                       weight_decay: float = 0.0, dampening: float = 0.0, nesterov: bool = False,
                       first_step: bool = False) -> Tuple[np.ndarray, np.ndarray]:

@@ -10,8 +10,9 @@ import argparse
 from dataclasses import asdict, dataclass
 from typing import Optional
 
-APPROACHES = ("baseline", "maj_vote", "cyclic")
+APPROACHES = ("baseline", "maj_vote", "cyclic", "detox")
 MODES = ("normal", "geometric_median", "krum", "maj_vote", "coordinate_median", "trimmed_mean", "multi_krum")
+DETOX_MODES = ("coordinate_median", "trimmed_mean", "multi_krum", "geometric_median")
 ROBUST_MAXP = 16                    # workers the fused coordinate-wise / Krum kernels take (TRIM_MAXP, KRUM_MAXP)
 ERR_MODES = ("rev_grad", "constant", "random", "omniscient", "none")
 TRANSPORTS = ("nvl", "nccl", "nccl_flat", "gloo")
@@ -93,7 +94,7 @@ class JobConfig:
             raise ValueError("cyclic code needs num_workers >= 2*worker_fail + 1")
         if self.approach == "cyclic" and 2 * self.worker_fail + 1 > 8:
             raise ValueError("cyclic code: redundancy 2*worker_fail + 1 is limited to 8 (DRC_MAX_R)")
-        if self.approach == "maj_vote" and self.num_workers >= self.group_size > 0:
+        if self.approach in ("maj_vote", "detox") and self.num_workers >= self.group_size > 0:
             # all remainder workers join the last group (codes/repetition.py): it can hold up to 2r-1 members, the vote kernel 8
             largest = self.group_size + self.num_workers % self.group_size
             if largest > 8:
@@ -113,6 +114,8 @@ class JobConfig:
             if self.transport == "nvl" and P > ROBUST_MAXP:
                 raise ValueError(f"--mode {self.mode} on the nvl transport handles at most {ROBUST_MAXP} workers (got {P}); "
                                  f"use --transport nccl for more")
+        if self.approach == "detox":
+            self._check_detox()
         if self.compress and self.transport == "nvl" and self.err_mode == "omniscient":
             raise ValueError("--err-mode omniscient reads the honest slots in PS memory while they arrive; with --compress-grad "
                              "compress they only exist after the PS unpacked them -- pass --compress-grad None")
@@ -123,6 +126,25 @@ class JobConfig:
             self.cuda_graphs = False
         return self
 
+    def _check_detox(self) -> None:
+        """DETOX runs the robust rule across the G group winners, tolerating b_G captured groups in place of f liars."""
+        if self.mode not in DETOX_MODES:
+            raise ValueError(f"--approach detox takes --mode {' | '.join(DETOX_MODES)} (the rule applied across the group "
+                             f"winners), got --mode {self.mode}")
+        if not 1 <= self.group_size <= self.num_workers:
+            raise ValueError(f"--approach detox needs 1 <= group_size <= num_workers (got group_size {self.group_size}, "
+                             f"{self.num_workers} workers)")
+        G, b = self.num_groups, self.captured_group_bound
+        if self.mode == "multi_krum" and G <= 2 * b + 2:
+            raise ValueError(f"--approach detox --mode multi_krum needs groups > 2*b_G + 2 (Krum's condition over the group "
+                             f"winners; got {G} groups, b_G = worker_fail // ceil(group_size / 2) = {b})")
+        if self.mode != "multi_krum" and 2 * b >= G:
+            raise ValueError(f"--approach detox --mode {self.mode} needs groups > 2*b_G (got {G} groups, b_G = worker_fail // "
+                             f"ceil(group_size / 2) = {b} groups the liars can capture)")
+        if self.transport == "nvl" and G > ROBUST_MAXP:
+            raise ValueError(f"--approach detox on the nvl transport handles at most {ROBUST_MAXP} groups (got {G}); use a larger "
+                             f"--group-size or --transport nccl")
+
     @property
     def compress(self) -> bool:
         return self.compress_grad == "compress"
@@ -131,9 +153,20 @@ class JobConfig:
     def redundancy(self) -> int:
         if self.approach == "cyclic":
             return 2 * self.worker_fail + 1
-        if self.approach == "maj_vote":
+        if self.approach in ("maj_vote", "detox"):
             return self.group_size
         return 1
+
+    @property
+    def num_groups(self) -> int:
+        """Repetition groups G of ``maj_vote`` / ``detox``: num_workers // group_size (the remainder joins the last group)."""
+        return self.num_workers // min(self.group_size, self.num_workers)
+
+    @property
+    def captured_group_bound(self) -> int:
+        """DETOX's b_G = worker_fail // ceil(group_size / 2): a group of r >= group_size members returns a liar's row only when
+        at least (r + 1) // 2 of them lie, so the liars capture at most b_G groups."""
+        return self.worker_fail // ((self.group_size + 1) // 2)
 
     @property
     def attack_magnitude(self) -> float:
@@ -167,12 +200,16 @@ def add_fit_args(parser: argparse.ArgumentParser) -> argparse.ArgumentParser:
     a("--network", type=str, default=d.network)
     a("--mode", type=str, default=d.mode,
       help="normal | geometric_median | krum | coordinate_median | trimmed_mean | multi_krum (baseline); normal | maj_vote "
-           "(maj_vote).  trimmed_mean drops --worker-fail values at each end of every coordinate; multi_krum averages the "
-           "num_workers - worker_fail workers with the lowest Krum scores")
+           "(maj_vote); coordinate_median | trimmed_mean | multi_krum | geometric_median (detox: the rule across the group "
+           "winners).  trimmed_mean drops --worker-fail values at each end of every coordinate (detox: b_G = worker_fail // "
+           "ceil(group_size / 2)); multi_krum averages the num_workers - worker_fail workers (detox: G - b_G group winners) with "
+           "the lowest Krum scores")
     a("--dataset", type=str, default=d.dataset)
     a("--comm-type", type=str, default=d.comm_type)
     a("--err-mode", type=str, default=d.err_mode, help="rev_grad | constant | random | omniscient | none")
-    a("--approach", type=str, default=d.approach, help="baseline | maj_vote | cyclic")
+    a("--approach", type=str, default=d.approach,
+      help="baseline | maj_vote | cyclic | detox (majority vote inside each repetition group, then --mode across the G group "
+           "winners)")
     a("--num-aggregate", type=int, default=d.num_aggregate)
     a("--eval-freq", type=int, default=d.eval_freq)
     a("--train-dir", type=str, default=d.train_dir)

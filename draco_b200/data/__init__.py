@@ -131,11 +131,11 @@ def augment_cifar(x_u8: torch.Tensor, seed: int) -> torch.Tensor:
 class BatchPlan:
     """Maps (step, worker rank) to dataset indices for one approach."""
 
-    approach: str                 # baseline | maj_vote | cyclic
+    approach: str                 # baseline | maj_vote | cyclic | detox
     dataset_size: int
     batch_size: int
     num_workers: int
-    group_of: Optional[dict] = None          # rank -> group id (maj_vote)
+    group_of: Optional[dict] = None          # rank -> group id (maj_vote, detox)
     group_seeds: Optional[List[int]] = None
     seed: int = 428
     redundancy: int = 1                       # cyclic: 2s+1
@@ -164,7 +164,7 @@ class BatchPlan:
         B = self.batch_size
         if self.approach == "baseline":
             return [self._slice(self._perm(self.seed * 1000003 + rank * 7919 + epoch), pos, B)]
-        if self.approach == "maj_vote":
+        if self.approach in ("maj_vote", "detox"):
             gseed = self.group_seeds[self.group_of[rank]]
             return [self._slice(self._perm(gseed + epoch), pos, B)]
         if self.approach == "cyclic":
@@ -177,6 +177,6 @@ class BatchPlan:
         """Identity of each sub-batch (used to seed dropout / augmentation identically across holders)."""
         if self.approach == "cyclic":
             return [int(j) for j in (rank - 1 + np.arange(self.redundancy)) % self.num_workers]
-        if self.approach == "maj_vote":
+        if self.approach in ("maj_vote", "detox"):
             return [int(self.group_of[rank])]
         return [int(rank)]

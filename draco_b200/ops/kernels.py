@@ -129,6 +129,19 @@ def vote(layout: ArenaLayout, grad_in: Addr, slot_stride: int, group_table: torc
 
 
 # ------------------------------------------------------------------------------------------------ update (K7/K8/K9)
+ROW_TABLE_MAXROWS = 16
+
+
+def _check_row_table(layout: ArenaLayout, table, rows: int) -> None:
+    """A row table of the trimmed mean, the weighted sum, pair distances or Krum: a contiguous int32 CUDA tensor [rows, T] with
+    1 <= rows <= 16 (the kernels read entry (k, t) at k * T + t)."""
+    T = layout.ntensors
+    if not isinstance(table, torch.Tensor) or table.dtype != torch.int32 or not table.is_cuda or not table.is_contiguous():
+        raise ValueError("row table: expected a contiguous int32 CUDA tensor")
+    if tuple(table.shape) != (rows, T) or not 1 <= rows <= ROW_TABLE_MAXROWS:
+        raise ValueError(f"row table: expected shape ({rows}, {T}) with at most {ROW_TABLE_MAXROWS} rows, got {tuple(table.shape)}")
+
+
 def aggregate_update(layout: ArenaLayout, grad_in: Addr, slot_stride: int, *, params: Addr, momentum: Addr, hp: Addr,
                      step_ptr: Addr, done_counter: Addr, K: int, scale: float, select: Addr = None,
                      recomb: Addr = None, first_step: int = 1, grad_out: Addr = None, mc_params: Addr = None,
@@ -136,16 +149,24 @@ def aggregate_update(layout: ArenaLayout, grad_in: Addr, slot_stride: int, *, pa
                      tile_range: Optional[tuple] = None, weights: Addr = None, exp_avg_sq: Addr = None,
                      max_exp_avg_sq: Addr = None, trim: Optional[int] = None) -> None:
     """Fused aggregate (select-sum, cyclic recombination, real per-tensor ``weights`` [T, K], or -- with ``trim`` -- the
-    coordinate-wise trimmed mean of rows 0..K-1 that drops ``trim`` values at each end, K <= 16) + optimizer step (SGD-momentum, or
+    coordinate-wise trimmed mean of K <= 16 rows that drops ``trim`` values at each end) + optimizer step (SGD-momentum, or
     Adam / AMSGrad when the hyper-parameter block says so: ``momentum`` = first moment, ``exp_avg_sq`` / ``max_exp_avg_sq`` = second
-    moment / its running maximum) + parameter broadcast + flags."""
+    moment / its running maximum) + parameter broadcast + flags.
+
+    ``select``: int32 [K, T] table of the worker slot that row k of tensor t is read from (rows 0..K-1 when None).  It applies to
+    the select-sum, to the ``weights`` sum and to the trimmed mean; DETOX passes the vote's ``winner_slot`` so that the rule runs
+    on the group winners."""
     a = N.UpdateArgs()
     a.mode = 1 if recomb is not None else (2 if weights is not None else 0)
     if weights is not None:
-        assert recomb is None and select is None
+        assert recomb is None
+        if select is not None:
+            _check_row_table(layout, select, K)
         recomb = weights
     if trim is not None:
-        assert recomb is None and select is None
+        assert recomb is None
+        if select is not None:
+            _check_row_table(layout, select, K)
         if not (1 <= K <= 16 and 0 <= 2 * trim < K):
             raise ValueError(f"trimmed mean: K = {K} rows (at most 16) must exceed 2 * trim = {2 * trim}")
         if abs(scale * (K - 2 * trim) - 1.0) > 1e-6:
@@ -289,13 +310,16 @@ GEOMED_FAST_MAXP = 16
 
 def geometric_median_weights(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, pair_d2: torch.Tensor,
                              weights: torch.Tensor, max_iter: int = 256, eps: float = 1e-10,
-                             iters_out: Optional[torch.Tensor] = None) -> torch.Tensor:
+                             iters_out: Optional[torch.Tensor] = None, rows: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Per-tensor geometric median as convex weights: ``median_t = sum_i weights[t, i] * slot_i`` (Weiszfeld run in weight
     space from the pairwise distances -- one pass over the slab; see csrc/cuda/robust.cu).  ``pair_d2``: zeroed fp64
-    [T, P(P-1)/2] scratch (left zeroed); ``weights``: fp32 [T, P] out."""
+    [T, P(P-1)/2] scratch (left zeroed); ``weights``: fp32 [T, P] out.  ``rows``: optional int32 [P, T] table, row i of tensor t
+    is worker slot ``rows[i, t]`` (the weights stay in row space: pass the same table to ``aggregate_update(select=)``)."""
     assert P <= GEOMED_FAST_MAXP
+    if rows is not None:
+        _check_row_table(layout, rows, P)
     lib = N.cuda()
-    pa = N.PairDistArgs(addr(grad_in), slot_stride, P, layout.tile_view(weights.device), pair_d2.data_ptr())
+    pa = N.PairDistArgs(addr(grad_in), slot_stride, P, layout.tile_view(weights.device), pair_d2.data_ptr(), addr(rows))
     N.check(lib.drc_pair_dist(C.byref(pa), stream_grid(layout, 4), _stream()), "pair_dist")
     wa = N.GeoMedWeightsArgs(pair_d2.data_ptr(), layout.ntensors, P, max_iter, eps, weights.data_ptr(),
                              iters_out.data_ptr() if iters_out is not None else None)
@@ -304,14 +328,17 @@ def geometric_median_weights(layout: ArenaLayout, grad_in: Addr, slot_stride: in
 
 
 def krum_select(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, s: int, pair_d2: torch.Tensor,
-                select: torch.Tensor, m: int = 1) -> None:
+                select: torch.Tensor, m: int = 1, rows: Optional[torch.Tensor] = None) -> None:
     """``pair_d2``: zeroed fp64 [T, P*(P-1)/2] scratch (left zeroed); ``select``: int32 [m, T] out, the ``m`` lowest Krum scores
-    per tensor ordered by (score, slot) -- ``m = 1``: the Krum winner, ``m = P - s``: multi-Krum (int32 [T] is fine for m = 1)."""
+    per tensor ordered by (score, slot) -- ``m = 1``: the Krum winner, ``m = P - s``: multi-Krum (int32 [T] is fine for m = 1).
+    ``rows``: optional int32 [P, T] table, row i of tensor t is worker slot ``rows[i, t]``; ``select`` then holds worker slots."""
     assert 1 <= m <= P and select.numel() >= m * layout.ntensors
+    if rows is not None:
+        _check_row_table(layout, rows, P)
     lib = N.cuda()
-    pa = N.PairDistArgs(addr(grad_in), slot_stride, P, layout.tile_view(select.device), pair_d2.data_ptr())
+    pa = N.PairDistArgs(addr(grad_in), slot_stride, P, layout.tile_view(select.device), pair_d2.data_ptr(), addr(rows))
     N.check(lib.drc_pair_dist(C.byref(pa), stream_grid(layout, 4), _stream()), "pair_dist")
-    ka = N.KrumSelectArgs(pair_d2.data_ptr(), layout.ntensors, P, s, m, select.data_ptr())
+    ka = N.KrumSelectArgs(pair_d2.data_ptr(), layout.ntensors, P, s, m, select.data_ptr(), addr(rows))
     N.check(lib.drc_krum_select(C.byref(ka), _stream()), "krum_select")
 
 

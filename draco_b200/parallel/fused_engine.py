@@ -11,7 +11,8 @@ Step anatomy (one PS + P logical workers hosted by ``nprocs`` GPU processes; see
                                                                  wait_flags(grad_ready[*] >= t)
                                                                  vote | project+locate | (multi-)krum | geomedian   (decode)
     params arena  <------ multimem.st / peer stores  ----------  aggregate_update: SGD-momentum + broadcast
-                                                                 (coordinate median / trimmed mean: sorted inside it)
+                                                                 (coordinate median / trimmed mean: sorted inside it;
+                                                                  detox: vote, then the rule across the group winners)
     flag params_ready = t+1  <---------------------------------  (last CTA)
 
 There is no NCCL / MPI call and no host synchronisation anywhere in that loop; ordering between GPUs is carried by
@@ -40,7 +41,7 @@ from ..ops import kernels as K
 from ..utils.metrics import PhaseTimer, limit_host_threads, wait_event
 from .arena import ArenaLayout
 from .placement import Placement
-from .ps import FusedPS, build_codes, select_rule
+from .ps import PIPELINED_RULES, FusedPS, build_codes, select_rule
 from .symm import SymmContext
 from .worker import WorkerCompute, make_model
 
@@ -80,7 +81,7 @@ class FusedEngine:
         self.compress = bool(cfg.compress)
         self.overlap_push = cfg.overlap_push and not self.cyclic and not self.compress
         # PS pipelining: decode + apply + broadcast each gradient bucket as soon as all workers pushed it
-        self.pipeline_ps = (self.overlap_push and cfg.pipeline_ps and select_rule(cfg) in ("mean", "vote", "median", "trimmed_mean")
+        self.pipeline_ps = (self.overlap_push and cfg.pipeline_ps and select_rule(cfg) in PIPELINED_RULES
                             and cfg.err_mode != "omniscient")
         self.push_stream = torch.cuda.Stream(device=device) if self.overlap_push else None
         ns = min(max(int(cfg.worker_streams), 1), len(self.local_workers))

@@ -27,18 +27,34 @@ def select_rule(cfg: JobConfig) -> str:
     """Aggregation rule of a job.  Mirrors the reference's dispatch: cyclic approach -> Fourier decode
     (cyclic_master.py:24); maj_vote approach -> vote only when ``--mode maj_vote``, plain mean for ``--mode normal``
     (rep_master.py:118-129); baseline approach -> mean / geometric median / Krum by ``--mode`` (baseline_master.py:118-129), plus
-    three rules beyond the reference: coordinate-wise median, coordinate-wise trimmed mean and multi-Krum."""
+    three rules beyond the reference: coordinate-wise median, coordinate-wise trimmed mean and multi-Krum.  The detox approach
+    (beyond the reference too) votes inside every group and runs ``--mode`` across the group winners: ``detox_*`` rules."""
     if cfg.approach == "cyclic":
         return "cyclic"
     if cfg.approach == "maj_vote":
         return "vote" if cfg.mode == "maj_vote" else "mean"
+    if cfg.approach == "detox":
+        return DETOX_RULES[cfg.mode]
     return {"normal": "mean", "geometric_median": "geomedian", "krum": "krum", "coordinate_median": "median",
             "trimmed_mean": "trimmed_mean", "multi_krum": "multi_krum"}.get(cfg.mode, "mean")
+
+
+DETOX_RULES = {"coordinate_median": "detox_median", "trimmed_mean": "detox_trimmed_mean", "multi_krum": "detox_multi_krum",
+               "geometric_median": "detox_geomedian"}
 
 
 def coordinate_trim(cfg: JobConfig) -> int:
     """Values dropped at each end of every coordinate: (P - 1) // 2 for the median, ``--worker-fail`` for the trimmed mean."""
     return (cfg.num_workers - 1) // 2 if select_rule(cfg) == "median" else cfg.worker_fail
+
+
+# rules the fused PS applies bucket by bucket while the workers still push (nothing in them needs the whole tensor at once)
+PIPELINED_RULES = ("mean", "vote", "median", "trimmed_mean", "detox_median", "detox_trimmed_mean")
+
+
+def detox_trim(cfg: JobConfig) -> int:
+    """DETOX's ``coordinate_trim`` over the G group winners: (G - 1) // 2 for the median, b_G for the trimmed mean."""
+    return (cfg.num_groups - 1) // 2 if select_rule(cfg) == "detox_median" else cfg.captured_group_bound
 
 
 def multi_krum_m(cfg: JobConfig) -> int:
@@ -75,12 +91,23 @@ class FusedPS:
         self.cyclic = cfg.approach == "cyclic"
         self.slot_stride = layout.total
         self.rule = select_rule(cfg)
-        if self.rule == "vote":
+        if self.rule == "vote" or self.rule.startswith("detox"):
             self.group_table = torch.from_numpy(groups.as_table()).to(device)
             G = self.group_table.shape[0]
             self.neq_mask = torch.zeros(G, T, dtype=torch.int32, device=device)
             self.winner_slot = torch.zeros(G, T, dtype=torch.int32, device=device)
             self.winner_member = torch.zeros(G, T, dtype=torch.int32, device=device)
+        # DETOX: the rule runs on the G rows the vote's winner_slot table names, inside the kernels that read the slab anyway
+        if self.rule in ("detox_median", "detox_trimmed_mean"):
+            self.trim = detox_trim(cfg)
+        elif self.rule == "detox_multi_krum":
+            self.b = cfg.captured_group_bound
+            self.m = G - self.b
+            self.pair_d2 = torch.zeros(T, G * (G - 1) // 2, dtype=torch.float64, device=device)
+            self.select = torch.zeros(self.m, T, dtype=torch.int32, device=device)
+        elif self.rule == "detox_geomedian":
+            self.pair_d2 = torch.zeros(T, G * (G - 1) // 2, dtype=torch.float64, device=device)
+            self.gm_weights = torch.zeros(T, G, dtype=torch.float32, device=device)
         elif self.rule == "krum":
             self.pair_d2 = torch.zeros(T, self.P * (self.P - 1) // 2, dtype=torch.float64, device=device)
             self.select = torch.zeros(T, dtype=torch.int32, device=device)
@@ -126,18 +153,22 @@ class FusedPS:
                       hp=self.hp, step_ptr=step_ptr,
                       done_counter=self.counters[0:1], first_step=1, grad_out=grad_out, mc_params=mc_params, dst=dst)
         n = 0
-        if buckets is not None and self.rule in ("mean", "vote", "median", "trimmed_mean"):
+        if buckets is not None and self.rule in PIPELINED_RULES:
             for bi, (t0, t1, idxs) in enumerate(buckets):
                 n += wait_bucket(bi)
                 fl = flags if bi == len(buckets) - 1 else []
-                if self.rule == "vote":
+                if self.rule in ("vote", "detox_median", "detox_trimmed_mean"):
                     K.vote(L, self.grad_in, self.slot_stride, self.group_table, self.neq_mask, self.winner_slot,
                            self.winner_member, tile_range=(t0, t1), tensor_range=(min(idxs), max(idxs) + 1)); n += 2
                     G = self.group_table.shape[0]
                     if bi == len(buckets) - 1:
                         n += before_update()
-                    K.aggregate_update(L, self.grad_in, self.slot_stride, K=G, scale=1.0 / G, select=self.winner_slot,
-                                       tile_range=(t0, t1), flags=fl, **common); n += 1
+                    if self.rule == "vote":
+                        K.aggregate_update(L, self.grad_in, self.slot_stride, K=G, scale=1.0 / G, select=self.winner_slot,
+                                           tile_range=(t0, t1), flags=fl, **common); n += 1
+                    else:                                  # DETOX: the coordinate-wise rule across the bucket's group winners
+                        K.aggregate_update(L, self.grad_in, self.slot_stride, K=G, scale=1.0 / (G - 2 * self.trim), trim=self.trim,
+                                           select=self.winner_slot, tile_range=(t0, t1), flags=fl, **common); n += 1
                 elif self.rule == "mean":
                     if bi == len(buckets) - 1:
                         n += before_update()
@@ -162,6 +193,18 @@ class FusedPS:
             K.vote(L, self.grad_in, self.slot_stride, self.group_table, self.neq_mask, self.winner_slot, self.winner_member); n += 2
             G = self.group_table.shape[0]
             _update(L, self.grad_in, self.slot_stride, K=G, scale=1.0 / G, select=self.winner_slot, **common); n += 1
+        elif self.rule.startswith("detox"):
+            K.vote(L, self.grad_in, self.slot_stride, self.group_table, self.neq_mask, self.winner_slot, self.winner_member); n += 2
+            G, win = self.group_table.shape[0], self.winner_slot
+            if self.rule == "detox_multi_krum":          # select holds the worker slots of the m best winners
+                K.krum_select(L, self.grad_in, self.slot_stride, G, self.b, self.pair_d2, self.select, m=self.m, rows=win); n += 2
+                _update(L, self.grad_in, self.slot_stride, K=self.m, scale=1.0 / self.m, select=self.select, **common); n += 1
+            elif self.rule == "detox_geomedian":         # weights in row space, applied through the same winner table
+                K.geometric_median_weights(L, self.grad_in, self.slot_stride, G, self.pair_d2, self.gm_weights, rows=win); n += 2
+                _update(L, self.grad_in, self.slot_stride, K=G, scale=1.0, weights=self.gm_weights, select=win, **common); n += 1
+            else:
+                _update(L, self.grad_in, self.slot_stride, K=G, scale=1.0 / (G - 2 * self.trim), trim=self.trim, select=win,
+                        **common); n += 1
         elif self.rule == "krum":
             K.krum_select(L, self.grad_in, self.slot_stride, self.P, self.cfg.worker_fail, self.pair_d2, self.select); n += 2
             _update(L, self.grad_in, self.slot_stride, K=1, scale=1.0, select=self.select, **common); n += 1
@@ -211,6 +254,8 @@ class TorchPS:
             f = (torch.randn(layout.total, generator=g) + 1.0) * torch.from_numpy(layout.valid_mask()).float()
             self.f = f.to(device)
         self.trim = coordinate_trim(cfg) if self.rule in ("median", "trimmed_mean") else 0
+        if self.rule in ("detox_median", "detox_trimmed_mean"):
+            self.trim = detox_trim(cfg)
         self.last_info: Dict[str, object] = {}
 
     # --- optimizer state for checkpoints (the reference saves none: src/master/baseline_master.py:237-243) ----------
@@ -292,19 +337,18 @@ class TorchPS:
                 break
         return m
 
-    def _krum_scores(self, X: torch.Tensor) -> torch.Tensor:
+    def _krum_scores(self, X: torch.Tensor, s: int) -> torch.Tensor:
         d2 = torch.cdist(X.double(), X.double()).pow(2)
         P = X.shape[0]
-        keep = max(P - self.cfg.worker_fail - 2, 0)
+        keep = max(P - s - 2, 0)
         d2 = d2 + torch.diag(torch.full((P,), float("inf"), dtype=d2.dtype, device=d2.device))
         return d2.sort(dim=1).values[:, :keep].sum(1)
 
     def _krum_tensor(self, X: torch.Tensor) -> int:
-        return int(torch.argsort(self._krum_scores(X), stable=True)[0])      # NaN scores last, like the kernel
+        return int(torch.argsort(self._krum_scores(X, self.cfg.worker_fail), stable=True)[0])      # NaN scores last, like the kernel
 
-    def _multi_krum_tensor(self, X: torch.Tensor) -> torch.Tensor:
-        m = multi_krum_m(self.cfg)
-        best = torch.argsort(self._krum_scores(X), stable=True)[:m]
+    def _multi_krum_tensor(self, X: torch.Tensor, s: int, m: int) -> torch.Tensor:
+        best = torch.argsort(self._krum_scores(X, s), stable=True)[:m]
         return X[best].sum(0) / m
 
     def _trimmed_mean_tensor(self, X: torch.Tensor) -> torch.Tensor:
@@ -346,11 +390,24 @@ class TorchPS:
             elif self.rule == "krum":
                 g = X[self._krum_tensor(X)]
             elif self.rule == "multi_krum":
-                g = self._multi_krum_tensor(X)
+                g = self._multi_krum_tensor(X, self.cfg.worker_fail, multi_krum_m(self.cfg))
             elif self.rule in ("median", "trimmed_mean"):
                 g = self._trimmed_mean_tensor(X)
             elif self.rule == "geomedian":
                 g = self._geomedian_tensor(X)
+            elif self.rule.startswith("detox"):
+                winners = []                               # stage 1: the vote inside every group
+                for grp in self.groups.groups:
+                    rows = [X[w - 1] for w in grp]
+                    winners.append(rows[self._vote_tensor(rows)])
+                W = torch.stack(winners)                   # stage 2: the rule across the G winners
+                if self.rule == "detox_multi_krum":
+                    b = self.cfg.captured_group_bound
+                    g = self._multi_krum_tensor(W, b, W.shape[0] - b)
+                elif self.rule == "detox_geomedian":
+                    g = self._geomedian_tensor(W)
+                else:
+                    g = self._trimmed_mean_tensor(W)
             elif self.rule == "cyclic":
                 g = self._cyclic_tensor(X, self.f[spec.offset: spec.offset + spec.numel])
             else:
@@ -363,13 +420,15 @@ class TorchPS:
 
     def apply(self, grads: List[torch.Tensor]) -> None:
         mode = {"mean": "normal", "vote": "maj_vote", "krum": "krum", "geomedian": "geometric_median", "cyclic": "cyclic",
-                "median": "coordinate_median", "trimmed_mean": "trimmed_mean", "multi_krum": "multi_krum"}[self.rule]
+                "median": "coordinate_median", "trimmed_mean": "trimmed_mean", "multi_krum": "multi_krum",
+                "detox_median": "coordinate_median", "detox_trimmed_mean": "trimmed_mean", "detox_multi_krum": "multi_krum",
+                "detox_geomedian": "geometric_median"}[self.rule]
         self.optimizer.step(grads=grads, mode=mode)
 
 
 def build_codes(cfg: JobConfig):
     """(GroupPlan | None, CyclicCode | None) for a job -- the coding part of the reference's ``prepare``."""
     from ..codes.repetition import group_assign
-    groups = group_assign(cfg.num_workers, cfg.group_size) if cfg.approach == "maj_vote" else None
+    groups = group_assign(cfg.num_workers, cfg.group_size) if cfg.approach in ("maj_vote", "detox") else None
     code = search_w(cfg.num_workers, cfg.worker_fail) if cfg.approach == "cyclic" else None
     return groups, code

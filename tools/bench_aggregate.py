@@ -1,12 +1,14 @@
 """Time the fused PS update kernel alone (csrc/cuda/aggregate_update.cu): mode 0, the mean of P gradient rows, against mode 3,
-the coordinate-wise trimmed mean and median, on the ResNet-18 (CIFAR) parameter arena.
+the coordinate-wise trimmed mean and median, on the ResNet-18 (CIFAR) parameter arena.  With a G-row winner table (DETOX: the
+majority vote's winner slot per group and tensor, here drawn at random from groups of 3) it times mode 0, the average of the G
+winners that ``--approach maj_vote`` applies, against mode 3 over the same G rows: the median and the b_G-trimmed mean.
 
 Each call reads the P x D fp32 gradient slab once and reads + writes the fp32 parameters and momentum (SGD-momentum, no
 broadcast destinations).  Timed with CUDA events over --iters back-to-back launches; the rules alternate over --rounds and the
 median round is reported.  Bandwidth is the slab bytes (P * D * 4) per microsecond, also as a share of the H100 SXM data-sheet
 HBM3 bandwidth of 3.35 TB/s (3.35e6 bytes/us); ``total_bytes_per_us`` adds the 16 * D bytes of parameter / momentum traffic.
 
-    python tools/bench_aggregate.py [--workers 7 16] [--iters 200] [--rounds 3] [--out FILE]
+    python tools/bench_aggregate.py [--workers 7 16] [--groups 3 5 8] [--iters 200] [--rounds 3] [--out FILE]
 """
 from __future__ import annotations
 
@@ -38,6 +40,8 @@ def main() -> int:
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--workers", type=int, nargs="+", default=[7, 16])
     ap.add_argument("--trim", type=int, default=2, help="values dropped at each end by the trimmed mean (= --worker-fail)")
+    ap.add_argument("--groups", type=int, nargs="*", default=[3, 5, 8], help="G of the winner-table rows (groups of 3 workers)")
+    ap.add_argument("--group-trim", type=int, default=1, help="b_G of the DETOX trimmed mean (worker_fail 3, group size 3: 1)")
     ap.add_argument("--iters", type=int, default=200)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--out", type=str, default=None, help="also append the JSON lines to this file")
@@ -63,11 +67,21 @@ def main() -> int:
     step = torch.full((1,), 2, dtype=torch.int64, device=dev)
     cnt = torch.zeros(4, dtype=torch.int32, device=dev)
     lines = [dict(gpu_info(), arena="ResNet18/Cifar10", D=D, iters=a.iters, rounds=a.rounds)]
+    cases = []
     for P in a.workers:
+        cases.append((dict(P=P), P, {"mean": dict(K=P, scale=1.0 / P),
+                                     f"trimmed_mean_b{a.trim}": dict(K=P, scale=1.0 / (P - 2 * a.trim), trim=a.trim),
+                                     "median": dict(K=P, scale=1.0 / (P - 2 * ((P - 1) // 2)), trim=(P - 1) // 2)}))
+    T = L.ntensors
+    for G in a.groups:
+        win = (torch.arange(G, device=dev)[:, None] * 3 + torch.randint(0, 3, (G, T), device=dev)).to(torch.int32).contiguous()
+        b = a.group_trim
+        cases.append((dict(G=G, P=3 * G), 3 * G, {"vote_mean": dict(K=G, scale=1.0 / G, select=win),
+                                                  f"detox_trimmed_mean_b{b}": dict(K=G, scale=1.0 / (G - 2 * b), trim=b, select=win),
+                                                  "detox_median": dict(K=G, scale=1.0 / (G - 2 * ((G - 1) // 2)), trim=(G - 1) // 2,
+                                                                       select=win)}))
+    for key, P, rules in cases:
         slab = torch.randn(P, D, device=dev) * 1e-3
-        rules = {"mean": dict(K=P, scale=1.0 / P),
-                 f"trimmed_mean_b{a.trim}": dict(K=P, scale=1.0 / (P - 2 * a.trim), trim=a.trim),
-                 "median": dict(K=P, scale=1.0 / (P - 2 * ((P - 1) // 2)), trim=(P - 1) // 2)}
 
         def launch(kw):
             K.aggregate_update(L, slab, D, params=params, momentum=mom, hp=hp, step_ptr=step, done_counter=cnt[0:1], **kw)
@@ -86,10 +100,11 @@ def main() -> int:
                 e.record()
                 e.synchronize()
                 times[name].append(s.elapsed_time(e) * 1e3 / a.iters)
-        slab_bytes = P * D * 4
         for name, ts in times.items():
+            rows = rules[name]["K"]                                # rows read per coordinate: P, or the G winners
+            slab_bytes = rows * D * 4
             us = sorted(ts)[len(ts) // 2]
-            lines.append({"P": P, "rule": name, "mode": 0 if name == "mean" else 3, "us_per_call": round(us, 2),
+            lines.append({**key, "rule": name, "mode": 3 if "trim" in rules[name] else 0, "us_per_call": round(us, 2),
                           "us_rounds": [round(t, 2) for t in ts], "slab_bytes": slab_bytes,
                           "slab_bytes_per_us": round(slab_bytes / us), "slab_share_of_3.35TBps": round(slab_bytes / us / HBM_BYTES_PER_US, 3),
                           "total_bytes_per_us": round((slab_bytes + 16 * D) / us)})
