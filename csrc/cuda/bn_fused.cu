@@ -213,7 +213,9 @@ __global__ void __launch_bounds__(BN_THREADS, 2) bn_stats_kernel(const BnFwdArgs
       a.mean[c] = m;
       a.invstd[c] = rsqrtf(var + a.eps);
       if (a.running_mean) {
-        const float unbiased = a.M > 1 ? var * ((float)a.M / (float)(a.M - 1)) : var;
+        // __fmul_rn: rounded on its own, never contracted into the fma below (the conv epilogue's finalisation does the same,
+        // so both paths update the running variance bit-identically)
+        const float unbiased = a.M > 1 ? __fmul_rn(var, (float)a.M / (float)(a.M - 1)) : var;
         a.running_mean[c] = fmaf(a.momentum, m - a.running_mean[c], a.running_mean[c]);
         a.running_var[c] = fmaf(a.momentum, unbiased - a.running_var[c], a.running_var[c]);
       }

@@ -300,7 +300,9 @@ __device__ __forceinline__ void finalize_stats(const BnStatArgs& st, float* s_st
     st.mean[c] = m;
     st.invstd[c] = rsqrtf(var + st.eps);
     if (st.running_mean) {
-      const float unbiased = st.count > 1 ? var * ((float)st.count / (float)(st.count - 1)) : var;
+      // __fmul_rn: rounded on its own, never contracted into the fma below (bn_fused.cu's finalisation does the same, so the
+      // epilogue and the standalone statistics kernel update the running variance bit-identically)
+      const float unbiased = st.count > 1 ? __fmul_rn(var, (float)st.count / (float)(st.count - 1)) : var;
       st.running_mean[c] = fmaf(st.momentum, m - st.running_mean[c], st.running_mean[c]);
       st.running_var[c] = fmaf(st.momentum, unbiased - st.running_var[c], st.running_var[c]);
     }

@@ -1,0 +1,248 @@
+"""Exact and component-wise references for the tensor-core GEMM / convolution kernels and the BatchNorm statistics.
+
+Integer operands.  Operands drawn from {-1, 0, +1} make every bf16 x bf16 product exact and every partial sum an integer; as
+long as no partial sum exceeds 2^24 in magnitude, every fp32 sum of them is exact in ANY order, on any tile, split-K or cluster
+plan.  A bf16 output must then equal ``bf16_rn(exact)`` bit for bit, and one reference checks every kernel variant with
+``torch.equal``.  The magnitude of a sum of K terms is at most K (< 2^24 for every layer here); ``int_operand`` additionally
+draws the nonzeros with a density p such that the expected number of nonzero products K * p^2 stays near ``target`` (2^11 by
+default), far below 2^24, as a margin against reduced-precision adders inside the tensor core.
+
+Component-wise bound.  For real-valued data a kernel that accumulates K exact products in fp32 (round-to-nearest, or
+round-toward-zero adders: relative error <= 2^-23 per addition) and rounds the result once to bf16 (relative error <= 2^-9)
+satisfies, element by element,
+
+    |y - ref64| <= 2^-8 * |ref64| + gamma * (|x| (*) |w|),   gamma = (K + 1) * 2^-23,
+
+where (*) is the same operation applied to the absolute values in fp64 (the standard dot-product bound with a factor 2 of slack
+in each term; the +1 covers a bias or residual added before rounding).  ``check_bound`` reports the worst element with its index.
+
+References are computed in fp64 (exact for integer data), by the tap decomposition the kernels use: a k x k convolution is the
+sum over its taps of one [pixels, Cin] x [Cin, Cout] product each; dgrad is the adjoint (scatter of the same slices), wgrad the
+product of dy^T with the same slices.
+"""
+from __future__ import annotations
+
+import math
+
+import torch
+
+FP32_EXACT = 2 ** 24          # every integer of magnitude <= 2^24 is an fp32
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# operands
+# ---------------------------------------------------------------------------------------------------------------------
+def density_for(K: int, target: int = 2 ** 11) -> float:
+    """Nonzero density p of both operands of a K-term dot product: K * p^2 nonzero products expected, at most ``target``."""
+    return min(1.0, math.sqrt(target / K))
+
+
+def int_operand(shape, K: int, gen: torch.Generator, target: int = 2 ** 11, device="cpu") -> torch.Tensor:
+    """fp32 tensor of {-1, 0, +1}: nonzero with probability ``density_for(K, target)``, sign uniform."""
+    p = density_for(K, target)
+    nz = torch.rand(shape, generator=gen) < p
+    sign = torch.randint(0, 2, shape, generator=gen) * 2 - 1
+    return (nz * sign).to(torch.float32).to(device)
+
+
+def cl(t: torch.Tensor) -> torch.Tensor:
+    """bf16 channels-last copy (exact for integer data)."""
+    return t.to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
+
+
+def wt(w: torch.Tensor) -> torch.Tensor:
+    """Weights [Cout, Cin, k, k] as bf16 in the arena storage order [Cout, k, k, Cin]."""
+    return w.to(torch.bfloat16).permute(0, 2, 3, 1).contiguous().permute(0, 3, 1, 2)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# rounding
+# ---------------------------------------------------------------------------------------------------------------------
+def bf16_rn(x: torch.Tensor) -> torch.Tensor:
+    """Round an fp64 tensor to bf16 once, to nearest, ties to even (no intermediate fp32 rounding).  Normal range only."""
+    x = x.double()
+    m, e = torch.frexp(x)                                   # x = m * 2^e, 0.5 <= |m| < 1
+    r = torch.ldexp(torch.round(m * 256.0), (e - 8).double())   # 8 significant bits; torch.round is half-to-even
+    r = torch.where(x == 0, x, r)
+    return r.float().to(torch.bfloat16)                     # exact: r has 8 significant bits
+
+
+def bf16_rz(x: torch.Tensor) -> torch.Tensor:
+    """Round an fp64 tensor to bf16 toward zero (the truncating store a kernel must not use)."""
+    x = x.double()
+    m, e = torch.frexp(x)
+    r = torch.ldexp(torch.trunc(m * 256.0), (e - 8).double())
+    return torch.where(x == 0, x, r).float().to(torch.bfloat16)
+
+
+def ulp_bf16(x: torch.Tensor) -> torch.Tensor:
+    """Spacing of bf16 values at |x| (normal range)."""
+    _, e = torch.frexp(x.double().abs().clamp_min(2.0 ** -126))
+    return torch.ldexp(torch.ones_like(x, dtype=torch.float64), (e - 8).double())
+
+
+def ulp_f32(x: torch.Tensor) -> torch.Tensor:
+    _, e = torch.frexp(x.double().abs().clamp_min(2.0 ** -126))
+    return torch.ldexp(torch.ones_like(x, dtype=torch.float64), (e - 24).double())
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# fp64 convolution references (NCHW logical tensors, any memory format)
+# ---------------------------------------------------------------------------------------------------------------------
+def _taps(ks, stride, oh, ow):
+    for r in range(ks):
+        for s in range(ks):
+            yield r, s, slice(r, r + stride * (oh - 1) + 1, stride), slice(s, s + stride * (ow - 1) + 1, stride)
+
+
+def conv_ref(x: torch.Tensor, w: torch.Tensor, stride: int, bias=None) -> torch.Tensor:
+    """fp64 y[N, Cout, H/s, W/s] of a k x k convolution with padding k // 2."""
+    ks = w.shape[2]
+    pad = ks // 2
+    n, _, h, wd = x.shape
+    oh, ow = h // stride, wd // stride
+    xp = torch.nn.functional.pad(x.double().permute(0, 2, 3, 1), (0, 0, pad, pad, pad, pad))     # [N, H+2p, W+2p, Cin]
+    wd64 = w.double()
+    y = torch.zeros(n, oh, ow, w.shape[0], dtype=torch.float64, device=x.device)
+    for r, s, hs, ws in _taps(ks, stride, oh, ow):
+        y += xp[:, hs, ws, :] @ wd64[:, :, r, s].t()
+    if bias is not None:
+        y += bias.double()
+    return y.permute(0, 3, 1, 2)
+
+
+def dgrad_ref(dy: torch.Tensor, w: torch.Tensor, in_hw, stride: int) -> torch.Tensor:
+    """fp64 dx[N, Cin, H, W] = adjoint of ``conv_ref`` applied to dy."""
+    ks = w.shape[2]
+    pad = ks // 2
+    h, wd = in_hw
+    n, _, oh, ow = dy.shape
+    d = dy.double().permute(0, 2, 3, 1)
+    wd64 = w.double()
+    dxp = torch.zeros(n, h + 2 * pad, wd + 2 * pad, w.shape[1], dtype=torch.float64, device=dy.device)
+    for r, s, hs, ws in _taps(ks, stride, oh, ow):
+        dxp[:, hs, ws, :] += d @ wd64[:, :, r, s]
+    return dxp[:, pad:pad + h, pad:pad + wd, :].permute(0, 3, 1, 2)
+
+
+def wgrad_ref(dy: torch.Tensor, x: torch.Tensor, ks: int, stride: int) -> torch.Tensor:
+    """fp64 dw[Cout, Cin, k, k] = sum over pixels of dy (outer) the tap slice of x."""
+    pad = ks // 2
+    n, cout, oh, ow = dy.shape
+    xp = torch.nn.functional.pad(x.double().permute(0, 2, 3, 1), (0, 0, pad, pad, pad, pad))
+    d = dy.double().permute(0, 2, 3, 1).reshape(-1, cout)
+    dw = torch.zeros(cout, x.shape[1], ks, ks, dtype=torch.float64, device=dy.device)
+    for r, s, hs, ws in _taps(ks, stride, oh, ow):
+        dw[:, :, r, s] = d.t() @ xp[:, hs, ws, :].reshape(-1, x.shape[1])
+    return dw
+
+
+def assert_exact_domain(*refs: torch.Tensor, limit: int = FP32_EXACT) -> None:
+    """The integer-operand argument needs every partial sum below 2^24: the sums of absolute values bound them all."""
+    for r in refs:
+        assert float(r.abs().max()) <= limit, f"reference magnitude {float(r.abs().max())} leaves the exact fp32 range"
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# checkers
+# ---------------------------------------------------------------------------------------------------------------------
+def _where(idx, shape, tile_rows: int):
+    """Index tuple, plus (pixel row, 128-row tile) for 4-D NCHW activations whose GEMM rows are NHWC pixels."""
+    pos = [int(v) for v in torch.unravel_index(torch.tensor(idx), shape)]
+    if len(shape) == 4:
+        n, c, h, w = pos
+        row = (n * shape[2] + h) * shape[3] + w
+        return f"(n={n}, c={c}, h={h}, w={w}), pixel row {row}, tile {row // tile_rows}"
+    return f"index {tuple(pos)}"
+
+
+def mismatch(out: torch.Tensor, ref: torch.Tensor, tile_rows: int = 128) -> str:
+    """'' if ``out`` equals ``ref`` bit for bit (same dtype), else a description of the first differing element and the count."""
+    assert out.shape == ref.shape, (out.shape, ref.shape)
+    a, b = out.float().cpu(), ref.float().cpu()
+    bad = (a != b) & ~(a.isnan() & b.isnan())
+    if not bool(bad.any()):
+        return ""
+    idx = int(bad.flatten().nonzero()[0])
+    return (f"{int(bad.sum())} of {bad.numel()} elements differ; first at {_where(idx, out.shape, tile_rows)}: "
+            f"got {float(a.flatten()[idx])}, expected {float(b.flatten()[idx])}")
+
+
+def assert_equal(out: torch.Tensor, ref: torch.Tensor, what: str = "", tile_rows: int = 128) -> None:
+    msg = mismatch(out, ref, tile_rows)
+    assert not msg, f"{what}: {msg}"
+
+
+def bound_violation(out: torch.Tensor, ref64: torch.Tensor, absref64: torch.Tensor, K: int, rel: float = 2.0 ** -8,
+                    tile_rows: int = 128) -> str:
+    """'' if |out - ref64| <= rel * |ref64| + (K + 1) * 2^-23 * absref64 everywhere, else the worst element (largest ratio of
+    error to bound) with its index, pixel row and tile."""
+    assert out.shape == ref64.shape == absref64.shape, (out.shape, ref64.shape, absref64.shape)
+    err = (out.double() - ref64).abs()
+    bound = rel * ref64.abs() + (K + 1) * 2.0 ** -23 * absref64
+    ratio = err / bound.clamp_min(1e-300)
+    ratio = torch.where(err == 0, torch.zeros_like(ratio), ratio)
+    worst = int(ratio.flatten().argmax())
+    if float(ratio.flatten()[worst]) <= 1.0 and bool(torch.isfinite(out).all()):
+        return ""
+    if not bool(torch.isfinite(out).all()):
+        worst = int((~torch.isfinite(out)).flatten().nonzero()[0])
+    return (f"{int((ratio > 1).sum())} elements outside the bound; worst at {_where(worst, out.shape, tile_rows)}: "
+            f"got {float(out.flatten()[worst])}, ref {float(ref64.flatten()[worst])}, |err| {float(err.flatten()[worst]):.3e} "
+            f"> bound {float(bound.flatten()[worst]):.3e}")
+
+
+def assert_bound(out, ref64, absref64, K: int, what: str = "", rel: float = 2.0 ** -8) -> None:
+    msg = bound_violation(out, ref64, absref64, K, rel)
+    assert not msg, f"{what}: {msg}"
+
+
+def rel_err(a: torch.Tensor, b: torch.Tensor) -> float:
+    """The global metric the older tests use: max |a - b| / max |b|."""
+    return float((a.double() - b.double()).abs().max() / b.double().abs().max().clamp_min(1e-6))
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# BatchNorm statistics
+# ---------------------------------------------------------------------------------------------------------------------
+def _f32(x: torch.Tensor) -> torch.Tensor:
+    return x.double().float().double()
+
+
+def bn_stats_ref(y: torch.Tensor, eps: float, momentum: float, running_mean=None, running_var=None):
+    """The kernels' fp32 finalisation applied to the EXACT per-channel sums of the bf16 tensor ``y`` [N, C, H, W]:
+
+        m = S * (1/M);  var = max(fma(-m, m, Q * (1/M)), 0);  invstd = rsqrt(var + eps)
+        running_mean += momentum * (m - running_mean);  running_var += momentum * (var * (M / (M - 1)) - running_var)
+
+    every operation rounded to fp32 (fma once).  The sums are exact in fp32 when S and Q stay below 2^24 (asserted here).
+    Returns fp64 tensors holding fp32 values (mean, var, invstd_ref64, rm, rv); ``invstd_ref64`` is the fp64 rsqrt of the fp32
+    ``var + eps`` (the kernels' rsqrtf is within 2 ulp of it)."""
+    yd = y.double()
+    M = yd.numel() // yd.shape[1]
+    S = yd.sum((0, 2, 3))
+    Q = (yd * yd).sum((0, 2, 3))
+    assert_exact_domain(yd.abs().sum((0, 2, 3)), Q)
+    inv_m = _f32(torch.tensor(1.0 / float(torch.tensor(float(M), dtype=torch.float32)), dtype=torch.float64))
+    m = _f32(S * inv_m)
+    var = _f32(-m * m + _f32(Q * inv_m))              # fma: one rounding (the fp64 sum is exact or within 2^-53)
+    var = var.clamp_min(0.0)
+    v = _f32(var + _f32(torch.tensor(eps, dtype=torch.float64)))
+    invstd = 1.0 / v.sqrt()
+    rm = rv = None
+    if running_mean is not None:
+        r = _f32(torch.tensor(float(torch.tensor(float(M), dtype=torch.float32)) / float(torch.tensor(float(M - 1),
+                                                                                                        dtype=torch.float32)),
+                              dtype=torch.float64))
+        unb = _f32(var * r)
+        mom = _f32(torch.tensor(momentum, dtype=torch.float64))
+        rm0, rv0 = running_mean.double().to(m.device), running_var.double().to(m.device)
+        rm = _f32(mom * _f32(m - rm0) + rm0)
+        rv = _f32(mom * _f32(unb - rv0) + rv0)
+    return m, var, invstd, rm, rv
+
+
+def ulps_f32(got: torch.Tensor, ref: torch.Tensor) -> float:
+    """max |got - ref| in units of the fp32 spacing at ref."""
+    g, r = got.double().to(ref.device), ref.double()
+    return float(((g - r).abs() / ulp_f32(r)).max())
