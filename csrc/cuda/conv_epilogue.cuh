@@ -1,9 +1,9 @@
 // Epilogue shared by the wgmma convolution kernels (conv_tap_wgmma.cu, conv_halo_wgmma.cu).
 //
-// A finished 128-pixel x BLOCK_N accumulator tile leaves the registers of the MMA warpgroup (handed over thread = pixel row,
-// tc::acc_row32) and is
-//   1. converted to bf16 (+ bias) and written into a shared-memory staging tile in the 128B-swizzled layout TMA expects
-//      (row = pixel, 16-byte chunk j of row r at chunk j ^ (r & 7): conflict-free 16-byte stores);
+// A finished 128-pixel x BLOCK_N accumulator tile is drained straight from the wgmma fragments of the MMA warpgroup and is
+//   1. converted to bf16 (+ bias, + residual, ReLU-backward mask) and written into a shared-memory staging tile in the
+//      128B-swizzled layout TMA expects (row = pixel, 16-byte chunk j of row r at chunk j ^ (r & 7)): every thread stores its own
+//      column pairs as bf16x2 words, conflict-free, with no hand-over of the accumulators between threads;
 //   2. handed to ONE TMA tensor store per 64-channel half (cp.async.bulk.tensor...global.shared::cta, SASS UTMASTG) -- the
 //      4-D box mirrors the load box, so partial batches are clipped by the TMA unit and every global write is a full line;
 //   3. (optional) reduced per channel for the BatchNorm that follows the convolution: every epilogue thread owns 8 channels
@@ -53,71 +53,82 @@ struct BnStatArgs {
 __host__ __device__ constexpr int staging_bytes(int block_n) { return block_n * 128 * 2; }          // 128 rows x block_n bf16
 __host__ __device__ constexpr int stat_bytes() { return 4 * 2 * STAT_MAX_C * 4; }                   // [4 warps][2][512] fp32
 
-// Drain one accumulator tile.  Called by all 128 threads of the MMA warpgroup (et = 0..127 = tile row).
-//   acc      : the tile's accumulators (wgmma fragment of this thread), scratch: tc::SCRATCH_BYTES of shared memory
-//   sbuf     : staging tile (1024-byte aligned), s_stat: statistics accumulators or null
-//   valid_rows: rows of the tile that are real pixels (partial batch tiles), col0: first output channel of the tile
-template <int BLOCK_N>
-__device__ __forceinline__ void drain_tile(const float (&acc)[2][BLOCK_N / 2], float* scratch, uint8_t* sbuf, float* s_stat, int et,
-                                           int valid_rows, int col0, int Cn, const float* bias_f32, const __nv_bfloat16* bias_bf16,
-                                           const __nv_bfloat16* resid_row = nullptr, const __nv_bfloat16* mask_row = nullptr) {
-  // mask_row: channel 0 of this thread's pixel in a tensor of the output's shape; the output is zeroed where it is <= 0 (ReLU
-  // backward of the BatchNorm output that fed this convolution), after the residual add
-  // resid_row: channel 0 of THIS thread's output pixel in a tensor of the output's shape that is added to the tile before rounding
-  // (dgrad: the gradient arriving over the other branch of a fork, e.g. the residual shortcut); null = nothing to add / row invalid
-  // the previous tile's TMA store must have finished READING the staging tile before it is overwritten
+// Drain one accumulator tile.  Called by all 128 threads of the MMA warpgroup (et = 0..127), straight from the wgmma fragment:
+// each thread takes its own column pairs of four tile rows (tc::frag_row / tc::frag_col) and writes them as bf16x2 words into the
+// staging tile.  For a fixed (h, j, rr) the 32 lanes of a warp cover 8 rows x 4 words of 16-byte chunk j ^ (row & 7): 32 distinct
+// banks, no conflicts, and no shared-memory round trip or barrier between the accumulators and the staged tile.
+//   acc       : the tile's accumulators (wgmma fragment of this thread)
+//   sbuf      : staging tile (1024-byte aligned), valid_rows: rows of the tile that are real pixels (partial batch tiles)
+//   col0, Cn  : first output channel of the tile, output channels
+//   resid     : optional tensor of the output's shape added to the tile before rounding (dgrad: the gradient arriving over the
+//               other branch of a fork, e.g. the residual shortcut)
+//   mask      : optional tensor of the output's shape; the output is zeroed where it is <= 0 (ReLU backward of the BatchNorm output
+//               that fed this convolution), after the residual add
+//   row_off(r): element offset of channel 0 of tile row r in those tensors (only called for r < valid_rows)
+// Per element: acc (+ bias) (+ resid) (mask), rounded once to nearest even -- the staged tile is what the TMA store and the
+// statistics read.
+template <int BLOCK_N, typename RowOff>
+__device__ __forceinline__ void drain_tile(const float (&acc)[2][BLOCK_N / 2], uint8_t* sbuf, int et, int valid_rows, int col0, int Cn,
+                                           const float* bias_f32, const __nv_bfloat16* bias_bf16, const __nv_bfloat16* resid,
+                                           const __nv_bfloat16* mask, RowOff row_off) {
+  const int cols = Cn - col0;                      // 64-column box b of the tile is real iff 64 b < cols (Cn % 64 == 0)
+  const int cq = tc::frag_col(et, 0);              // this thread's first column inside a block
+  // the previous tile's TMA store (and every thread's statistics pass) must have finished READING the staging tile
   if (et == 0) tc::tma_store_wait_read<0>();
   tc::named_bar_sync(EPI_BAR_ID, EPI_THREADS);
 #pragma unroll
-  for (int c = 0; c < BLOCK_N; c += 32) {
-    float f[32];
-    tc::acc_row32<BLOCK_N>(acc, c, scratch, et, f, EPI_BAR_ID);
-    if (bias_f32 || bias_bf16) {
+  for (int h = 0; h < 2; ++h) {
 #pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const int cc = col0 + c + j;
-        if (cc < Cn) f[j] += bias_f32 ? bias_f32[cc] : __bfloat162float(bias_bf16[cc]);
-      }
-    }
-    if (resid_row) {
+    for (int rr = 0; rr < 2; ++rr) {
+      const int r = tc::frag_row(et, h, rr);
+      const uint32_t srow = tc::smem_u32(sbuf) + r * 128 + 4 * (et & 3);
+      // one 64-column box at a time: at most 8 column pairs and 8 residual / mask words in flight (register pressure)
 #pragma unroll
-      for (int jj = 0; jj < 4; ++jj) {
-        const int cc = col0 + c + jj * 8;
-        if (cc < Cn) {
-          const uint4 rv = __ldg(reinterpret_cast<const uint4*>(resid_row + cc));
-          const __nv_bfloat162* rp = reinterpret_cast<const __nv_bfloat162*>(&rv);
+      for (int box = 0; box < BLOCK_N / 64; ++box) {
+        if (64 * box >= cols) continue;            // Cn % 64 == 0: the box is real or entirely beyond Cn
+        float v[8][2];
 #pragma unroll
-          for (int e = 0; e < 4; ++e) { const float2 g = __bfloat1622float2(rp[e]); f[jj * 8 + 2 * e] += g.x; f[jj * 8 + 2 * e + 1] += g.y; }
+        for (int jj = 0; jj < 8; ++jj) {
+          v[jj][0] = acc[h][4 * (8 * box + jj) + 2 * rr];
+          v[jj][1] = acc[h][4 * (8 * box + jj) + 2 * rr + 1];
         }
-      }
-    }
-    if (mask_row) {
+        const int cc0 = col0 + 64 * box + cq;
+        if (bias_f32 || bias_bf16) {
 #pragma unroll
-      for (int jj = 0; jj < 4; ++jj) {
-        const int cc = col0 + c + jj * 8;
-        if (cc < Cn) {
-          const uint4 mv = __ldg(reinterpret_cast<const uint4*>(mask_row + cc));
-          const __nv_bfloat162* mp = reinterpret_cast<const __nv_bfloat162*>(&mv);
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float2 g = __bfloat1622float2(mp[e]);
-            f[jj * 8 + 2 * e] = g.x > 0.f ? f[jj * 8 + 2 * e] : 0.f;
-            f[jj * 8 + 2 * e + 1] = g.y > 0.f ? f[jj * 8 + 2 * e + 1] : 0.f;
+          for (int jj = 0; jj < 8; ++jj) {
+            const int cc = cc0 + 8 * jj;
+            v[jj][0] += bias_f32 ? bias_f32[cc] : __bfloat162float(bias_bf16[cc]);
+            v[jj][1] += bias_f32 ? bias_f32[cc + 1] : __bfloat162float(bias_bf16[cc + 1]);
           }
         }
-      }
-    }
-    uint8_t* row = sbuf + (c >> 6) * (128 * 128) + et * 128;
-    const int lc0 = (c & 63) >> 3;
+        if ((resid || mask) && r < valid_rows) {
+          const long long off = row_off(r) + cc0;
+          __nv_bfloat162 g[8];
+          if (resid) {
 #pragma unroll
-    for (int jj = 0; jj < 4; ++jj) {
-      const int phys = (lc0 + jj) ^ (et & 7);
-      *reinterpret_cast<uint4*>(row + phys * 16) = tc::pack8(f + jj * 8);
+            for (int jj = 0; jj < 8; ++jj) g[jj] = __ldg(reinterpret_cast<const __nv_bfloat162*>(resid + off + 8 * jj));
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) { const float2 f = __bfloat1622float2(g[jj]); v[jj][0] += f.x; v[jj][1] += f.y; }
+          }
+          if (mask) {
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) g[jj] = __ldg(reinterpret_cast<const __nv_bfloat162*>(mask + off + 8 * jj));
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const float2 f = __bfloat1622float2(g[jj]);
+              v[jj][0] = f.x > 0.f ? v[jj][0] : 0.f;
+              v[jj][1] = f.y > 0.f ? v[jj][1] : 0.f;
+            }
+          }
+        }
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj)                 // ordered before the fence below: both volatile
+          asm volatile("st.shared.b32 [%0], %1;" ::"r"(srow + box * (128 * 128) + ((jj ^ (r & 7)) << 4)), "r"(tc::pack2(v[jj][0], v[jj][1])));
+      }
     }
   }
   tc::fence_async_smem();                          // generic-proxy writes -> visible to the TMA store
   tc::named_bar_sync(EPI_BAR_ID, EPI_THREADS);
-  (void)valid_rows; (void)s_stat;
 }
 
 // Per-channel sum / sum of squares of the staged (bf16-rounded) tiles, kept in REGISTERS across the tiles of a CTA: epilogue

@@ -33,7 +33,7 @@ constexpr int W_TAP_BYTES = BLOCK_N * 128;           // 8 KB
 constexpr int W_BYTES = 9 * W_TAP_BYTES;             // 72 KB
 constexpr int STAGES = 2;
 constexpr int EPI_BYTES = convepi::staging_bytes(BLOCK_N) + convepi::stat_bytes();
-constexpr int SMEM_BYTES = W_BYTES + STAGES * HALO_BYTES + EPI_BYTES + SCRATCH_BYTES + 1024 + 256;
+constexpr int SMEM_BYTES = W_BYTES + STAGES * HALO_BYTES + EPI_BYTES + 1024 + 256;
 static_assert(SMEM_BYTES <= 227 * 1024, "H100: 227 KB of shared memory per block");
 
 struct HaloArgs {
@@ -60,8 +60,7 @@ conv_halo_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_
   uint8_t* s_halo = smem + W_BYTES;                 // STAGES x HALO_BYTES
   uint8_t* sbuf = s_halo + STAGES * HALO_BYTES;     // staging tile [128][128 B]
   float* s_stat = reinterpret_cast<float*>(sbuf + convepi::staging_bytes(BLOCK_N));
-  float* scratch = reinterpret_cast<float*>(sbuf + EPI_BYTES);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sbuf + EPI_BYTES + SCRATCH_BYTES);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sbuf + EPI_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
   uint64_t* w_bar = empty_bar + STAGES;
 
@@ -117,6 +116,8 @@ conv_halo_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_
       }
       mbar_wait(&full_bar[stage], phase);
       const uint32_t halo = smem_u32(s_halo + stage * HALO_BYTES);
+      acc_undef<BLOCK_N / 2>(acc[0]);               // the previous tile's values: dead during its epilogue
+      acc_undef<BLOCK_N / 2>(acc[1]);
 #pragma unroll
       for (int tap = 0; tap < 9; ++tap) {
         const int r = tap / 3, s = tap - 3 * r;
@@ -131,9 +132,8 @@ conv_halo_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_
       if (lane == 0) mbar_arrive(&empty_bar[stage]);
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
       auto row_off = [&](int r) -> long long { return (((long long)n0 * a.H + (h0 + r / TW)) * a.W + (w0 + r % TW)) * BLOCK_N; };
-      const __nv_bfloat16* rrow = a.resid ? a.resid + row_off(et) : nullptr;
-      const __nv_bfloat16* mrow = (want_stats && a.stat.bwd_mask) ? a.stat.bwd_mask + row_off(et) : nullptr;
-      convepi::drain_tile<BLOCK_N>(acc, scratch, sbuf, s_stat, et, BLOCK_M, 0, BLOCK_N, a.bias_f32, a.bias_bf16, rrow, mrow);
+      convepi::drain_tile<BLOCK_N>(acc, sbuf, et, BLOCK_M, 0, BLOCK_N, a.bias_f32, a.bias_bf16, a.resid,
+                                   want_stats ? a.stat.bwd_mask : nullptr, row_off);
       if (et == 0) {
         tma_store_4d(&tmap_out, sbuf, 0, w0, h0, n0);
         tma_store_commit();

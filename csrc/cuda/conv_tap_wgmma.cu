@@ -1,7 +1,7 @@
 // K10 (convolution part, continued): generalised tap-table implicit-GEMM convolutions on wgmma -- stride 1 or 2, 1x1 or 3x3.
 //
 // Machinery: TMA patch loads into 128B-swizzled tiles, wgmma 64xNx16 on both halves of a 128-pixel tile by one warpgroup with
-// the accumulators in registers, pixel-mapped epilogue (wgmma_common.cuh).  What is specific is how a filter tap reaches the
+// the accumulators in registers, epilogue from the accumulator fragments (wgmma_common.cuh).  What is specific is how a filter tap reaches the
 // tensor core:
 //
 //   * strided fprop : the activation tensor map carries elementStrides {1, s, s, 1}, so ONE box load delivers the
@@ -16,9 +16,10 @@
 // 9-tap instance of the same kernel.  Motivation: the strided dgrads of ResNet-18 cost 5-10x their FLOP time in the library
 // path (zero-insertion or one launch per parity class).
 //
-// The epilogue (conv_epilogue.cuh) stages the bf16 tile in swizzled shared memory, stores it with ONE TMA tensor store per
-// 64-channel half and can reduce it per channel for the BatchNorm that follows (statistics pass fused into the convolution);
-// the stride-2 dgrad parity classes, whose output pixels are strided, keep the direct-store epilogue.
+// The epilogue (conv_epilogue.cuh) stages the bf16 tile in swizzled shared memory straight from the accumulator fragments, stores
+// it with ONE TMA tensor store per 64-channel half and can reduce it per channel for the BatchNorm that follows (statistics pass
+// fused into the convolution); the stride-2 dgrad parity classes, whose output pixels are strided, stage the tile the same way
+// and then store each pixel row with 16-byte global stores.
 //
 // Reference counterpart: the strided nn.Conv2d layers of src/model_ops/resnet.py:14-64 (downsampling blocks + shortcuts).
 #include <cstdio>
@@ -71,7 +72,6 @@ struct TapConvArgs {
 // MODE 0: one CTA per tile.  MODE 1: multicast cluster (see TapConvArgs::cm).
 // tmap_xs / tmap_ws: the same tensors with the SLICE boxes (1/cn of the patch, 1/cm of the weight rows).
 constexpr int MODE_PLAIN = 0, MODE_MCAST = 1;
-constexpr int EPI_BAR_ID = convepi::EPI_BAR_ID;
 
 // Releases a consumed stage: every warp of the MMA warpgroup arrives once on the stage's empty barrier of every CTA that filled
 // it (cluster: the CTAs of my row and column multicast into it; mask bit i = cluster rank i).
@@ -90,14 +90,13 @@ convg_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_cons
   constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;
   constexpr int B_BYTES = BLOCK_N * BLOCK_K * 2;
   constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  constexpr int EPI_BYTES = TMA_EPI ? convepi::staging_bytes(BLOCK_N) + convepi::stat_bytes() : 0;
+  constexpr int EPI_BYTES = convepi::staging_bytes(BLOCK_N) + (TMA_EPI ? convepi::stat_bytes() : 0);
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sbuf = smem + STAGES * STAGE_BYTES;                                   // staging tile (1024-aligned: STAGE_BYTES % 1024 == 0)
-  float* s_stat = reinterpret_cast<float*>(sbuf + (TMA_EPI ? convepi::staging_bytes(BLOCK_N) : 0));
-  float* scratch = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES + EPI_BYTES);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + EPI_BYTES + SCRATCH_BYTES);
+  float* s_stat = reinterpret_cast<float*>(sbuf + convepi::staging_bytes(BLOCK_N));
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + EPI_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
 
   const int warp = threadIdx.x >> 5;
@@ -239,6 +238,8 @@ convg_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_cons
         dbg[3] = clock64();
       }
       int prev = -1;
+      acc_undef<BLOCK_N / 2>(acc[0]);                             // the previous tile's values: dead during its epilogue
+      acc_undef<BLOCK_N / 2>(acc[1]);
       for (int kb = 0; kb < k_blocks; ++kb) {
         mbar_wait(&full_bar[stage], phase);
         const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
@@ -255,18 +256,15 @@ convg_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_cons
       if (dbg && et == 0) dbg[5] = clock64();                      // accumulator complete
       release_stage(&empty_bar[prev], CLUSTER, rel_mask, lane);
       const bool tile_ok = mt < m_tiles && n0 < a.Cn;              // false: overhang of the cluster grid, nothing to store
+      int valid_rows = tile_ok ? (a.N - nb0) * a.BW * a.BH : 0;    // rows are pixels, w fastest: the real ones are a prefix
+      if (valid_rows > BLOCK_M) valid_rows = BLOCK_M;
       if (TMA_EPI) {
-        int valid_rows = tile_ok ? (a.N - nb0) * a.BW * a.BH : 0;
-        if (valid_rows > BLOCK_M) valid_rows = BLOCK_M;
         // element offset of channel 0 of tile row r in a tensor of the output's shape
         auto row_off = [&](int r) -> long long {
           const int rw = w0 + r % a.BW, rh = h0 + (r / a.BW) % a.BH, rn_ = nb0 + r / (a.BW * a.BH);
           return (((long long)rn_ * a.out_H + rh) * a.out_W + rw) * a.Cn;
         };
-        const bool row_ok = et < valid_rows;
-        const __nv_bfloat16* rrow = (a.resid && row_ok) ? a.resid + row_off(et) : nullptr;
-        const __nv_bfloat16* mrow = (a.stat.bwd_mask && row_ok) ? a.stat.bwd_mask + row_off(et) : nullptr;
-        convepi::drain_tile<BLOCK_N>(acc, scratch, sbuf, s_stat, et, valid_rows, n0, a.Cn, a.bias_f32, a.bias_bf16, rrow, mrow);
+        convepi::drain_tile<BLOCK_N>(acc, sbuf, et, valid_rows, n0, a.Cn, a.bias_f32, a.bias_bf16, a.resid, a.stat.bwd_mask, row_off);
         if (et == 0 && tile_ok) {
 #pragma unroll
           for (int j = 0; j < BLOCK_N / 64; ++j)
@@ -280,43 +278,22 @@ convg_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_cons
           if (!stat_keep) sacc.flush(s_stat, et, n0, a.Cn);
         }
       } else {
-        const int m = et;                                        // row of the tile = pixel of the patch (w fastest)
-        const int pw = w0 + m % a.BW, ph = h0 + (m / a.BW) % a.BH, pn = nb0 + m / (a.BW * a.BH);
-        const bool row_ok = tile_ok && pn < a.N;
-        __nv_bfloat16* orow = a.out + (((long long)pn * a.out_H + (ph * a.out_mul + a.cls_oh[cls])) * a.out_W + (pw * a.out_mul + a.cls_ow[cls])) * a.Cn;
+        // strided output pixels (stride-2 dgrad parity class): the same staged tile, then every thread stores its row (pixel
+        // (out_mul * i + cls_oh, out_mul * j + cls_ow)) with 16-byte global stores
+        auto row_off = [&](int r) -> long long {
+          const int pw = w0 + r % a.BW, ph = h0 + (r / a.BW) % a.BH, pn = nb0 + r / (a.BW * a.BH);
+          return (((long long)pn * a.out_H + (ph * a.out_mul + a.cls_oh[cls])) * a.out_W + (pw * a.out_mul + a.cls_ow[cls])) * a.Cn;
+        };
+        convepi::drain_tile<BLOCK_N>(acc, sbuf, et, valid_rows, n0, a.Cn, a.bias_f32, a.bias_bf16, a.resid, nullptr, row_off);
+        if (et < valid_rows) {
+          __nv_bfloat16* orow = a.out + row_off(et) + n0;
 #pragma unroll
-        for (int c = 0; c < BLOCK_N; c += 32) {
-          float f[32];
-          acc_row32<BLOCK_N>(acc, c, scratch, et, f, EPI_BAR_ID);
-          const int col0 = n0 + c;
-          if (row_ok && col0 < a.Cn) {
-            if (a.bias_f32 || a.bias_bf16) {
+          for (int j = 0; j < BLOCK_N / 64; ++j) {
+            if (n0 + 64 * j < a.Cn) {
 #pragma unroll
-              for (int j = 0; j < 32; ++j)
-                if (col0 + j < a.Cn) f[j] += a.bias_f32 ? a.bias_f32[col0 + j] : __bfloat162float(a.bias_bf16[col0 + j]);
-            }
-            __nv_bfloat16* dst = orow + col0;
-            if (a.resid) {
-              const __nv_bfloat16* rsrc = a.resid + (dst - a.out);
-              if (col0 + 32 <= a.Cn) {
-#pragma unroll
-                for (int j = 0; j < 32; j += 8) {
-                  const uint4 rv = __ldg(reinterpret_cast<const uint4*>(rsrc + j));
-                  const __nv_bfloat162* rp = reinterpret_cast<const __nv_bfloat162*>(&rv);
-#pragma unroll
-                  for (int e = 0; e < 4; ++e) { const float2 g = __bfloat1622float2(rp[e]); f[j + 2 * e] += g.x; f[j + 2 * e + 1] += g.y; }
-                }
-              } else {
-#pragma unroll
-                for (int j = 0; j < 32; ++j) if (col0 + j < a.Cn) f[j] += __bfloat162float(rsrc[j]);
-              }
-            }
-            if (col0 + 32 <= a.Cn) {
-#pragma unroll
-              for (int j = 0; j < 32; j += 8) *reinterpret_cast<uint4*>(dst + j) = pack8(f + j);
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) if (col0 + j < a.Cn) dst[j] = __float2bfloat16_rn(f[j]);
+              for (int c = 0; c < 8; ++c)
+                *reinterpret_cast<uint4*>(orow + 64 * j + 8 * c) =
+                    *reinterpret_cast<const uint4*>(sbuf + j * (128 * 128) + et * 128 + ((c ^ (et & 7)) << 4));
             }
           }
         }
@@ -368,8 +345,7 @@ convg_wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __gr
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  float* scratch = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + SCRATCH_BYTES);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
 
   const int warp = threadIdx.x >> 5;
@@ -445,22 +421,22 @@ convg_wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __gr
       fence_acc<BLOCK_N / 2>(acc[0]);
       fence_acc<BLOCK_N / 2>(acc[1]);
       if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
-      const int co = co0 + et;
-      float* orow = a.partial + ((long long)split * a.Cout + co) * row_pitch + (long long)tap * a.Cin;
-      // an empty K range (more splits than K-blocks) must still produce zeros
+      // fp32 partial straight from the fragment: float2 stores of rows co0 + frag_row, columns ci0 + frag_col; an empty K range
+      // (more splits than K-blocks) must still produce zeros
       const bool empty = kb1 <= kb0;
 #pragma unroll
-      for (int c = 0; c < BLOCK_N; c += 32) {
-        float f[32];
-        acc_row32<BLOCK_N>(acc, c, scratch, et, f, 1);
-        const int col0 = ci0 + c;
-        if (co < a.Cout && col0 < a.Cin) {
+      for (int h = 0; h < 2; ++h) {
 #pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            if (col0 + j + 4 <= a.Cin) {
-              float4 o = empty ? make_float4(0.f, 0.f, 0.f, 0.f) : make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
-              *reinterpret_cast<float4*>(orow + col0 + j) = o;
-            }
+        for (int rr = 0; rr < 2; ++rr) {
+          const int co = co0 + frag_row(et, h, rr);
+          if (co >= a.Cout) continue;
+          float* orow = a.partial + ((long long)split * a.Cout + co) * row_pitch + (long long)tap * a.Cin;
+#pragma unroll
+          for (int j = 0; j < BLOCK_N / 8; ++j) {
+            const int ci = ci0 + frag_col(et, j);
+            if (ci < a.Cin)
+              *reinterpret_cast<float2*>(orow + ci) =
+                  empty ? make_float2(0.f, 0.f) : make_float2(acc[h][4 * j + 2 * rr], acc[h][4 * j + 2 * rr + 1]);
           }
         }
       }
@@ -486,10 +462,10 @@ template <int BLOCK_N, bool B_MN, bool TMA_EPI, int MODE>
 int launch_g(const CUtensorMap& tx, const CUtensorMap& tw, const CUtensorMap& tout, const CUtensorMap& txs, const CUtensorMap& tws,
              const TapConvArgs& a, int grid, cudaStream_t stream) {
   constexpr int STAGE_BYTES = BLOCK_M * BLOCK_K * 2 + BLOCK_N * BLOCK_K * 2;
-  constexpr int EPI_BYTES = TMA_EPI ? convepi::staging_bytes(BLOCK_N) + convepi::stat_bytes() : 0;
-  constexpr int BUDGET = 220 * 1024 - EPI_BYTES - SCRATCH_BYTES;        // 227 KB per block on H100, minus alignment + barriers
+  constexpr int EPI_BYTES = convepi::staging_bytes(BLOCK_N) + (TMA_EPI ? convepi::stat_bytes() : 0);
+  constexpr int BUDGET = 220 * 1024 - EPI_BYTES;                         // 227 KB per block on H100, minus alignment + barriers
   constexpr int STAGES = BUDGET / STAGE_BYTES > 8 ? 8 : BUDGET / STAGE_BYTES;
-  constexpr int SMEM = STAGES * STAGE_BYTES + EPI_BYTES + SCRATCH_BYTES + 1024 + 256;
+  constexpr int SMEM = STAGES * STAGE_BYTES + EPI_BYTES + 1024 + 256;
   auto kern = convg_wgmma_kernel<BLOCK_N, STAGES, B_MN, TMA_EPI, MODE>;
   static bool configured = false;
   if (!configured) {
@@ -818,14 +794,14 @@ extern "C" int drc_convg_wgrad(const void* dy, const void* x, void* dw, float* w
   const int grid = work < num_sms ? work : num_sms;
   if (block_n == 64) {
     constexpr int BN_ = 64, SB = BLOCK_M * BLOCK_K * 2 + BN_ * BLOCK_K * 2, ST = (200 * 1024) / SB > 8 ? 8 : (200 * 1024) / SB;
-    constexpr int SM = ST * SB + SCRATCH_BYTES + 1280;
+    constexpr int SM = ST * SB + 1280;
     auto kern = convg_wgrad_wgmma_kernel<BN_, ST>;
     static bool cfgd = false;
     if (!cfgd) { cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SM); if (e != cudaSuccess) return (int)e; cfgd = true; }
     kern<<<grid, NUM_THREADS, SM, stream>>>(tdy, tx, a);
   } else {
     constexpr int BN_ = 128, SB = BLOCK_M * BLOCK_K * 2 + BN_ * BLOCK_K * 2, ST = (200 * 1024) / SB > 8 ? 8 : (200 * 1024) / SB;
-    constexpr int SM = ST * SB + SCRATCH_BYTES + 1280;
+    constexpr int SM = ST * SB + 1280;
     auto kern = convg_wgrad_wgmma_kernel<BN_, ST>;
     static bool cfgd = false;
     if (!cfgd) { cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SM); if (e != cudaSuccess) return (int)e; cfgd = true; }

@@ -1,6 +1,7 @@
 // K10 (dense part): bf16 GEMM on the Hopper tensor cores, written directly against the sm_90a programming model -- TMA
 // (cp.async.bulk.tensor) stages 128B-swizzled operand tiles in shared memory, one warpgroup issues wgmma with the fp32
-// accumulator in registers and, once a tile is complete, applies bias / ReLU / down-conversion on the way to global memory.
+// accumulator in registers and, once a tile is complete, applies bias / ReLU / down-conversion on the way to global memory,
+// straight from the accumulator fragments (every thread stores its own column pairs).
 //
 //   C[M,N] = op(A) * op(B)^T   with  A: M x K,  B: N x K  (both described K-major *or* MN-major, so the
 //   three products of a linear layer -- y = x W^T, dx = dy W, dW = dy^T x -- run without a transpose pass)
@@ -19,7 +20,6 @@ namespace {
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;           // 64 bf16 = 128 bytes = one swizzle-128B atom row
 constexpr int NUM_THREADS = 256;
-constexpr int EPI_BAR_ID = 1;
 
 struct GemmArgs {
   int M, N, K;
@@ -57,8 +57,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  float* scratch = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + SCRATCH_BYTES);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
 
   const int warp = threadIdx.x >> 5;
@@ -108,7 +107,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     }
   } else if (warp >= 4) {
     // ===================== MMA + epilogue (one warpgroup) =====================
-    const int et = threadIdx.x - 128;                 // tile row this thread stores
+    const int et = threadIdx.x - 128;                 // thread of the warpgroup: owns the fragment rows / columns of tc::frag_row / frag_col
     int stage = 0; uint32_t phase = 0;
     const bool vec_ok = (args.ldc % 8 == 0) && ((reinterpret_cast<uintptr_t>(args.C) & 15) == 0);
     float acc[2][BLOCK_N / 2];
@@ -130,44 +129,42 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
       fence_acc<BLOCK_N / 2>(acc[0]);
       fence_acc<BLOCK_N / 2>(acc[1]);
       if (lane == 0) mbar_arrive(&empty_bar[prev]);
-      const int row = m0 + et;
-      const bool row_ok = row < args.M;
+      // epilogue straight from the fragment: column pairs (c, c + 1) of four rows per thread, 8- / 4-byte stores
 #pragma unroll
-      for (int c = 0; c < BLOCK_N; c += 32) {
-        float f[32];
-        acc_row32<BLOCK_N>(acc, c, scratch, et, f, EPI_BAR_ID);
-        const int col0 = n0 + c;
-        if (row_ok && col0 < args.N) {
-          if (args.bias_f32 || args.bias_bf16) {
+      for (int h = 0; h < 2; ++h) {
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              if (col0 + j < args.N)
-                f[j] += args.bias_f32 ? args.bias_f32[col0 + j] : __bfloat162float(args.bias_bf16[col0 + j]);
+        for (int rr = 0; rr < 2; ++rr) {
+          const int row = m0 + frag_row(et, h, rr);
+          if (row >= args.M) continue;
+#pragma unroll
+          for (int j = 0; j < BLOCK_N / 8; ++j) {
+            const int col = n0 + frag_col(et, j);
+            if (col >= args.N) continue;
+            float f[2] = {acc[h][4 * j + 2 * rr], acc[h][4 * j + 2 * rr + 1]};
+            if (args.bias_f32 || args.bias_bf16) {
+#pragma unroll
+              for (int e = 0; e < 2; ++e)
+                if (col + e < args.N) f[e] += args.bias_f32 ? args.bias_f32[col + e] : __bfloat162float(args.bias_bf16[col + e]);
             }
-          }
-          if (args.relu) {
+            if (args.relu) { f[0] = fmaxf(f[0], 0.f); f[1] = fmaxf(f[1], 0.f); }
+            const bool pair = col + 1 < args.N && vec_ok && !args.accumulate;
+            if (args.c_fp32) {
+              float* dst = reinterpret_cast<float*>(args.C) + (long long)row * args.ldc + col;
+              if (pair) {
+                *reinterpret_cast<float2*>(dst) = make_float2(f[0], f[1]);
+              } else {
 #pragma unroll
-            for (int j = 0; j < 32; ++j) f[j] = fmaxf(f[j], 0.f);
-          }
-          const bool full = col0 + 32 <= args.N;
-          if (args.c_fp32) {
-            float* dst = reinterpret_cast<float*>(args.C) + (long long)row * args.ldc + col0;
-            if (full && vec_ok && !args.accumulate) {
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(dst + j) = make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
+                for (int e = 0; e < 2; ++e) if (col + e < args.N) dst[e] = args.accumulate ? dst[e] + f[e] : f[e];
+              }
             } else {
+              __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(args.C) + (long long)row * args.ldc + col;
+              if (pair) {
+                *reinterpret_cast<uint32_t*>(dst) = pack2(f[0], f[1]);
+              } else {
 #pragma unroll
-              for (int j = 0; j < 32; ++j) if (col0 + j < args.N) dst[j] = args.accumulate ? dst[j] + f[j] : f[j];
-            }
-          } else {
-            __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(args.C) + (long long)row * args.ldc + col0;
-            if (full && vec_ok && !args.accumulate) {
-#pragma unroll
-              for (int j = 0; j < 32; j += 8) *reinterpret_cast<uint4*>(dst + j) = pack8(f + j);
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; ++j)
-                if (col0 + j < args.N) dst[j] = __float2bfloat16_rn(args.accumulate ? __bfloat162float(dst[j]) + f[j] : f[j]);
+                for (int e = 0; e < 2; ++e)
+                  if (col + e < args.N) dst[e] = __float2bfloat16_rn(args.accumulate ? __bfloat162float(dst[e]) + f[e] : f[e]);
+              }
             }
           }
         }
@@ -197,9 +194,9 @@ int make_tmap(CUtensorMap* out, const void* ptr, long long rows, long long K, lo
 template <int BLOCK_N, bool A_MN, bool B_MN>
 int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmArgs& g, int num_sms, cudaStream_t stream) {
   constexpr int STAGE_BYTES = BLOCK_M * BLOCK_K * 2 + BLOCK_N * BLOCK_K * 2;
-  constexpr int BUDGET = 200 * 1024 - SCRATCH_BYTES;
+  constexpr int BUDGET = 200 * 1024;
   constexpr int STAGES = BUDGET / STAGE_BYTES > 8 ? 8 : BUDGET / STAGE_BYTES;
-  constexpr int SMEM = STAGES * STAGE_BYTES + SCRATCH_BYTES + 1024 + 256;
+  constexpr int SMEM = STAGES * STAGE_BYTES + 1024 + 256;
   auto kern = gemm_bf16_wgmma_kernel<BLOCK_N, STAGES, A_MN, B_MN>;
   static bool configured = false;
   if (!configured) {

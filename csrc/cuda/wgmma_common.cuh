@@ -1,11 +1,11 @@
 // Shared sm_90a building blocks of every tensor-core kernel in this tree (GEMM, tap-table / halo convolutions, wgrad):
 // mbarrier + TMA (load, multicast load, store) wrappers, the wgmma shared-memory descriptor and warpgroup MMA wrappers, the
-// register-accumulator -> row hand-over the epilogues use, and the host-side cuTensorMapEncodeTiled lookup.  One copy instead of
-// one per .cu file.
+// accumulator-fragment coordinates the epilogues use, and the host-side cuTensorMapEncodeTiled lookup.  One copy instead of one
+// per .cu file.
 //
 // Kernel shape shared by the tensor-core kernels: warp 0 is the TMA producer (one elected lane), warpgroup 1 (warps 4-7) issues
-// wgmma on a 128-row tile (two m64 halves, fp32 accumulators in registers) and then runs the epilogue of that tile while the
-// producer already fills the stages of the next one.
+// wgmma on a 128-row tile (two m64 halves, fp32 accumulators in registers) and then runs the epilogue of that tile straight from
+// the accumulator fragments while the producer already fills the stages of the next one.
 //
 // Every shared-memory operand starts on a 1024-byte boundary of a 128B-swizzled tile or at +32 / +64 / +96 bytes (K steps inside
 // a swizzle row) or +2048 bytes (16 K rows of an MN-major tile), so the descriptor base-offset field is always 0.
@@ -142,6 +142,14 @@ __device__ __forceinline__ void fence_acc(float* d) {
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
+// The next tile's first wgmma overwrites the accumulators (scale-d = 0), but its "+f" operands would keep the drained values live
+// through the whole epilogue: declare them dead here, right before that tile's MMAs.  Emits no instruction.
+template <int N>
+__device__ __forceinline__ void acc_undef(float* d) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "=f"(d[i]));
+}
+
 // D[64 x N] (+)= A[64 x 16] * B[16 x N], bf16 operands from shared memory, fp32 accumulators in registers.
 // TA / TB: 0 = K-major, 1 = MN-major operand.  `accumulate` = 0 overwrites D.
 template <int N, int TA, int TB>
@@ -215,34 +223,17 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[2][BN / 2], uint32_t sa,
   wgmma_commit();
 }
 
-// Accumulator -> rows.  Thread t of warp w (in the warpgroup) holds, for half h, rows 64h + 16w + t/4 (+8) and columns
-// 8j + 2(t%4) (+1) at acc[h][4j + {0,1,2,3}].  The epilogues work thread-per-row (thread et owns tile row et): acc_row32 hands
-// columns [c, c + 32) of row et to thread et through `scratch` (128 x 17 floats), 16 columns at a time.  All 128 threads of the
-// warpgroup call it with the same compile-time c.
-constexpr int SCRATCH_PITCH = 17;
-constexpr int SCRATCH_BYTES = 128 * SCRATCH_PITCH * 4;
-template <int BN>
-__device__ __forceinline__ void acc_row32(const float (&acc)[2][BN / 2], int c, float* scratch, int et, float* f, int bar_id) {
-  const int w = et >> 5, l = et & 31;
-#pragma unroll
-  for (int q = 0; q < 2; ++q) {
-    named_bar_sync(bar_id, 128);                    // the previous chunk has been read by every row
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-#pragma unroll
-      for (int jj = 0; jj < 2; ++jj) {
-        const int j = (c >> 3) + 2 * q + jj;
-#pragma unroll
-        for (int r = 0; r < 4; ++r) {
-          const int row = 64 * h + 16 * w + (l >> 2) + 8 * (r >> 1);
-          scratch[row * SCRATCH_PITCH + 8 * jj + 2 * (l & 3) + (r & 1)] = acc[h][4 * j + r];
-        }
-      }
-    }
-    named_bar_sync(bar_id, 128);
-#pragma unroll
-    for (int k = 0; k < 16; ++k) f[16 * q + k] = scratch[et * SCRATCH_PITCH + k];
-  }
+// Accumulator fragment of a 128 x BN tile: thread l of warp w (in the warpgroup) holds, for half h, rows 64h + 16w + l/4 (+8) and
+// columns 8j + 2(l%4) (+1) at acc[h][4j + {0,1,2,3}].  The epilogues consume it in place: frag_row / frag_col give the tile row
+// of acc[h][4j + 2rr + {0,1}] and the first of its two columns, so every thread handles column PAIRS of four rows per 8-wide
+// column block.  A quad (four consecutive lanes) covers 8 contiguous columns (16 bf16 bytes / 32 fp32 bytes) of one row.
+__device__ __forceinline__ int frag_row(int et, int h, int rr) { return 64 * h + 16 * (et >> 5) + ((et & 31) >> 2) + 8 * rr; }
+__device__ __forceinline__ int frag_col(int et, int j) { return 8 * j + 2 * (et & 3); }
+
+// two floats -> bf16x2 (round to nearest even), as a 32-bit word
+__device__ __forceinline__ uint32_t pack2(float a, float b) {
+  __nv_bfloat162 p = __floats2bfloat162_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&p);
 }
 
 // pack 8 floats -> 8 bf16 (16 bytes)
