@@ -129,6 +129,13 @@ class KrumSelectArgs(C.Structure):
                 ("rows", ptr)]
 
 
+class AttackArgs(C.Structure):
+    _fields_ = [("grad_in", ptr), ("slot_stride", i64), ("P", C.c_int), ("mode", C.c_int), ("tv", TileView),
+                ("adv_bitmap", ptr), ("adv_len", C.c_int), ("step_ptr", ptr), ("z", C.c_double), ("stats", ptr),
+                ("partials", ptr), ("gamma", ptr), ("tile_begin", C.c_int), ("tile_end", C.c_int), ("t_begin", C.c_int),
+                ("t_end", C.c_int)]
+
+
 def _maybe_build() -> None:
     if os.environ.get("DRACO_NO_AUTOBUILD"):
         return
@@ -200,6 +207,9 @@ def cuda() -> C.CDLL:
             "drc_geomed_weights": [C.POINTER(GeoMedWeightsArgs), st],
             "drc_pair_dist": [C.POINTER(PairDistArgs), C.c_int, st],
             "drc_krum_select": [C.POINTER(KrumSelectArgs), st],
+            "drc_attack_stats": [C.POINTER(AttackArgs), C.c_int, st],
+            "drc_attack_solve": [C.POINTER(AttackArgs), st],
+            "drc_attack_write": [C.POINTER(AttackArgs), C.c_int, st],
             "drc_gemm_bf16": [ptr, i64, C.c_int, ptr, i64, C.c_int, ptr, i64, C.c_int, C.c_int, C.c_int, C.c_int, ptr, ptr,
                               C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, st],
             "drc_rt_init": [C.c_int],

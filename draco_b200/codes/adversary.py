@@ -12,14 +12,20 @@ Attack parity (src/model_ops/utils.py:3-23), ``mag = -100``:
              (cyclic: g + sigma*N(0,1)) from a counter-based generator keyed by (seed, step, worker)
   omniscient (north-star extension): g -> -k * mean(honest gradients); needs a view of the honest
              gradients so it is applied by the engine, not by the per-worker hook.
+  alie     : "A Little Is Enough" (Baruch, Baruch and Goldberg, NeurIPS 2019): mu - z * sigma
+  minmax   : min-max (Shejwalkar and Houmansadr, NDSS 2021): mu - gamma * sigma with the largest gamma that keeps the row
+             within the largest honest pairwise distance of every honest row
+             (both per tensor, over the honest workers' pushed slots; applied by the PS, see ``alie_row`` / ``minmax_row``)
 
 The device implementation of the same hook lives in csrc/cuda/push_encode.cu; the integer codes
 below are shared with it.
 """
 from __future__ import annotations
 
+import math
 from dataclasses import dataclass
-from typing import List, Optional
+from statistics import NormalDist
+from typing import List, Optional, Tuple
 
 import numpy as np
 
@@ -31,6 +37,9 @@ ATTACK_REV_GRAD = 1
 ATTACK_CONSTANT = 2
 ATTACK_RANDOM = 3
 ATTACK_OMNISCIENT = 4
+ATTACK_ALIE = 5
+ATTACK_MINMAX = 6
+PS_ATTACKS = ("alie", "minmax")     # built by the PS from the honest slots; the liars push their true gradient
 
 _ATTACK_CODES = {
     "none": ATTACK_NONE,
@@ -38,6 +47,8 @@ _ATTACK_CODES = {
     "constant": ATTACK_CONSTANT,
     "random": ATTACK_RANDOM,
     "omniscient": ATTACK_OMNISCIENT,
+    "alie": ATTACK_ALIE,
+    "minmax": ATTACK_MINMAX,
 }
 
 
@@ -106,3 +117,86 @@ def err_simulation(grad: np.ndarray, mode: str, cyclic: bool = False, *, magnitu
     if cyclic:
         return g + adv
     return adv if np.iscomplexobj(g) else adv.astype(g.dtype, copy=False)
+
+
+# ------------------------------------------------------------------------------------------------ PS-side attacks (fp64 oracle)
+def alie_s(num_workers: int, worker_fail: int) -> int:
+    """Baruch et al.'s s = floor(P/2 + 1) - f: honest workers the liars need on their side for a majority."""
+    return num_workers // 2 + 1 - worker_fail
+
+
+def alie_z_max(num_workers: int, worker_fail: int) -> float:
+    """z_max = Phi^-1((P - s) / P); undefined (ValueError) when s < 1."""
+    s = alie_s(num_workers, worker_fail)
+    if s < 1:
+        raise ValueError(f"ALIE's z_max is undefined for {num_workers} workers and {worker_fail} liars (s = {s} < 1)")
+    return NormalDist().inv_cdf((num_workers - s) / num_workers)
+
+
+def honest_stats(H: np.ndarray) -> Tuple[np.ndarray, np.ndarray]:
+    """Per-coordinate mean and population standard deviation (ddof 0) of the honest rows ``H`` [n_h, d], in fp64."""
+    H = np.asarray(H, dtype=np.float64)
+    with np.errstate(invalid="ignore", over="ignore"):            # +-Inf rows: NaN sigma, as on the device
+        mu = H.sum(0) / H.shape[0]
+        return mu, np.sqrt(((H - mu) ** 2).sum(0) / H.shape[0])
+
+
+def alie_row(H: np.ndarray, z: float) -> np.ndarray:
+    """The row every ALIE liar sends for one tensor: mu - z * sigma (fp64)."""
+    mu, sd = honest_stats(H)
+    with np.errstate(invalid="ignore"):
+        return mu - z * sd
+
+
+def minmax_gamma(H: np.ndarray) -> float:
+    """Largest gamma with max_i ||mu + gamma p - g_i|| <= Dmax = max_{i<j} ||g_i - g_j|| over the honest rows, p = -sigma.
+
+    Each constraint is c g^2 + 2 b_i g + (a_i - Dmax^2) <= 0 with a_i = ||mu - g_i||^2, b_i = <mu - g_i, p>, c = ||p||^2; its
+    largest root is (-b_i + sqrt(b_i^2 - c (a_i - Dmax^2))) / c, written as (Dmax^2 - a_i) / (b_i + sqrt(.)) when b_i > 0
+    (the same number without cancellation).  a_i <= Dmax^2 because mu lies in the honest hull, so every root is real and
+    >= 0; the clamps only absorb rounding.  c == 0 (all honest rows equal): gamma = 0.  NaN in, NaN out."""
+    H = np.asarray(H, dtype=np.float64)
+    n = H.shape[0]
+    mu, sd = honest_stats(H)
+    with np.errstate(invalid="ignore", over="ignore"):
+        p = -sd
+        E = mu[None, :] - H
+        a = (E * E).sum(1)
+        b = (E * p[None, :]).sum(1)
+        c = float((p * p).sum())
+        d2 = [float(((H[i] - H[j]) ** 2).sum()) for j in range(1, n) for i in range(j)]
+        D2 = max(d2, key=lambda x: (math.isnan(x), x)) if d2 else 0.0
+        if c == 0.0:
+            return 0.0
+        roots = []
+        for ai, bi in zip(a, b):
+            disc = bi * bi + c * (D2 - ai)
+            disc = 0.0 if disc < 0.0 else disc
+            r = math.sqrt(disc) if not math.isnan(disc) else math.nan
+            g = (r - bi) / c if bi <= 0.0 else (D2 - ai) / (bi + r)
+            roots.append(0.0 if g < 0.0 else g)
+    return math.nan if any(math.isnan(g) for g in roots) else min(roots)
+
+
+def minmax_row(H: np.ndarray) -> np.ndarray:
+    """The row every min-max liar sends for one tensor: mu + gamma * p = mu - gamma * sigma (fp64)."""
+    mu, sd = honest_stats(H)
+    with np.errstate(invalid="ignore"):
+        return mu - minmax_gamma(H) * sd
+
+
+def ps_attack(slots: np.ndarray, liars, mode: str, spans, z: Optional[float] = None) -> np.ndarray:
+    """Oracle of the whole PS-side step: ``slots`` [P, D] with the liar slots (0-based) replaced, per tensor span
+    ``(offset, numel)``, by the attack row built from the honest slots (fp64, rounded to the slots' dtype).  Padding outside
+    the spans is left alone."""
+    out = np.array(slots, copy=True)
+    liars = sorted(set(int(w) for w in liars))
+    honest = [w for w in range(out.shape[0]) if w not in liars]
+    if not liars or not honest:
+        return out
+    for off, numel in spans:
+        H = np.asarray(slots[honest, off:off + numel], dtype=np.float64)
+        row = alie_row(H, z) if mode == "alie" else minmax_row(H)
+        with np.errstate(over="ignore", invalid="ignore"):
+            out[liars, off:off + numel] = row.astype(out.dtype)
+    return out

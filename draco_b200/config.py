@@ -14,7 +14,7 @@ APPROACHES = ("baseline", "maj_vote", "cyclic", "detox")
 MODES = ("normal", "geometric_median", "krum", "maj_vote", "coordinate_median", "trimmed_mean", "multi_krum")
 DETOX_MODES = ("coordinate_median", "trimmed_mean", "multi_krum", "geometric_median")
 ROBUST_MAXP = 16                    # workers the fused coordinate-wise / Krum kernels take (TRIM_MAXP, KRUM_MAXP)
-ERR_MODES = ("rev_grad", "constant", "random", "omniscient", "none")
+ERR_MODES = ("rev_grad", "constant", "random", "omniscient", "alie", "minmax", "none")
 TRANSPORTS = ("nvl", "nccl", "nccl_flat", "gloo")
 
 
@@ -78,6 +78,7 @@ class JobConfig:
     push_ctas: int = 16             # CTAs of an overlapped bucket push (NVLink-bound: a handful of SMs saturates the link)
     worker_streams: int = 4         # >1: logical workers sharing a GPU run on (up to) this many concurrent CUDA streams
     zero_copy_grads: bool = True    # push reads gradients where autograd left them (pointer table), no flat gather
+    attack_z: Optional[float] = None  # --err-mode alie: z of mu - z * sigma (None: Baruch et al.'s z_max for P and f)
 
     # ---- derived --------------------------------------------------------------------------
     def resolve(self, world_size: int) -> "JobConfig":
@@ -121,10 +122,40 @@ class JobConfig:
                              "compress they only exist after the PS unpacked them -- pass --compress-grad None")
         if self.compress and self.transport == "nccl_flat":
             raise ValueError("--transport nccl_flat is the uncompressed library comparator: pass --compress-grad None")
+        self._check_ps_attack()
         if self.transport == "gloo":
             self.dtype = "fp32"
             self.cuda_graphs = False
         return self
+
+    def _check_ps_attack(self) -> None:
+        """--err-mode alie | minmax: the PS replaces the liars' slots with a row built from the honest slots."""
+        from .codes.adversary import PS_ATTACKS, alie_s
+        if self.attack_z is not None and self.err_mode != "alie":
+            raise ValueError(f"--attack-z sets ALIE's z: it needs --err-mode alie (got --err-mode {self.err_mode})")
+        if self.err_mode not in PS_ATTACKS:
+            return
+        m = self.err_mode
+        if self.approach == "cyclic":
+            raise ValueError(f"--err-mode {m} builds a real gradient row from the honest ones; the cyclic code's slots hold complex "
+                             f"codewords, so it has no meaning there -- use another --approach or --err-mode")
+        if self.transport == "nccl_flat":
+            raise ValueError(f"--transport nccl_flat implements the rev_grad and constant attacks only (got --err-mode {m})")
+        if self.worker_fail >= self.num_workers:
+            raise ValueError(f"--err-mode {m} builds the liars' row from the honest workers: it needs worker_fail < num_workers "
+                             f"(got {self.worker_fail} of {self.num_workers})")
+        if self.transport == "nvl" and self.num_workers > ROBUST_MAXP:
+            raise ValueError(f"--err-mode {m} on the nvl transport handles at most {ROBUST_MAXP} workers (got {self.num_workers}); "
+                             f"use --transport nccl for more")
+        if m == "alie" and self.attack_z is None and alie_s(self.num_workers, self.worker_fail) < 1:
+            raise ValueError(f"--err-mode alie: z_max = Phi^-1((P - s) / P) with s = floor(P/2 + 1) - f is undefined for "
+                             f"{self.num_workers} workers and worker_fail {self.worker_fail} (s < 1); pass --attack-z")
+
+    @property
+    def alie_z(self) -> float:
+        """z of the ALIE attack: --attack-z, else z_max(num_workers, worker_fail)."""
+        from .codes.adversary import alie_z_max
+        return float(self.attack_z) if self.attack_z is not None else alie_z_max(self.num_workers, self.worker_fail)
 
     def _check_detox(self) -> None:
         """DETOX runs the robust rule across the G group winners, tolerating b_G captured groups in place of f liars."""
@@ -206,7 +237,11 @@ def add_fit_args(parser: argparse.ArgumentParser) -> argparse.ArgumentParser:
            "the lowest Krum scores")
     a("--dataset", type=str, default=d.dataset)
     a("--comm-type", type=str, default=d.comm_type)
-    a("--err-mode", type=str, default=d.err_mode, help="rev_grad | constant | random | omniscient | none")
+    a("--err-mode", type=str, default=d.err_mode,
+      help="rev_grad | constant | random | omniscient | alie | minmax | none.  alie (A Little Is Enough) and minmax (min-max, "
+           "inverse-std direction) are applied by the PS per tensor from the honest workers' mean and standard deviation")
+    a("--attack-z", type=float, default=None,
+      help="--err-mode alie: the liars send mu - z * sigma (default: z_max = Phi^-1((P - s) / P), s = floor(P/2 + 1) - f)")
     a("--approach", type=str, default=d.approach,
       help="baseline | maj_vote | cyclic | detox (majority vote inside each repetition group, then --mode across the G group "
            "winners)")

@@ -109,6 +109,56 @@ def omniscient(grad_in: Addr, slot_stride: int, honest_mask: int, worker: int, m
     N.check(N.cuda().drc_omniscient(C.byref(a), grid, _stream()), "omniscient")
 
 
+# ------------------------------------------------------------------------------------------------ PS-side attacks (C12)
+ATTACK_MAXP = 16
+
+
+class AttackWorkspace:
+    """Scratch of the min-max attack: fp32 [2, D] mu / sigma, fp64 [ntiles, Q] per-tile partials, fp64 [T] gamma.  ALIE needs
+    none (one pass writes the liars' row)."""
+
+    def __init__(self, layout: ArenaLayout, P: int, device):
+        Q = 2 * P + 1 + P * (P - 1) // 2
+        self.stats = torch.zeros(2, layout.total, dtype=torch.float32, device=device)
+        self.partials = torch.zeros(layout.ntiles, Q, dtype=torch.float64, device=device)
+        self.gamma = torch.zeros(layout.ntensors, dtype=torch.float64, device=device)
+
+
+def ps_attack(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, mode: int, *, adv_bitmap: Addr, adv_len: int,
+              step_ptr: Addr, z: float = 0.0, ws: Optional[AttackWorkspace] = None, tile_range: Optional[tuple] = None,
+              tensor_range: Optional[tuple] = None, grid: Optional[int] = None) -> int:
+    """Overwrite the liar slots of the step (``adv_bitmap[*step_ptr % adv_len]``) of ``grad_in`` [P, slot_stride] with the ALIE
+    (``mode`` 5, ``z``) or min-max (``mode`` 6, workspace ``ws``) row of every tensor, built from the honest slots
+    (csrc/cuda/attack.cu).  ``tile_range`` / ``tensor_range``: one bucket (whole tensors).  Returns the kernels launched."""
+    if not 1 <= P <= ATTACK_MAXP:
+        raise ValueError(f"the PS-side attacks take 1..{ATTACK_MAXP} worker slots, got {P}")
+    if mode not in (5, 6):
+        raise ValueError(f"attack mode must be 5 (alie) or 6 (minmax), got {mode}")
+    if mode == 6 and ws is None:
+        raise ValueError("the min-max attack needs an AttackWorkspace")
+    dev = torch.device("cuda", torch.cuda.current_device())
+    a = N.AttackArgs()
+    a.grad_in, a.slot_stride, a.P, a.mode = addr(grad_in), slot_stride, P, mode
+    a.tv = layout.tile_view(dev)
+    a.adv_bitmap, a.adv_len, a.step_ptr, a.z = addr(adv_bitmap), int(adv_len) if adv_bitmap is not None else 0, addr(step_ptr), float(z)
+    if ws is not None:
+        a.stats, a.partials, a.gamma = ws.stats.data_ptr(), ws.partials.data_ptr(), ws.gamma.data_ptr()
+    ntiles = layout.ntiles
+    if tile_range is not None:
+        a.tile_begin, a.tile_end = int(tile_range[0]), int(tile_range[1])
+        ntiles = a.tile_end - a.tile_begin
+    if tensor_range is not None:
+        a.t_begin, a.t_end = int(tensor_range[0]), int(tensor_range[1])
+    g = grid or max(1, min(ntiles, sm_count() * 8))
+    lib = N.cuda()
+    N.check(lib.drc_attack_stats(C.byref(a), g, _stream()), "attack_stats")
+    if mode == 5:
+        return 1
+    N.check(lib.drc_attack_solve(C.byref(a), _stream()), "attack_solve")
+    N.check(lib.drc_attack_write(C.byref(a), g, _stream()), "attack_write")
+    return 3
+
+
 # ------------------------------------------------------------------------------------------------ vote (K3)
 def vote(layout: ArenaLayout, grad_in: Addr, slot_stride: int, group_table: torch.Tensor, neq_mask: torch.Tensor,
          winner_slot: torch.Tensor, winner_member: Optional[torch.Tensor] = None, tile_range: Optional[tuple] = None,

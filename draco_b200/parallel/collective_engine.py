@@ -19,7 +19,7 @@ from typing import Dict, Optional
 import torch
 import torch.distributed as dist
 
-from ..codes.adversary import generate_schedule
+from ..codes.adversary import PS_ATTACKS, generate_schedule
 from ..config import JobConfig
 from ..data import TensorDataset
 from ..utils.codec import compress, decompress
@@ -139,6 +139,18 @@ class CollectiveEngine:
         for w in liars:
             self.slots[w - 1].copy_(mean * self.cfg.attack_magnitude)
 
+    def _ps_attack(self, step: int) -> None:
+        """--err-mode alie | minmax: every liar slot gets the attack row of each tensor, built in fp64 from the honest slots."""
+        liars = [w - 1 for w in range(1, self.P + 1) if self.schedule.is_adversary(w, step)]
+        honest = [w for w in range(self.P) if w not in liars]
+        if not liars or not honest:
+            return
+        z = self.cfg.alie_z if self.cfg.err_mode == "alie" else 0.0
+        for s in self.layout.specs:
+            H = self.slots[honest, s.offset: s.offset + s.numel].double()
+            row = attack_row(H, self.cfg.err_mode, z).to(self.slots.dtype)
+            self.slots[liars, s.offset: s.offset + s.numel] = row
+
     def _exchange_gradients(self, step: int) -> None:
         """Per-tensor point-to-point: every remote worker -> PS."""
         L = self.layout
@@ -240,6 +252,8 @@ class CollectiveEngine:
         if self.is_ps:
             if self.use_adv and self.cfg.err_mode == "omniscient":
                 self._omniscient(step)
+            elif self.use_adv and self.cfg.err_mode in PS_ATTACKS:
+                self._ps_attack(step)
             with self._phase("t_decode"):                 # reference: "Method Time Cost"
                 grads = self.ps.aggregate(self.slots)
             with self._phase("t_update"):                 # reference: "Update Time Cost"
@@ -270,3 +284,24 @@ class CollectiveEngine:
 
     def close(self) -> None:
         pass
+
+
+def attack_row(H: torch.Tensor, mode: str, z: float = 0.0) -> torch.Tensor:
+    """The ALIE / min-max row of one tensor from its honest rows ``H`` [n_h, numel] (fp64), with the formulas and roundings of
+    the oracle (codes/adversary.py ``alie_row`` / ``minmax_gamma``): mu - z sigma, or mu - gamma sigma."""
+    n = H.shape[0]
+    mu = H.sum(0) / n
+    sd = (((H - mu) ** 2).sum(0) / n).sqrt()
+    if mode == "alie":
+        return mu - z * sd
+    p = -sd
+    c = (p * p).sum()
+    if bool(c == 0):
+        return mu.clone()
+    E = mu - H
+    a, b = (E * E).sum(1), (E * p).sum(1)
+    d2 = [((H[i] - H[j]) ** 2).sum() for j in range(1, n) for i in range(j)]
+    D2 = torch.stack(d2).max() if d2 else torch.zeros((), dtype=H.dtype, device=H.device)     # NaN propagates
+    r = (b * b + c * (D2 - a)).clamp_min(0).sqrt()
+    g = torch.where(b <= 0, (r - b) / c, (D2 - a) / (b + r)).clamp_min(0)
+    return mu - g.min() * sd

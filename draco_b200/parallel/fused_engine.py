@@ -33,7 +33,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
-from ..codes.adversary import attack_code, generate_schedule
+from ..codes.adversary import ATTACK_OMNISCIENT, PS_ATTACKS, attack_code, generate_schedule
 from ..config import JobConfig
 from ..data import BatchPlan, TensorDataset
 from ..ops import conv as _conv_ops
@@ -179,7 +179,8 @@ class FusedEngine:
             self.worker = WorkerCompute(cfg, device, self.local_workers, plan, dataset, self.layout, self.params_f32, model)
             self.worker.step_dev = self.step_dev       # dropout masks are keyed by the device step (graph replays advance it)
         if self.is_ps:
-            self.ps = FusedPS(cfg, self.layout, device, self.params_f32, self.grad_in, self.groups, self.code)
+            self.ps = FusedPS(cfg, self.layout, device, self.params_f32, self.grad_in, self.groups, self.code,
+                              adv_bitmap=self.adv_bitmap, adv_len=len(sched.ranks))
             self.dst_ptrs = [mapA[p].ptr for p in self.place.worker_procs() if p != 0]
             self.param_flag_ptrs = [mapA[p].ptr + D * 4 for p in self.place.active_procs()]
         self._dbg_buf = (torch.zeros(D * self.esize // 4, dtype=torch.float32, device=device)
@@ -206,6 +207,9 @@ class FusedEngine:
         if self.is_ps:
             got = self._dbg_ps_sums.cpu()
             exp, hv = sums.cpu(), have.cpu()
+            if self.cfg.err_mode in PS_ATTACKS and self.adv_bitmap is not None:
+                for w in self.schedule.ranks[step % len(self.schedule.ranks)]:   # slots the PS overwrote with the attack row
+                    hv[int(w) - 1] = 0
             bad = [w + 1 for w in range(self.P) if hv[w] and int(got[w]) != int(exp[w])]
             self.checksum_log.append({"step": step, "checked": int(hv.sum()), "bad": bad})
             if bad:
@@ -388,7 +392,8 @@ class FusedEngine:
                      and self.schedule.is_adversary(w, step_host))
         push_kw = dict(step_ptr=self.step_dev, worker=w - 1, done_counter=self.push_counters[w:w + 1], coef=coef,
                        adv_bitmap=self.adv_bitmap, adv_len=len(self.schedule.ranks),
-                       attack=self.attack if self.attack != 4 else 0, magnitude=cfg.attack_magnitude, seed=cfg.seed,
+                       attack=self.attack if self.attack < ATTACK_OMNISCIENT else 0,    # 4..6: not the worker's doing
+                       magnitude=cfg.attack_magnitude, seed=cfg.seed,
                        src_table=wc.ptr_dev[w] if wc.zero_copy else None)
         if self.overlap_push and not lying_now:
             # bucketed push on a side stream, overlapped with the rest of the backward pass

@@ -17,6 +17,7 @@ import numpy as np
 import torch
 
 from .. import _native as N
+from ..codes.adversary import ATTACK_ALIE, ATTACK_MINMAX, PS_ATTACKS, attack_code
 from ..codes.cyclic import CyclicCode, search_w
 from ..codes.repetition import GroupPlan
 from ..config import JobConfig
@@ -74,7 +75,8 @@ class FusedPS:
     """Kernel-driven PS state for one job (lives on the PS GPU)."""
 
     def __init__(self, cfg: JobConfig, layout: ArenaLayout, device: torch.device, params: torch.Tensor,
-                 grad_in: torch.Tensor, groups: Optional[GroupPlan], code: Optional[CyclicCode]):
+                 grad_in: torch.Tensor, groups: Optional[GroupPlan], code: Optional[CyclicCode],
+                 adv_bitmap: Optional[torch.Tensor] = None, adv_len: int = 0):
         from ..ops import kernels as K
         self.K = K
         self.cfg, self.layout, self.device = cfg, layout, device
@@ -91,6 +93,11 @@ class FusedPS:
         self.cyclic = cfg.approach == "cyclic"
         self.slot_stride = layout.total
         self.rule = select_rule(cfg)
+        # --err-mode alie | minmax: the liar slots of each bucket are overwritten after its flags and before its decode
+        self.attack = attack_code(cfg.err_mode) if cfg.err_mode in PS_ATTACKS and adv_bitmap is not None else 0
+        self.adv_bitmap, self.adv_len = adv_bitmap, adv_len
+        self.attack_z = cfg.alie_z if self.attack == ATTACK_ALIE else 0.0
+        self.attack_ws = K.AttackWorkspace(layout, self.P, device) if self.attack == ATTACK_MINMAX else None
         if self.rule == "vote" or self.rule.startswith("detox"):
             self.group_table = torch.from_numpy(groups.as_table()).to(device)
             G = self.group_table.shape[0]
@@ -153,9 +160,17 @@ class FusedPS:
                       hp=self.hp, step_ptr=step_ptr,
                       done_counter=self.counters[0:1], first_step=1, grad_out=grad_out, mc_params=mc_params, dst=dst)
         n = 0
+
+        def attack(tile_range=None, tensor_range=None) -> int:
+            if not self.attack:
+                return 0
+            return K.ps_attack(L, self.grad_in, self.slot_stride, self.P, self.attack, adv_bitmap=self.adv_bitmap,
+                               adv_len=self.adv_len, step_ptr=step_ptr, z=self.attack_z, ws=self.attack_ws,
+                               tile_range=tile_range, tensor_range=tensor_range)
         if buckets is not None and self.rule in PIPELINED_RULES:
             for bi, (t0, t1, idxs) in enumerate(buckets):
                 n += wait_bucket(bi)
+                n += attack((t0, t1), (min(idxs), max(idxs) + 1))
                 fl = flags if bi == len(buckets) - 1 else []
                 if self.rule in ("vote", "detox_median", "detox_trimmed_mean"):
                     K.vote(L, self.grad_in, self.slot_stride, self.group_table, self.neq_mask, self.winner_slot,
@@ -181,6 +196,7 @@ class FusedPS:
                                        trim=self.trim, tile_range=(t0, t1), flags=fl, **common); n += 1
             return n
         common["flags"] = flags
+        n += attack()
         _agg = K.aggregate_update
 
         def _update(*a, **kw):                             # every rule below ends in exactly one fused update kernel

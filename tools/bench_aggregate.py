@@ -8,7 +8,12 @@ broadcast destinations).  Timed with CUDA events over --iters back-to-back launc
 median round is reported.  Bandwidth is the slab bytes (P * D * 4) per microsecond, also as a share of the H100 SXM data-sheet
 HBM3 bandwidth of 3.35 TB/s (3.35e6 bytes/us); ``total_bytes_per_us`` adds the 16 * D bytes of parameter / momentum traffic.
 
-    python tools/bench_aggregate.py [--workers 7 16] [--groups 3 5 8] [--iters 200] [--rounds 3] [--out FILE]
+With --attack-workers it also times the PS-side attacks alone (csrc/cuda/attack.cu) on the same arena with --attack-fail liar
+slots: ALIE (one pass: reads the honest rows, writes the liar rows) and min-max (stats pass + per-tensor solve + write pass).
+``bytes`` counts the HBM traffic the algorithm needs: ALIE (n_h + f) * D * 4; min-max n_h * D * 4 read, 2 * D * 4 of mu / sigma
+written and read again, the fp64 per-tile partials twice, and f * D * 4 written.
+
+    python tools/bench_aggregate.py [--workers 7 16] [--groups 3 5 8] [--attack-workers 7 15] [--iters 200] [--rounds 3] [--out FILE]
 """
 from __future__ import annotations
 
@@ -36,12 +41,50 @@ def gpu_info() -> dict:
     return info
 
 
+def attack_arm(K, L, P, f, iters, rounds, dev) -> list:
+    import torch
+    from draco_b200.codes.adversary import alie_z_max
+    D, nh = L.total, P - f
+    slab = torch.randn(P, D, device=dev) * 1e-3
+    bm = torch.tensor([(1 << f) - 1], dtype=torch.int32, device=dev)          # slots 0..f-1 lie
+    step = torch.ones(1, dtype=torch.int64, device=dev)
+    ws = K.AttackWorkspace(L, P, dev)
+    Q = ws.partials.shape[1]
+    arms = {"alie": (5, (nh + f) * D * 4), "minmax": (6, (nh + 4 + f) * D * 4 + 2 * L.ntiles * Q * 8)}
+
+    def launch(mode):
+        K.ps_attack(L, slab, D, P, mode, adv_bitmap=bm, adv_len=1, step_ptr=step, z=alie_z_max(P, f), ws=ws)
+
+    for mode, _ in arms.values():
+        for _ in range(20):
+            launch(mode)
+    torch.cuda.synchronize()
+    times = {name: [] for name in arms}
+    for _ in range(rounds):
+        for name, (mode, _) in arms.items():
+            s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            s.record()
+            for _ in range(iters):
+                launch(mode)
+            e.record()
+            e.synchronize()
+            times[name].append(s.elapsed_time(e) * 1e3 / iters)
+    out = []
+    for name, ts in times.items():
+        us, nbytes = sorted(ts)[len(ts) // 2], arms[name][1]
+        out.append({"P": P, "liars": f, "attack": name, "us_per_call": round(us, 2), "us_rounds": [round(t, 2) for t in ts],
+                    "bytes": nbytes, "bytes_per_us": round(nbytes / us), "share_of_3.35TBps": round(nbytes / us / HBM_BYTES_PER_US, 3)})
+    return out
+
+
 def main() -> int:
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
-    ap.add_argument("--workers", type=int, nargs="+", default=[7, 16])
+    ap.add_argument("--workers", type=int, nargs="*", default=[7, 16])
     ap.add_argument("--trim", type=int, default=2, help="values dropped at each end by the trimmed mean (= --worker-fail)")
     ap.add_argument("--groups", type=int, nargs="*", default=[3, 5, 8], help="G of the winner-table rows (groups of 3 workers)")
     ap.add_argument("--group-trim", type=int, default=1, help="b_G of the DETOX trimmed mean (worker_fail 3, group size 3: 1)")
+    ap.add_argument("--attack-workers", type=int, nargs="*", default=[], help="P of the ALIE / min-max kernel arm (none: skipped)")
+    ap.add_argument("--attack-fail", type=int, default=3, help="liar slots of the attack arm")
     ap.add_argument("--iters", type=int, default=200)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--out", type=str, default=None, help="also append the JSON lines to this file")
@@ -109,6 +152,8 @@ def main() -> int:
                           "slab_bytes_per_us": round(slab_bytes / us), "slab_share_of_3.35TBps": round(slab_bytes / us / HBM_BYTES_PER_US, 3),
                           "total_bytes_per_us": round((slab_bytes + 16 * D) / us)})
         del slab
+    for P in a.attack_workers:
+        lines += attack_arm(K, L, P, a.attack_fail, a.iters, a.rounds, dev)
     for ln in lines:
         print(json.dumps(ln), flush=True)
     if a.out:
