@@ -14,7 +14,8 @@
 struct UpdateArgs {
   // gradient source ---------------------------------------------------------------------------
   int mode;                       // 0: select-sum over `select` table; 1: cyclic recombination; 2: real per-tensor weights;
-                                  // 3: coordinate-wise trimmed mean over K rows (see `trim`)
+                                  // 3: coordinate-wise trimmed mean over K rows (see `trim`);
+                                  // 4: Bulyan's average of the K - 2 trim values nearest the coordinate median of K rows
   const float* grad_in;           // mode 0: [P][slot_stride] fp32 ; mode 1: [n][2*slot_stride] complex64
   long long slot_stride;          // elements (fp32 words for mode 0, complex elements for mode 1)
   const int* select;              // modes 0, 2, 3: [K][T] worker slot to read for (k, tensor); null -> rows 0..K-1 for all
@@ -40,7 +41,8 @@ struct UpdateArgs {
   FlagList flags;                 // params_ready flags (peer pointers); value written = step + 1
   int tile_begin, tile_end;       // bucket of tiles to update + broadcast (tile_end == 0: whole arena)
   int trim;                       // mode 3: values dropped at each end of every coordinate (K = P <= TRIM_MAXP rows,
-                                  // scale = 1 / (P - 2 * trim)); coordinate median: trim = (P - 1) / 2
+                                  // scale = 1 / (P - 2 * trim)); coordinate median: trim = (P - 1) / 2.  Mode 4: Bulyan's f
+                                  // (K = theta = P - 2f selected rows, scale = 1 / (K - 2 * trim))
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -111,9 +113,85 @@ __device__ __forceinline__ float4 trimmed_mean_f4(const UpdateArgs& a, long long
   return make_float4(out[0], out[1], out[2], out[3]);
 }
 
-// SORT_N: mode 3 only, the sorting-network size (4, 8 or 16 >= K).  Each size is its own instantiation so that a launch pays the
+// ---------------------------------------------------------------------------------------------
+// Mode 4: Bulyan's coordinate stage (El Mhamdi, Guerraoui and Rouault, ICML 2018).  The K = theta rows named by `select`
+// (bulyan_select's choice) are sorted per coordinate as in mode 3.  m is the median in fp32: the middle value for odd K,
+// 0.5f * a + 0.5f * b of the two middle values for even K.  The beta = K - 2 trim values nearest to m are a window
+// [s, s + beta) of the sorted order with s in [0, 2 trim]: starting from s = 0, the window moves right while the value
+// entering it is strictly nearer to m than the value leaving it (distance fabsf(v - m), NaN farthest), or equal to it, so a
+// tie in distance keeps the smaller value.  The window is summed in ascending order in fp32 like mode 3.
+//
+// The entering value sits beta places after the leaving one.  beta is the same for the whole launch, so a barrel shift of
+// the sorted keys by beta (one conditional shift per bit of beta) lines them up under constant register indices; the
+// median is read the same way, through a shift by (K - 1) / 2 (a plain `r == mid` select loop is turned into an indexed
+// load by the compiler and puts the keys in local memory).
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ bool nearer(float d, float e) { return d < e || (e != e && d == d); }   // NaN farthest
+
+// sh[j] <- sh[j + n] for the bits B, 2B, ... <= N of n (padding shifts in past the end); one template level per bit so that
+// every index is a constant
+template <int N, int B>
+__device__ __forceinline__ void barrel_shift(unsigned int (&sh)[N], int n) {
+  if constexpr (B <= N) {
+    if (n & B) {
+#pragma unroll
+      for (int j = 0; j < N; ++j) sh[j] = j + B < N ? sh[j + B] : 0xFFFFFFFFu;
+    }
+    barrel_shift<N, 2 * B>(sh, n);
+  }
+}
+
+template <int N>
+__device__ __forceinline__ float4 near_median_mean_f4(const UpdateArgs& a, long long idx, int tensor) {
+  unsigned int k[4][N];
+#pragma unroll
+  for (int r = 0; r < N; ++r) {
+    if (r < a.K) {
+      const int slot = a.select[r * a.tv.ntensors + tensor];
+      const float4 v = ld_f4(reinterpret_cast<const float4*>(a.grad_in + slot * a.slot_stride + idx));
+      k[0][r] = float_key(v.x); k[1][r] = float_key(v.y); k[2][r] = float_key(v.z); k[3][r] = float_key(v.w);
+    } else {
+      k[0][r] = k[1][r] = k[2][r] = k[3][r] = 0xFFFFFFFFu;
+    }
+  }
+  const int beta = a.K - 2 * a.trim, span = 2 * a.trim;
+  float out[4];
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    sort_net<N>(k[e]);
+    unsigned int md[N];                                        // md[0], md[1] = k[e][(K - 1) / 2], k[e][(K - 1) / 2 + 1]
+#pragma unroll
+    for (int j = 0; j < N; ++j) md[j] = k[e][j];
+    barrel_shift<N, 1>(md, (a.K - 1) / 2);
+    const float lo = key_float(md[0]), hi = key_float(md[1]);
+    const float m = (a.K & 1) ? lo : __fadd_rn(__fmul_rn(0.5f, lo), __fmul_rn(0.5f, hi));
+    unsigned int sh[N];                                        // sh[j] = k[e][j + beta]
+#pragma unroll
+    for (int j = 0; j < N; ++j) sh[j] = k[e][j];
+    barrel_shift<N, 1>(sh, beta);
+    int s = 0;
+    bool moving = true;
+#pragma unroll
+    for (int j = 0; j < N - 1; ++j) {
+      if (j < span && moving) {
+        const float vin = key_float(sh[j]), vout = key_float(k[e][j]);
+        moving = nearer(fabsf(__fsub_rn(vin, m)), fabsf(__fsub_rn(vout, m))) || vin == vout || (vin != vin && vout != vout);
+        s += moving;
+      }
+    }
+    float sum = 0.f;
+#pragma unroll
+    for (int r = 0; r < N; ++r)
+      if (r >= s && r < s + beta) sum += key_float(k[e][r]);
+    out[e] = sum;
+  }
+  return make_float4(out[0], out[1], out[2], out[3]);
+}
+
+// SORT_N: modes 3 and 4, the sorting-network size (4, 8 or 16 >= K).  Each size is its own instantiation so that a launch pays the
 // registers of its own network (4 x SORT_N keys per thread), not those of the largest one.  SEL: mode 3 only, rows come through
-// the `select` table (DETOX); a separate instantiation, so the launches without a table run the code they always ran.
+// the `select` table (DETOX); a separate instantiation, so the launches without a table run the code they always ran.  Mode 4
+// always reads through the table and is instantiated as <4, N, true>.
 template <int MODE, int SORT_N = 0, bool SEL = false>
 __global__ void __launch_bounds__(DRC_THREADS) aggregate_update_kernel(const __grid_constant__ UpdateArgs a) {
   const HyperParams hp = *a.hp;
@@ -147,6 +225,8 @@ __global__ void __launch_bounds__(DRC_THREADS) aggregate_update_kernel(const __g
       }
     } else if constexpr (MODE == 3) {
       g = trimmed_mean_f4<SORT_N, SEL>(a, idx, tensor);
+    } else if constexpr (MODE == 4) {
+      g = near_median_mean_f4<SORT_N>(a, idx, tensor);
     } else {
       for (int k = 0; k < a.K; ++k) {
         const float2 v = a.recomb[tensor * a.K + k];
@@ -222,6 +302,15 @@ extern "C" int drc_aggregate_update(const UpdateArgs* args, int grid, cudaStream
   // recombination reads every worker's slot and has no use for one
   if (args->select && (args->mode == 1 || (args->mode == 2 && (args->K < 1 || args->K > TRIM_MAXP))))
     return (int)cudaErrorInvalidValue;
+  // mode 4 reads its K = theta rows through the table bulyan_select filled
+  if (args->mode == 4) {
+    if (args->K < 1 || args->K > TRIM_MAXP || args->trim < 0 || 2 * args->trim >= args->K || !args->select)
+      return (int)cudaErrorInvalidValue;
+    if (args->K <= 4) aggregate_update_kernel<4, 4, true><<<grid, DRC_THREADS, 0, stream>>>(*args);
+    else if (args->K <= 8) aggregate_update_kernel<4, 8, true><<<grid, DRC_THREADS, 0, stream>>>(*args);
+    else aggregate_update_kernel<4, 16, true><<<grid, DRC_THREADS, 0, stream>>>(*args);
+    return (int)cudaGetLastError();
+  }
   if (args->mode == 0) aggregate_update_kernel<0><<<grid, DRC_THREADS, 0, stream>>>(*args);
   else if (args->mode == 2) aggregate_update_kernel<2><<<grid, DRC_THREADS, 0, stream>>>(*args);
   else if (args->mode == 3 && args->K <= 4) launch_trimmed_mean<4>(args, grid, stream);

@@ -247,6 +247,100 @@ __global__ void krum_select_kernel(const __grid_constant__ KrumSelectArgs a) {
   for (int q = 0; q < npairs; ++q) d2[q] = 0.0;
 }
 
+// ---------------------------------------------------------------------------------------------
+// Bulyan (El Mhamdi, Guerraoui and Rouault, ICML 2018), selection stage: theta = P - 2f rounds of Krum, each moving the
+// lowest-scoring row of the remaining set R into the selection.  In a round every row i of R scores the sum of its
+// keep = max(|R| - f - 2, 0) smallest squared distances to the other rows of R (ascending, NaN last; zero terms sum to 0),
+// and the lowest score wins (NaN last, ties to the lower row).  The coordinate stage is aggregate_update MODE 4.
+//
+// One warp per tensor, lane i owns row i: it sorts its P - 1 neighbour distances once, with the neighbour's row index
+// alongside, in a compare-exchange network with constant indices.  A round then sums the first `keep` entries whose row is
+// still in R, and a warp argmin picks the winner.  Nothing is re-sorted, and every array index is a compile-time constant.
+// ---------------------------------------------------------------------------------------------
+#define BULYAN_SELECT_THREADS 128
+
+struct BulyanSelectArgs {
+  double* pair_d2;                // [T][P(P-1)/2] consumed and zeroed
+  int T, P, f;                    // P >= 4f + 3 rows, f tolerated
+  int* select;                    // [P - 2f][T] out: the worker slot chosen in round k at select[k][t]
+  const int* rows;                // [P][T] row -> worker slot (the table pair_dist read); null -> row i is slot i
+};
+
+// Distances are sums of squares (>= +0) or NaN, so their bit patterns as unsigned integers order them with NaN last once
+// every NaN is made the canonical positive one; ~0 pads the entries past the P - 1 neighbours.
+__device__ __forceinline__ unsigned long long dist_key(double d) {
+  return d != d ? 0x7FF8000000000000ull : (unsigned long long)__double_as_longlong(d);
+}
+
+// Batcher's odd-even merge sort of 16 (key, row) pairs (the 63 comparators of aggregate_update.cu's sort_net<16>), written
+// out so that every index is a constant and the pairs never leave registers
+#define CXP(x, y) {                                                                                  \
+    const bool sw_ = key[y] < key[x];                                                                \
+    const unsigned long long kx_ = sw_ ? key[y] : key[x], ky_ = sw_ ? key[x] : key[y];               \
+    const int ix_ = sw_ ? id[y] : id[x], iy_ = sw_ ? id[x] : id[y];                                  \
+    key[x] = kx_; key[y] = ky_; id[x] = ix_; id[y] = iy_; }
+__device__ __forceinline__ void sort_pairs16(unsigned long long (&key)[KRUM_MAXP], int (&id)[KRUM_MAXP]) {
+  CXP(0, 1) CXP(2, 3) CXP(4, 5) CXP(6, 7) CXP(8, 9) CXP(10, 11) CXP(12, 13) CXP(14, 15) CXP(0, 2) CXP(1, 3) CXP(4, 6)
+  CXP(5, 7) CXP(8, 10) CXP(9, 11) CXP(12, 14) CXP(13, 15) CXP(1, 2) CXP(5, 6) CXP(9, 10) CXP(13, 14) CXP(0, 4) CXP(1, 5)
+  CXP(2, 6) CXP(3, 7) CXP(8, 12) CXP(9, 13) CXP(10, 14) CXP(11, 15) CXP(2, 4) CXP(3, 5) CXP(10, 12) CXP(11, 13) CXP(1, 2)
+  CXP(3, 4) CXP(5, 6) CXP(9, 10) CXP(11, 12) CXP(13, 14) CXP(0, 8) CXP(1, 9) CXP(2, 10) CXP(3, 11) CXP(4, 12) CXP(5, 13)
+  CXP(6, 14) CXP(7, 15) CXP(4, 8) CXP(5, 9) CXP(6, 10) CXP(7, 11) CXP(2, 4) CXP(3, 5) CXP(6, 8) CXP(7, 9) CXP(10, 12)
+  CXP(11, 13) CXP(1, 2) CXP(3, 4) CXP(5, 6) CXP(7, 8) CXP(9, 10) CXP(11, 12) CXP(13, 14)
+}
+#undef CXP
+
+__global__ void __launch_bounds__(BULYAN_SELECT_THREADS) bulyan_select_kernel(const __grid_constant__ BulyanSelectArgs a) {
+  const int t = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (t >= a.T) return;                                        // whole warps: t is uniform across the warp
+  const int npairs = a.P * (a.P - 1) / 2;
+  double* d2 = a.pair_d2 + (long long)t * npairs;
+  unsigned long long key[KRUM_MAXP];
+  int id[KRUM_MAXP];
+#pragma unroll
+  for (int j = 0; j < KRUM_MAXP; ++j) {
+    key[j] = ~0ull;
+    id[j] = lane;
+    if (j < a.P && lane < a.P && j != lane) {
+      const int lo = lane < j ? lane : j, hi = lane < j ? j : lane;
+      key[j] = dist_key(d2[hi * (hi - 1) / 2 + lo]);
+      id[j] = j;
+    }
+  }
+  __syncwarp();
+  for (int q = lane; q < npairs; q += 32) d2[q] = 0.0;
+  sort_pairs16(key, id);                                       // the P - 1 neighbours first, nearest first, NaN last
+
+  const int theta = a.P - 2 * a.f;
+  unsigned int chosen = 0;                                     // rows moved out of R so far (the same in every lane)
+  for (int q = 0; q < theta; ++q) {
+    int keep = a.P - q - a.f - 2;                              // |R| = P - q
+    if (keep < 0) keep = 0;
+    double score = 0.0;
+    int n = 0;
+#pragma unroll
+    for (int x = 0; x < KRUM_MAXP - 1; ++x) {
+      if (x < a.P - 1 && !((chosen >> id[x]) & 1u) && n < keep) {
+        score += __longlong_as_double((long long)key[x]);
+        ++n;
+      }
+    }
+    // warp argmin over the rows still in R: NaN scores last, ties to the lower row
+    bool valid = lane < a.P && !((chosen >> lane) & 1u);
+    int best = lane;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const double s2 = __shfl_xor_sync(0xffffffffu, score, o);
+      const int b2 = __shfl_xor_sync(0xffffffffu, best, o);
+      const bool v2 = __shfl_xor_sync(0xffffffffu, (int)valid, o) != 0;
+      const bool take = v2 && (!valid || less_nan_last(s2, score) || (!less_nan_last(score, s2) && b2 < best));
+      if (take) { score = s2; best = b2; valid = true; }
+    }
+    chosen |= 1u << best;
+    if (lane == 0) a.select[q * a.T + t] = a.rows ? a.rows[best * a.T + t] : best;
+  }
+}
+
 extern "C" int drc_pair_dist(const PairDistArgs* args, int grid, cudaStream_t stream) {
   // with or without a row table: at most KRUM_MAXP rows (the pair table of one tensor lives in shared memory)
   if (args->P > KRUM_MAXP) return (int)cudaErrorInvalidValue;
@@ -256,6 +350,11 @@ extern "C" int drc_pair_dist(const PairDistArgs* args, int grid, cudaStream_t st
 extern "C" int drc_krum_select(const KrumSelectArgs* args, cudaStream_t stream) {
   if (args->P > KRUM_MAXP || args->m < 1 || args->m > args->P) return (int)cudaErrorInvalidValue;
   krum_select_kernel<<<(args->T + KRUM_SELECT_THREADS - 1) / KRUM_SELECT_THREADS, KRUM_SELECT_THREADS, 0, stream>>>(*args);
+  return (int)cudaGetLastError();
+}
+extern "C" int drc_bulyan_select(const BulyanSelectArgs* args, cudaStream_t stream) {
+  if (args->P > KRUM_MAXP || args->f < 0 || args->P < 4 * args->f + 3 || !args->select) return (int)cudaErrorInvalidValue;
+  bulyan_select_kernel<<<(args->T * 32 + BULYAN_SELECT_THREADS - 1) / BULYAN_SELECT_THREADS, BULYAN_SELECT_THREADS, 0, stream>>>(*args);
   return (int)cudaGetLastError();
 }
 
@@ -332,3 +431,4 @@ extern "C" int drc_sizeof_GeoMedArgs() { return (int)sizeof(GeoMedArgs); }
 extern "C" int drc_sizeof_GeoMedPrepArgs() { return (int)sizeof(GeoMedPrepArgs); }
 extern "C" int drc_sizeof_PairDistArgs() { return (int)sizeof(PairDistArgs); }
 extern "C" int drc_sizeof_KrumSelectArgs() { return (int)sizeof(KrumSelectArgs); }
+extern "C" int drc_sizeof_BulyanSelectArgs() { return (int)sizeof(BulyanSelectArgs); }

@@ -129,6 +129,10 @@ class KrumSelectArgs(C.Structure):
                 ("rows", ptr)]
 
 
+class BulyanSelectArgs(C.Structure):
+    _fields_ = [("pair_d2", ptr), ("T", C.c_int), ("P", C.c_int), ("f", C.c_int), ("select", ptr), ("rows", ptr)]
+
+
 class AttackArgs(C.Structure):
     _fields_ = [("grad_in", ptr), ("slot_stride", i64), ("P", C.c_int), ("mode", C.c_int), ("tv", TileView),
                 ("adv_bitmap", ptr), ("adv_len", C.c_int), ("step_ptr", ptr), ("z", C.c_double), ("stats", ptr),
@@ -207,6 +211,7 @@ def cuda() -> C.CDLL:
             "drc_geomed_weights": [C.POINTER(GeoMedWeightsArgs), st],
             "drc_pair_dist": [C.POINTER(PairDistArgs), C.c_int, st],
             "drc_krum_select": [C.POINTER(KrumSelectArgs), st],
+            "drc_bulyan_select": [C.POINTER(BulyanSelectArgs), st],
             "drc_attack_stats": [C.POINTER(AttackArgs), C.c_int, st],
             "drc_attack_solve": [C.POINTER(AttackArgs), st],
             "drc_attack_write": [C.POINTER(AttackArgs), C.c_int, st],

@@ -134,6 +134,73 @@ def coordinate_median(slots: np.ndarray) -> np.ndarray:
     return trimmed_mean(slots, (np.asarray(slots).shape[0] - 1) // 2)
 
 
+def bulyan_indices(slots: np.ndarray, f: int) -> List[int]:
+    """Bulyan's selection stage (El Mhamdi, Guerraoui and Rouault, *The Hidden Vulnerability of Distributed Learning in
+    Byzantium*, ICML 2018) with A = Krum, for n = P >= 4f + 3 rows: S = {A(R_1), ..., A(R_theta)}, theta = n - 2f, where R_1
+    is all rows and R_{k+1} = R_k minus the row A(R_k) picked.  Each round scores every row i of R as Krum does over R
+    (``krum_scores``: the sum of the keep = max(|R| - f - 2, 0) smallest squared distances from i to the other rows of R, NaN
+    distances last, a sum of zero terms is 0) and moves the lowest-scoring row out of R into S (NaN scores last, ties to the
+    lower row index).  Returns the row chosen in each round, in round order.
+
+    keep = |R| - f - 2 is the paper's recursion as written: R shrinks by one per round, so keep falls by one per round too.  In
+    the last round |R| = 2f + 1 and keep = f - 1, which is 0 for f <= 1: every score is then 0 and the lowest remaining row
+    index wins.  That is kept as written rather than patched."""
+    X = np.asarray(slots, dtype=np.float64)
+    P = X.shape[0]
+    if not (f >= 0 and P >= 4 * f + 3):
+        raise ValueError(f"Bulyan needs P >= 4f + 3 rows (got P = {P}, f = {f})")
+    with np.errstate(invalid="ignore", over="ignore"):                # Inf - Inf: a NaN distance, which sorts last
+        d2 = ((X[:, None, :] - X[None, :, :]) ** 2).sum(axis=2)
+    R, chosen = list(range(P)), []
+    for _ in range(P - 2 * f):
+        keep = max(len(R) - f - 2, 0)
+        scores = np.array([np.sort(d2[i, [j for j in R if j != i]])[:keep].sum() for i in R])
+        chosen.append(R.pop(int(np.argsort(scores, kind="stable")[0])))
+    return chosen
+
+
+def nearest_to_median_mean(slots: np.ndarray, b: int) -> np.ndarray:
+    """Bulyan's coordinate stage (El Mhamdi et al., ICML 2018): with beta = theta - 2f, coordinate i of the result is
+    (1 / beta) sum_{x in M_i} x, M_i = argmin_{|M| = beta} sum_{x in M} |x - median_i| over the theta selected values -- the beta
+    values closest to the coordinate median.  Here over the theta rows of ``slots``, with b = f.  Per coordinate:
+
+    * sort the theta values, -Inf < finite < +Inf < NaN (``np.sort``);
+    * m = the median: the middle value for odd theta, 0.5 a + 0.5 b of the two middle values for even theta;
+    * keep beta = theta - 2b values nearest to m (distance |v - m|, a NaN distance the farthest; a tie in distance keeps the
+      smaller value).  They form a window [s, s + beta) of the sorted order with 0 <= s <= 2b: starting from s = 0 the window
+      moves right while the value entering it is strictly nearer to m than the value leaving it, or equal to it;
+    * average the kept values.
+
+    This is not the b-trimmed mean, which keeps the middle window s = b whatever the distances."""
+    S = np.sort(np.asarray(slots, dtype=np.float64), axis=0)
+    theta = S.shape[0]
+    if not 0 <= 2 * b < theta:
+        raise ValueError(f"f = {b} leaves nothing of {theta} rows")
+    beta = theta - 2 * b
+    lo, hi = S[(theta - 1) // 2], S[theta // 2]
+    m = lo if theta % 2 else 0.5 * lo + 0.5 * hi
+    s = np.zeros(S.shape[1:], dtype=np.int64)
+    moving = np.ones(S.shape[1:], dtype=bool)
+    with np.errstate(invalid="ignore"):
+        for j in range(2 * b):
+            vin, vout = S[j + beta], S[j]
+            din, dout = np.abs(vin - m), np.abs(vout - m)
+            nearer = (din < dout) | (np.isnan(dout) & ~np.isnan(din))
+            same = (vin == vout) | (np.isnan(vin) & np.isnan(vout))
+            moving &= nearer | same
+            s += moving
+    win = np.arange(theta).reshape((theta,) + (1,) * (S.ndim - 1))
+    keep = (win >= s) & (win < s + beta)
+    return np.where(keep, S, 0.0).sum(axis=0) / beta
+
+
+def bulyan(slots: np.ndarray, f: int) -> np.ndarray:
+    """Bulyan with Krum (El Mhamdi, Guerraoui and Rouault, ICML 2018) on one tensor of P >= 4f + 3 rows:
+    ``nearest_to_median_mean`` over the theta = P - 2f rows ``bulyan_indices`` selects.  With f = 0 it is the mean of all rows."""
+    X = np.asarray(slots, dtype=np.float64)
+    return nearest_to_median_mean(X[bulyan_indices(X, f)], f)
+
+
 def captured_group_bound(worker_fail: int, group_size: int) -> int:
     """DETOX's b_G: a group of r >= ``group_size`` members returns a liar's row only when at least (r + 1) // 2 of them lie
     (fewer leave the honest rows a strict majority, which Boyer-Moore always returns; for even r, r / 2 liars can tie and win),
@@ -152,7 +219,8 @@ def detox(slots: np.ndarray, groups: Sequence[Sequence[int]], mode: str, b: int)
     ``mode`` across the G winner rows, with the tolerance b = b_G (``captured_group_bound``) in place of the worker count f:
 
     * ``coordinate_median``: trim (G - 1) // 2;   * ``trimmed_mean``: trim b;
-    * ``multi_krum``: s = b, averaging G - b rows; * ``geometric_median``: Weiszfeld over the G rows.
+    * ``multi_krum``: s = b, averaging G - b rows; * ``geometric_median``: Weiszfeld over the G rows;
+    * ``bulyan``: f = b, for G >= 4b + 3 rows.
 
     With group size 1 every worker is its own group and this is the baseline rule on the same rows."""
     X = np.asarray(slots, dtype=np.float64)
@@ -166,6 +234,8 @@ def detox(slots: np.ndarray, groups: Sequence[Sequence[int]], mode: str, b: int)
         return multi_krum(W, b, G - b)
     if mode == "geometric_median":
         return geometric_median(W)
+    if mode == "bulyan":
+        return bulyan(W, b)
     raise ValueError(f"DETOX has no rule {mode!r}")
 
 

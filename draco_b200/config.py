@@ -11,9 +11,9 @@ from dataclasses import asdict, dataclass
 from typing import Optional
 
 APPROACHES = ("baseline", "maj_vote", "cyclic", "detox")
-MODES = ("normal", "geometric_median", "krum", "maj_vote", "coordinate_median", "trimmed_mean", "multi_krum")
-DETOX_MODES = ("coordinate_median", "trimmed_mean", "multi_krum", "geometric_median")
-ROBUST_MAXP = 16                    # workers the fused coordinate-wise / Krum kernels take (TRIM_MAXP, KRUM_MAXP)
+MODES = ("normal", "geometric_median", "krum", "maj_vote", "coordinate_median", "trimmed_mean", "multi_krum", "bulyan")
+DETOX_MODES = ("coordinate_median", "trimmed_mean", "multi_krum", "geometric_median", "bulyan")
+ROBUST_MAXP = 16                    # workers the fused coordinate-wise / Krum / Bulyan kernels take (TRIM_MAXP, KRUM_MAXP)
 ERR_MODES = ("rev_grad", "constant", "random", "omniscient", "alie", "minmax", "none")
 TRANSPORTS = ("nvl", "nccl", "nccl_flat", "gloo")
 
@@ -104,13 +104,16 @@ class JobConfig:
                                  f"divides num_workers more evenly")
         if self.no_cuda:
             self.transport = "gloo"
-        if self.approach == "baseline" and self.mode in ("coordinate_median", "trimmed_mean", "multi_krum"):
+        if self.approach == "baseline" and self.mode in ("coordinate_median", "trimmed_mean", "multi_krum", "bulyan"):
             P, f = self.num_workers, self.worker_fail
-            if self.mode != "multi_krum" and 2 * f >= P:
+            if self.mode in ("coordinate_median", "trimmed_mean") and 2 * f >= P:
                 raise ValueError(f"--mode {self.mode} trims --worker-fail {f} values at each end of every coordinate: it needs "
                                  f"num_workers > 2*worker_fail (got {P} workers)")
             if self.mode == "multi_krum" and P <= 2 * f + 2:
                 raise ValueError(f"--mode multi_krum needs num_workers > 2*worker_fail + 2 (Krum's condition; got {P} workers, "
+                                 f"worker_fail {f})")
+            if self.mode == "bulyan" and P < 4 * f + 3:
+                raise ValueError(f"--mode bulyan needs num_workers >= 4*worker_fail + 3 (Bulyan's condition; got {P} workers, "
                                  f"worker_fail {f})")
             if self.transport == "nvl" and P > ROBUST_MAXP:
                 raise ValueError(f"--mode {self.mode} on the nvl transport handles at most {ROBUST_MAXP} workers (got {P}); "
@@ -169,7 +172,10 @@ class JobConfig:
         if self.mode == "multi_krum" and G <= 2 * b + 2:
             raise ValueError(f"--approach detox --mode multi_krum needs groups > 2*b_G + 2 (Krum's condition over the group "
                              f"winners; got {G} groups, b_G = worker_fail // ceil(group_size / 2) = {b})")
-        if self.mode != "multi_krum" and 2 * b >= G:
+        if self.mode == "bulyan" and G < 4 * b + 3:
+            raise ValueError(f"--approach detox --mode bulyan needs groups >= 4*b_G + 3 (Bulyan's condition over the group "
+                             f"winners; got {G} groups, b_G = worker_fail // ceil(group_size / 2) = {b})")
+        if self.mode in ("coordinate_median", "trimmed_mean", "geometric_median") and 2 * b >= G:
             raise ValueError(f"--approach detox --mode {self.mode} needs groups > 2*b_G (got {G} groups, b_G = worker_fail // "
                              f"ceil(group_size / 2) = {b} groups the liars can capture)")
         if self.transport == "nvl" and G > ROBUST_MAXP:
@@ -230,11 +236,13 @@ def add_fit_args(parser: argparse.ArgumentParser) -> argparse.ArgumentParser:
       help="time the reference's phases (Comm / Comp / Encode / Method / Update) with CUDA events each step; eager mode")
     a("--network", type=str, default=d.network)
     a("--mode", type=str, default=d.mode,
-      help="normal | geometric_median | krum | coordinate_median | trimmed_mean | multi_krum (baseline); normal | maj_vote "
-           "(maj_vote); coordinate_median | trimmed_mean | multi_krum | geometric_median (detox: the rule across the group "
-           "winners).  trimmed_mean drops --worker-fail values at each end of every coordinate (detox: b_G = worker_fail // "
-           "ceil(group_size / 2)); multi_krum averages the num_workers - worker_fail workers (detox: G - b_G group winners) with "
-           "the lowest Krum scores")
+      help="normal | geometric_median | krum | coordinate_median | trimmed_mean | multi_krum | bulyan (baseline); normal | "
+           "maj_vote (maj_vote); coordinate_median | trimmed_mean | multi_krum | geometric_median | bulyan (detox: the rule "
+           "across the group winners).  trimmed_mean drops --worker-fail values at each end of every coordinate (detox: b_G = "
+           "worker_fail // ceil(group_size / 2)); multi_krum averages the num_workers - worker_fail workers (detox: G - b_G group "
+           "winners) with the lowest Krum scores; bulyan picks num_workers - 2 worker_fail workers by repeated Krum, then "
+           "averages, per coordinate, the num_workers - 4 worker_fail picked values nearest their median (needs num_workers >= "
+           "4 worker_fail + 3; detox: G and b_G)")
     a("--dataset", type=str, default=d.dataset)
     a("--comm-type", type=str, default=d.comm_type)
     a("--err-mode", type=str, default=d.err_mode,

@@ -197,9 +197,11 @@ def aggregate_update(layout: ArenaLayout, grad_in: Addr, slot_stride: int, *, pa
                      recomb: Addr = None, first_step: int = 1, grad_out: Addr = None, mc_params: Addr = None,
                      dst: Sequence[Addr] = (), flags: Sequence[Addr] = (), grid: Optional[int] = None,
                      tile_range: Optional[tuple] = None, weights: Addr = None, exp_avg_sq: Addr = None,
-                     max_exp_avg_sq: Addr = None, trim: Optional[int] = None) -> None:
-    """Fused aggregate (select-sum, cyclic recombination, real per-tensor ``weights`` [T, K], or -- with ``trim`` -- the
-    coordinate-wise trimmed mean of K <= 16 rows that drops ``trim`` values at each end) + optimizer step (SGD-momentum, or
+                     max_exp_avg_sq: Addr = None, trim: Optional[int] = None, near_median: Optional[int] = None) -> None:
+    """Fused aggregate (select-sum, cyclic recombination, real per-tensor ``weights`` [T, K], -- with ``trim`` -- the
+    coordinate-wise trimmed mean of K <= 16 rows that drops ``trim`` values at each end, or -- with ``near_median = f`` --
+    Bulyan's coordinate stage: the mean of the K - 2f values nearest the coordinate median of the K <= 16 rows ``select``
+    names, csrc/cuda/aggregate_update.cu mode 4) + optimizer step (SGD-momentum, or
     Adam / AMSGrad when the hyper-parameter block says so: ``momentum`` = first moment, ``exp_avg_sq`` / ``max_exp_avg_sq`` = second
     moment / its running maximum) + parameter broadcast + flags.
 
@@ -222,6 +224,17 @@ def aggregate_update(layout: ArenaLayout, grad_in: Addr, slot_stride: int, *, pa
         if abs(scale * (K - 2 * trim) - 1.0) > 1e-6:
             raise ValueError(f"trimmed mean: scale must be 1 / (K - 2 * trim) = {1.0 / (K - 2 * trim)}, got {scale}")
         a.mode, a.trim = 3, int(trim)
+    if near_median is not None:
+        assert recomb is None and trim is None
+        if select is None:
+            raise ValueError("nearest-to-median mean: needs the select table of the rows bulyan_select chose")
+        _check_row_table(layout, select, K)
+        f = near_median
+        if not (1 <= K <= 16 and 0 <= 2 * f < K):
+            raise ValueError(f"nearest-to-median mean: K = {K} rows (at most 16) must exceed 2 * f = {2 * f}")
+        if abs(scale * (K - 2 * f) - 1.0) > 1e-6:
+            raise ValueError(f"nearest-to-median mean: scale must be 1 / (K - 2 * f) = {1.0 / (K - 2 * f)}, got {scale}")
+        a.mode, a.trim = 4, int(f)
     a.grad_in = addr(grad_in)
     a.slot_stride = slot_stride
     a.select = addr(select)
@@ -390,6 +403,24 @@ def krum_select(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, s:
     N.check(lib.drc_pair_dist(C.byref(pa), stream_grid(layout, 4), _stream()), "pair_dist")
     ka = N.KrumSelectArgs(pair_d2.data_ptr(), layout.ntensors, P, s, m, select.data_ptr(), addr(rows))
     N.check(lib.drc_krum_select(C.byref(ka), _stream()), "krum_select")
+
+
+def bulyan_select(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, f: int, pair_d2: torch.Tensor,
+                  select: torch.Tensor, rows: Optional[torch.Tensor] = None) -> None:
+    """Bulyan's selection stage per tensor (``oracle.bulyan_indices``): theta = P - 2f rounds of Krum over the rows not chosen
+    yet, for P >= 4f + 3 rows.  ``pair_d2``: zeroed fp64 [T, P*(P-1)/2] scratch (left zeroed); ``select``: int32 [theta, T] out,
+    the worker slot chosen in round k at ``select[k, t]`` -- pass it to ``aggregate_update(K=theta, near_median=f, select=)``.
+    ``rows``: optional int32 [P, T] table, row i of tensor t is worker slot ``rows[i, t]`` (DETOX: the vote's winner_slot)."""
+    if not (f >= 0 and 4 * f + 3 <= P <= ROW_TABLE_MAXROWS):
+        raise ValueError(f"bulyan_select: needs 4 * f + 3 <= P <= {ROW_TABLE_MAXROWS} (got P = {P}, f = {f})")
+    _check_row_table(layout, select, P - 2 * f)
+    if rows is not None:
+        _check_row_table(layout, rows, P)
+    lib = N.cuda()
+    pa = N.PairDistArgs(addr(grad_in), slot_stride, P, layout.tile_view(select.device), pair_d2.data_ptr(), addr(rows))
+    N.check(lib.drc_pair_dist(C.byref(pa), stream_grid(layout, 4), _stream()), "pair_dist")
+    ba = N.BulyanSelectArgs(pair_d2.data_ptr(), layout.ntensors, P, f, select.data_ptr(), addr(rows))
+    N.check(lib.drc_bulyan_select(C.byref(ba), _stream()), "bulyan_select")
 
 
 # ------------------------------------------------------------------------------------------------ GEMM (K10)

@@ -17,7 +17,8 @@ from typing import Iterable, List, Sequence
 import numpy as np
 import torch
 
-_MODES = ("normal", "geometric_median", "maj_vote", "cyclic", "krum", "coordinate_median", "trimmed_mean", "multi_krum")
+_MODES = ("normal", "geometric_median", "maj_vote", "cyclic", "krum", "coordinate_median", "trimmed_mean", "multi_krum",
+          "bulyan")
 
 
 def _as_tensor(g, like: torch.Tensor) -> torch.Tensor:

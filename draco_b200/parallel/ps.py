@@ -29,7 +29,8 @@ def select_rule(cfg: JobConfig) -> str:
     (cyclic_master.py:24); maj_vote approach -> vote only when ``--mode maj_vote``, plain mean for ``--mode normal``
     (rep_master.py:118-129); baseline approach -> mean / geometric median / Krum by ``--mode`` (baseline_master.py:118-129), plus
     three rules beyond the reference: coordinate-wise median, coordinate-wise trimmed mean and multi-Krum.  The detox approach
-    (beyond the reference too) votes inside every group and runs ``--mode`` across the group winners: ``detox_*`` rules."""
+    (beyond the reference too) votes inside every group and runs ``--mode`` across the group winners: ``detox_*`` rules.  Bulyan
+    (``--mode bulyan``) is beyond the reference as well."""
     if cfg.approach == "cyclic":
         return "cyclic"
     if cfg.approach == "maj_vote":
@@ -37,11 +38,11 @@ def select_rule(cfg: JobConfig) -> str:
     if cfg.approach == "detox":
         return DETOX_RULES[cfg.mode]
     return {"normal": "mean", "geometric_median": "geomedian", "krum": "krum", "coordinate_median": "median",
-            "trimmed_mean": "trimmed_mean", "multi_krum": "multi_krum"}.get(cfg.mode, "mean")
+            "trimmed_mean": "trimmed_mean", "multi_krum": "multi_krum", "bulyan": "bulyan"}.get(cfg.mode, "mean")
 
 
 DETOX_RULES = {"coordinate_median": "detox_median", "trimmed_mean": "detox_trimmed_mean", "multi_krum": "detox_multi_krum",
-               "geometric_median": "detox_geomedian"}
+               "geometric_median": "detox_geomedian", "bulyan": "detox_bulyan"}
 
 
 def coordinate_trim(cfg: JobConfig) -> int:
@@ -61,6 +62,11 @@ def detox_trim(cfg: JobConfig) -> int:
 def multi_krum_m(cfg: JobConfig) -> int:
     """Rows multi-Krum averages: P - f."""
     return cfg.num_workers - cfg.worker_fail
+
+
+def bulyan_f(cfg: JobConfig) -> int:
+    """Bulyan's tolerance: ``--worker-fail`` over the P workers, b_G over the G group winners under DETOX."""
+    return cfg.captured_group_bound if select_rule(cfg) == "detox_bulyan" else cfg.worker_fail
 
 
 def hyperparams_tensor(cfg: JobConfig, device) -> torch.Tensor:
@@ -115,6 +121,12 @@ class FusedPS:
         elif self.rule == "detox_geomedian":
             self.pair_d2 = torch.zeros(T, G * (G - 1) // 2, dtype=torch.float64, device=device)
             self.gm_weights = torch.zeros(T, G, dtype=torch.float32, device=device)
+        elif self.rule in ("bulyan", "detox_bulyan"):
+            rows = G if self.rule == "detox_bulyan" else self.P
+            self.f = bulyan_f(cfg)
+            self.theta = rows - 2 * self.f                 # rows selected per tensor; their worker slots go in `select`
+            self.pair_d2 = torch.zeros(T, rows * (rows - 1) // 2, dtype=torch.float64, device=device)
+            self.select = torch.zeros(self.theta, T, dtype=torch.int32, device=device)
         elif self.rule == "krum":
             self.pair_d2 = torch.zeros(T, self.P * (self.P - 1) // 2, dtype=torch.float64, device=device)
             self.select = torch.zeros(T, dtype=torch.int32, device=device)
@@ -218,6 +230,10 @@ class FusedPS:
             elif self.rule == "detox_geomedian":         # weights in row space, applied through the same winner table
                 K.geometric_median_weights(L, self.grad_in, self.slot_stride, G, self.pair_d2, self.gm_weights, rows=win); n += 2
                 _update(L, self.grad_in, self.slot_stride, K=G, scale=1.0, weights=self.gm_weights, select=win, **common); n += 1
+            elif self.rule == "detox_bulyan":            # select holds the worker slots of the theta winners Bulyan keeps
+                K.bulyan_select(L, self.grad_in, self.slot_stride, G, self.f, self.pair_d2, self.select, rows=win); n += 2
+                _update(L, self.grad_in, self.slot_stride, K=self.theta, scale=1.0 / (self.theta - 2 * self.f), near_median=self.f,
+                        select=self.select, **common); n += 1
             else:
                 _update(L, self.grad_in, self.slot_stride, K=G, scale=1.0 / (G - 2 * self.trim), trim=self.trim, select=win,
                         **common); n += 1
@@ -227,6 +243,10 @@ class FusedPS:
         elif self.rule == "multi_krum":
             K.krum_select(L, self.grad_in, self.slot_stride, self.P, self.cfg.worker_fail, self.pair_d2, self.select, m=self.m); n += 2
             _update(L, self.grad_in, self.slot_stride, K=self.m, scale=1.0 / self.m, select=self.select, **common); n += 1
+        elif self.rule == "bulyan":
+            K.bulyan_select(L, self.grad_in, self.slot_stride, self.P, self.f, self.pair_d2, self.select); n += 2
+            _update(L, self.grad_in, self.slot_stride, K=self.theta, scale=1.0 / (self.theta - 2 * self.f), near_median=self.f,
+                    select=self.select, **common); n += 1
         elif self.rule in ("median", "trimmed_mean"):
             _update(L, self.grad_in, self.slot_stride, K=self.P, scale=1.0 / (self.P - 2 * self.trim), trim=self.trim, **common); n += 1
         elif self.rule == "geomedian" and self.gm is None:
@@ -376,6 +396,37 @@ class TorchPS:
             acc += S[k]
         return acc * (1.0 / (P - 2 * b))
 
+    def _bulyan_tensor(self, X: torch.Tensor, f: int) -> torch.Tensor:
+        """Bulyan (``oracle.bulyan``): theta = P - 2f rounds of Krum over the rows not chosen yet (squared distances in fp64, NaN
+        last, ties to the lower row), then per coordinate the mean of the beta = theta - 2f chosen values nearest their median,
+        in fp32 with the fused kernel's window walk and ascending sum."""
+        P = X.shape[0]
+        d2 = torch.cdist(X.double(), X.double()).pow(2)
+        R, chosen = list(range(P)), []
+        for _ in range(P - 2 * f):
+            keep = max(len(R) - f - 2, 0)
+            sub = d2[R][:, R].clone()
+            sub.fill_diagonal_(float("nan"))               # sorts last; keep <= |R| - 2 never reaches it unless a real NaN does
+            scores = sub.sort(1).values[:, :keep].sum(1)
+            chosen.append(R.pop(int(torch.argsort(scores, stable=True)[0])))
+        S = X[chosen].sort(0).values
+        theta = S.shape[0]
+        beta = theta - 2 * f
+        lo, hi = S[(theta - 1) // 2], S[theta // 2]
+        m = lo if theta % 2 else 0.5 * lo + 0.5 * hi
+        s = torch.zeros(S.shape[1], dtype=torch.int64, device=S.device)
+        moving = torch.ones(S.shape[1], dtype=torch.bool, device=S.device)
+        for j in range(2 * f):                             # slide the window right while the entering value is nearer
+            vin, vout = S[j + beta], S[j]
+            din, dout = (vin - m).abs(), (vout - m).abs()
+            nearer = (din < dout) | (dout.isnan() & ~din.isnan())
+            moving &= nearer | (vin == vout) | (vin.isnan() & vout.isnan())
+            s += moving
+        acc = S.gather(0, s[None]).squeeze(0).clone()
+        for k in range(1, beta):
+            acc += S.gather(0, (s + k)[None]).squeeze(0)
+        return acc * (1.0 / beta)
+
     def _cyclic_tensor(self, R: torch.Tensor, f: torch.Tensor) -> torch.Tensor:
         """R: [n, d] complex64 -> Re(v^T R) / n with v from the C++ locator (N1 replacement)."""
         n, s = self.P, self.cfg.worker_fail
@@ -411,6 +462,8 @@ class TorchPS:
                 g = self._trimmed_mean_tensor(X)
             elif self.rule == "geomedian":
                 g = self._geomedian_tensor(X)
+            elif self.rule == "bulyan":
+                g = self._bulyan_tensor(X, self.cfg.worker_fail)
             elif self.rule.startswith("detox"):
                 winners = []                               # stage 1: the vote inside every group
                 for grp in self.groups.groups:
@@ -422,6 +475,8 @@ class TorchPS:
                     g = self._multi_krum_tensor(W, b, W.shape[0] - b)
                 elif self.rule == "detox_geomedian":
                     g = self._geomedian_tensor(W)
+                elif self.rule == "detox_bulyan":
+                    g = self._bulyan_tensor(W, self.cfg.captured_group_bound)
                 else:
                     g = self._trimmed_mean_tensor(W)
             elif self.rule == "cyclic":
@@ -438,7 +493,7 @@ class TorchPS:
         mode = {"mean": "normal", "vote": "maj_vote", "krum": "krum", "geomedian": "geometric_median", "cyclic": "cyclic",
                 "median": "coordinate_median", "trimmed_mean": "trimmed_mean", "multi_krum": "multi_krum",
                 "detox_median": "coordinate_median", "detox_trimmed_mean": "trimmed_mean", "detox_multi_krum": "multi_krum",
-                "detox_geomedian": "geometric_median"}[self.rule]
+                "detox_geomedian": "geometric_median", "bulyan": "bulyan", "detox_bulyan": "bulyan"}[self.rule]
         self.optimizer.step(grads=grads, mode=mode)
 
 

@@ -13,7 +13,14 @@ slots: ALIE (one pass: reads the honest rows, writes the liar rows) and min-max 
 ``bytes`` counts the HBM traffic the algorithm needs: ALIE (n_h + f) * D * 4; min-max n_h * D * 4 read, 2 * D * 4 of mu / sigma
 written and read again, the fp64 per-tile partials twice, and f * D * 4 written.
 
-    python tools/bench_aggregate.py [--workers 7 16] [--groups 3 5 8] [--attack-workers 7 15] [--iters 200] [--rounds 3] [--out FILE]
+With --bulyan-workers it times Bulyan against multi-Krum on the same arena, f = (P - 3) // 4 (P = 7: f = 1, P = 15: f = 3),
+each launch on its own and as the chain the PS runs after the last bucket: the pair-distance pass (shared), ``bulyan_select``
+(theta = P - 2f rounds of Krum, csrc/cuda/robust.cu) against ``krum_select`` with m = P - f, and the update kernel's mode 4
+(the beta = theta - 2f values nearest the coordinate median of theta rows) against mode 0 over the P - f multi-Krum rows and
+mode 3 over the same theta rows (the f-trimmed mean: the same sort, without the median and the window walk).
+
+    python tools/bench_aggregate.py [--workers 7 16] [--groups 3 5 8] [--attack-workers 7 15] [--bulyan-workers 7 15]
+                                    [--iters 200] [--rounds 3] [--out FILE]
 """
 from __future__ import annotations
 
@@ -77,6 +84,56 @@ def attack_arm(K, L, P, f, iters, rounds, dev) -> list:
     return out
 
 
+def bulyan_arm(K, L, P, iters, rounds, dev, update) -> list:
+    """Bulyan's three launches against multi-Krum's, timed alone and chained (see the module docstring)."""
+    import ctypes as C
+
+    import torch
+    from draco_b200 import _native as N
+    f = (P - 3) // 4
+    theta, m, T, D = P - 2 * f, P - f, L.ntensors, L.total
+    slab = torch.randn(P, D, device=dev) * 1e-3
+    pair = torch.zeros(T, P * (P - 1) // 2, dtype=torch.float64, device=dev)
+    sel_b = torch.zeros(theta, T, dtype=torch.int32, device=dev)
+    sel_k = torch.zeros(m, T, dtype=torch.int32, device=dev)
+    K.bulyan_select(L, slab, D, P, f, pair, sel_b)
+    K.krum_select(L, slab, D, P, f, pair, sel_k, m=m)
+    lib, tv = N.cuda(), L.tile_view(dev)
+    pa = N.PairDistArgs(slab.data_ptr(), D, P, tv, pair.data_ptr(), None)
+    ba = N.BulyanSelectArgs(pair.data_ptr(), T, P, f, sel_b.data_ptr(), None)
+    ka = N.KrumSelectArgs(pair.data_ptr(), T, P, f, m, sel_k.data_ptr(), None)
+    grid = K.stream_grid(L, 4)
+    arms = {
+        "pair_dist": lambda: lib.drc_pair_dist(C.byref(pa), grid, K._stream()),
+        "bulyan_select": lambda: lib.drc_bulyan_select(C.byref(ba), K._stream()),
+        "krum_select_m": lambda: lib.drc_krum_select(C.byref(ka), K._stream()),
+        "mode4_near_median": lambda: update(slab, dict(K=theta, scale=1.0 / (theta - 2 * f), near_median=f, select=sel_b)),
+        "mode3_trimmed_theta": lambda: update(slab, dict(K=theta, scale=1.0 / (theta - 2 * f), trim=f, select=sel_b)),
+        "mode0_multi_krum": lambda: update(slab, dict(K=m, scale=1.0 / m, select=sel_k)),
+        "bulyan_chain": lambda: (K.bulyan_select(L, slab, D, P, f, pair, sel_b),
+                                 update(slab, dict(K=theta, scale=1.0 / (theta - 2 * f), near_median=f, select=sel_b))),
+        "multi_krum_chain": lambda: (K.krum_select(L, slab, D, P, f, pair, sel_k, m=m),
+                                     update(slab, dict(K=m, scale=1.0 / m, select=sel_k))),
+    }
+    for fn in arms.values():
+        for _ in range(20):
+            fn()
+    torch.cuda.synchronize()
+    times = {name: [] for name in arms}
+    for _ in range(rounds):
+        for name, fn in arms.items():
+            s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            s.record()
+            for _ in range(iters):
+                fn()
+            e.record()
+            e.synchronize()
+            times[name].append(s.elapsed_time(e) * 1e3 / iters)
+    pair.zero_()
+    return [{"P": P, "f": f, "theta": theta, "arm": name, "us_per_call": round(sorted(ts)[len(ts) // 2], 2),
+             "us_rounds": [round(t, 2) for t in ts]} for name, ts in times.items()]
+
+
 def main() -> int:
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--workers", type=int, nargs="*", default=[7, 16])
@@ -85,6 +142,7 @@ def main() -> int:
     ap.add_argument("--group-trim", type=int, default=1, help="b_G of the DETOX trimmed mean (worker_fail 3, group size 3: 1)")
     ap.add_argument("--attack-workers", type=int, nargs="*", default=[], help="P of the ALIE / min-max kernel arm (none: skipped)")
     ap.add_argument("--attack-fail", type=int, default=3, help="liar slots of the attack arm")
+    ap.add_argument("--bulyan-workers", type=int, nargs="*", default=[], help="P of the Bulyan / multi-Krum arm (none: skipped)")
     ap.add_argument("--iters", type=int, default=200)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--out", type=str, default=None, help="also append the JSON lines to this file")
@@ -154,6 +212,11 @@ def main() -> int:
         del slab
     for P in a.attack_workers:
         lines += attack_arm(K, L, P, a.attack_fail, a.iters, a.rounds, dev)
+
+    def update(slab, kw):
+        K.aggregate_update(L, slab, D, params=params, momentum=mom, hp=hp, step_ptr=step, done_counter=cnt[0:1], **kw)
+    for P in a.bulyan_workers:
+        lines += bulyan_arm(K, L, P, a.iters, a.rounds, dev, update)
     for ln in lines:
         print(json.dumps(ln), flush=True)
     if a.out:
