@@ -43,6 +43,10 @@ struct UpdateArgs {
   int trim;                       // mode 3: values dropped at each end of every coordinate (K = P <= TRIM_MAXP rows,
                                   // scale = 1 / (P - 2 * trim)); coordinate median: trim = (P - 1) / 2.  Mode 4: Bulyan's f
                                   // (K = theta = P - 2f selected rows, scale = 1 / (K - 2 * trim))
+  // nearest-neighbour mixing in front of modes 3 and 4 (appended: the fields above keep their offsets) ------------------
+  const unsigned int* mix;        // [mixP][T] neighbour masks of nnm_mix (bit j = raw row j is in N_i), or null: no mixing
+  int mixP;                       // raw rows P (slots 0..P-1); mode 3 sorts K = P mixed rows, mode 4 the K = theta of `select`
+  float mix_scale;                // fp32(1 / n_mix), n_mix = P - f
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -85,6 +89,18 @@ template <> __device__ __forceinline__ void sort_net<16>(unsigned int (&k)[16]) 
   CX(5, 6) CX(7, 8) CX(9, 10) CX(11, 12) CX(13, 14)
 }
 #undef CX
+
+// One coordinate of mode 3 (trimmed_sum) and of mode 4 (near_median_sum) for the mixed path: the same steps as the loops of
+// trimmed_mean_f4 and near_median_mean_f4, which keep their own copies so that the unmixed kernels compile as before.
+template <int N>
+__device__ __forceinline__ float trimmed_sum(unsigned int (&k)[N], int K, int trim) {
+  sort_net<N>(k);
+  float s = 0.f;
+#pragma unroll
+  for (int r = 0; r < N; ++r)
+    if (r >= trim && r < K - trim) s += key_float(k[r]);
+  return s;
+}
 
 // SEL: row r of `tensor` is worker slot select[r][tensor] instead of slot r
 template <int N, bool SEL>
@@ -142,6 +158,37 @@ __device__ __forceinline__ void barrel_shift(unsigned int (&sh)[N], int n) {
 }
 
 template <int N>
+__device__ __forceinline__ float near_median_sum(unsigned int (&k)[N], int K, int trim) {
+  const int beta = K - 2 * trim, span = 2 * trim;
+  sort_net<N>(k);
+  unsigned int md[N];                                          // md[0], md[1] = k[(K - 1) / 2], k[(K - 1) / 2 + 1]
+#pragma unroll
+  for (int j = 0; j < N; ++j) md[j] = k[j];
+  barrel_shift<N, 1>(md, (K - 1) / 2);
+  const float lo = key_float(md[0]), hi = key_float(md[1]);
+  const float m = (K & 1) ? lo : __fadd_rn(__fmul_rn(0.5f, lo), __fmul_rn(0.5f, hi));
+  unsigned int sh[N];                                          // sh[j] = k[j + beta]
+#pragma unroll
+  for (int j = 0; j < N; ++j) sh[j] = k[j];
+  barrel_shift<N, 1>(sh, beta);
+  int s = 0;
+  bool moving = true;
+#pragma unroll
+  for (int j = 0; j < N - 1; ++j) {
+    if (j < span && moving) {
+      const float vin = key_float(sh[j]), vout = key_float(k[j]);
+      moving = nearer(fabsf(__fsub_rn(vin, m)), fabsf(__fsub_rn(vout, m))) || vin == vout || (vin != vin && vout != vout);
+      s += moving;
+    }
+  }
+  float sum = 0.f;
+#pragma unroll
+  for (int r = 0; r < N; ++r)
+    if (r >= s && r < s + beta) sum += key_float(k[r]);
+  return sum;
+}
+
+template <int N>
 __device__ __forceinline__ float4 near_median_mean_f4(const UpdateArgs& a, long long idx, int tensor) {
   unsigned int k[4][N];
 #pragma unroll
@@ -188,11 +235,50 @@ __device__ __forceinline__ float4 near_median_mean_f4(const UpdateArgs& a, long 
   return make_float4(out[0], out[1], out[2], out[3]);
 }
 
+// ---------------------------------------------------------------------------------------------
+// Modes 3 and 4 behind nearest-neighbour mixing (MIX; robust.cu nnm_mix_kernel).  The thread loads the mixP raw rows (slots
+// 0..mixP-1) once.  Per coordinate, mixed row i is formed in fp32 exactly as
+//     y = +0.0f;  for j = 0, 1, ..., mixP - 1 in ascending order: if bit j of mask_i is set, y = y + x_j  (round to nearest);
+//     y = y * mix_scale  (one rounded multiply, mix_scale = fp32(1 / n_mix)),
+// with mask_i = mix[i][t] for mode 3 (the K = mixP mixed rows) and mask_r = mix[select[r][t]][t] for mode 4 (the K = theta
+// mixed rows bulyan_select chose).  The K mixed values are then sorted and reduced exactly as modes 3 and 4 do without
+// mixing.  The raw rows stay in registers (N = SORT_N >= mixP float4s); the keys are built one coordinate at a time.
+// ---------------------------------------------------------------------------------------------
+template <int MODE, int N>
+__device__ __forceinline__ float4 mixed_robust_f4(const UpdateArgs& a, long long idx, int tensor) {
+  const int T = a.tv.ntensors;
+  float4 x[N];
+#pragma unroll
+  for (int j = 0; j < N; ++j)
+    if (j < a.mixP) x[j] = ld_f4(reinterpret_cast<const float4*>(a.grad_in + j * a.slot_stride + idx));
+  unsigned int mask[N];
+#pragma unroll
+  for (int r = 0; r < N; ++r) mask[r] = r < a.K ? a.mix[(MODE == 4 ? a.select[r * T + tensor] : r) * T + tensor] : 0u;
+  float out[4];
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    unsigned int k[N];
+#pragma unroll
+    for (int r = 0; r < N; ++r) {
+      float y = 0.f;
+#pragma unroll
+      for (int j = 0; j < N; ++j) {
+        const float v = e == 0 ? x[j].x : e == 1 ? x[j].y : e == 2 ? x[j].z : x[j].w;
+        if (j < a.mixP && ((mask[r] >> j) & 1u)) y = __fadd_rn(y, v);
+      }
+      k[r] = r < a.K ? float_key(__fmul_rn(y, a.mix_scale)) : 0xFFFFFFFFu;
+    }
+    out[e] = MODE == 3 ? trimmed_sum<N>(k, a.K, a.trim) : near_median_sum<N>(k, a.K, a.trim);
+  }
+  return make_float4(out[0], out[1], out[2], out[3]);
+}
+
 // SORT_N: modes 3 and 4, the sorting-network size (4, 8 or 16 >= K).  Each size is its own instantiation so that a launch pays the
 // registers of its own network (4 x SORT_N keys per thread), not those of the largest one.  SEL: mode 3 only, rows come through
 // the `select` table (DETOX); a separate instantiation, so the launches without a table run the code they always ran.  Mode 4
-// always reads through the table and is instantiated as <4, N, true>.
-template <int MODE, int SORT_N = 0, bool SEL = false>
+// always reads through the table and is instantiated as <4, N, true>.  MIX: modes 3 and 4 over nearest-neighbour mixed rows
+// (mixed_robust_f4), instantiated as <3, N, false, true> and <4, N, true, true> with N >= mixP.
+template <int MODE, int SORT_N = 0, bool SEL = false, bool MIX = false>
 __global__ void __launch_bounds__(DRC_THREADS) aggregate_update_kernel(const __grid_constant__ UpdateArgs a) {
   const HyperParams hp = *a.hp;
   const unsigned long long step = *a.step_ptr;
@@ -223,6 +309,8 @@ __global__ void __launch_bounds__(DRC_THREADS) aggregate_update_kernel(const __g
         float4 v = ld_f4(reinterpret_cast<const float4*>(a.grad_in + slot * a.slot_stride + idx));
         g.x = fmaf(w, v.x, g.x); g.y = fmaf(w, v.y, g.y); g.z = fmaf(w, v.z, g.z); g.w = fmaf(w, v.w, g.w);
       }
+    } else if constexpr (MIX) {
+      g = mixed_robust_f4<MODE, SORT_N>(a, idx, tensor);
     } else if constexpr (MODE == 3) {
       g = trimmed_mean_f4<SORT_N, SEL>(a, idx, tensor);
     } else if constexpr (MODE == 4) {
@@ -294,8 +382,24 @@ static void launch_trimmed_mean(const UpdateArgs* args, int grid, cudaStream_t s
   else aggregate_update_kernel<3, N, false><<<grid, DRC_THREADS, 0, stream>>>(*args);
 }
 
+template <int MODE>
+static void launch_mixed(const UpdateArgs* args, int grid, cudaStream_t stream) {
+  if (args->mixP <= 4) aggregate_update_kernel<MODE, 4, MODE == 4, true><<<grid, DRC_THREADS, 0, stream>>>(*args);
+  else if (args->mixP <= 8) aggregate_update_kernel<MODE, 8, MODE == 4, true><<<grid, DRC_THREADS, 0, stream>>>(*args);
+  else aggregate_update_kernel<MODE, 16, MODE == 4, true><<<grid, DRC_THREADS, 0, stream>>>(*args);
+}
+
 extern "C" int drc_aggregate_update(const UpdateArgs* args, int grid, cudaStream_t stream) {
   if (args->ndst > DRC_MAX_DST || args->flags.n > DRC_MAX_DST) return (int)cudaErrorInvalidValue;
+  // nearest-neighbour mixing: modes 3 (K = mixP mixed rows, no row table) and 4 (K = theta mixed rows named by `select`)
+  if (args->mix) {
+    if (args->mixP < 1 || args->mixP > TRIM_MAXP || !(args->mix_scale > 0.f) || args->trim < 0 || 2 * args->trim >= args->K)
+      return (int)cudaErrorInvalidValue;
+    if (args->mode == 3 && args->K == args->mixP && !args->select) launch_mixed<3>(args, grid, stream);
+    else if (args->mode == 4 && args->K >= 1 && args->K <= args->mixP && args->select) launch_mixed<4>(args, grid, stream);
+    else return (int)cudaErrorInvalidValue;
+    return (int)cudaGetLastError();
+  }
   if (args->mode == 3 && (args->K < 1 || args->K > TRIM_MAXP || args->trim < 0 || 2 * args->trim >= args->K))
     return (int)cudaErrorInvalidValue;
   // a row table names at most TRIM_MAXP rows under the weighted sum (the weight-space geometric median's limit); the cyclic

@@ -341,6 +341,158 @@ __global__ void __launch_bounds__(BULYAN_SELECT_THREADS) bulyan_select_kernel(co
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// Nearest-neighbour mixing (Allouah, Farhadkhani, Guerraoui, Gupta, Pinot and Stephan, AISTATS 2023), per tensor: with
+// n_mix = P - f, mixed row y_i is the mean of the rows of N_i = {i} + the n_mix - 1 rows nearest to row i (squared distance,
+// ascending, NaN last, ties to the lower row; row i itself comes first even when another row duplicates it).
+//
+// nnm_mix_kernel: one warp per tensor, lane i owns row i.  It sorts row i's P - 1 neighbour distances with sort_pairs16,
+// takes the (n_mix - 1)-th key as a threshold and keeps every neighbour below it plus, among the neighbours equal to it, the
+// lowest rows (the network is not stable, so ties are resolved on the row index, not on the sorted position).  The bitmask
+// of N_i goes to mix[i][t].  Every mixed row is a fixed combination y = A x / n_mix of the raw rows, so for
+// c = (a_i - a_k) / n_mix (which sums to 0), ||y_i - y_k||^2 = -1/2 c^T D c with D the raw table: with u_i = D a_i (lane i
+// gathers the rows D[j] of its neighbours through shuffles), S_i = a_i^T u_i and Q_ik = a_k^T u_i,
+//     ||y_i - y_k||^2 = (2 Q_ik - S_i - S_k) / (2 n_mix^2),
+// in fp64 and clamped at 0 (a NaN stays NaN).  With `mixed_out` the kernel overwrites the raw table with the mixed one for
+// krum_select / bulyan_select / geomed_weights, which consume and zero it as usual; without, it zeroes the table (the
+// coordinate rules need only the masks).  O(P^3) fp64 work per tensor, no pass over the slab.
+// ---------------------------------------------------------------------------------------------
+#define NNM_THREADS 128
+
+struct NnmMixArgs {
+  double* pair_d2;                // [T][P(P-1)/2] in: raw squared distances; out: the mixed table (mixed_out) or zeros
+  int T, P, f;                    // n_mix = P - f rows per neighbourhood, 0 <= f < P <= KRUM_MAXP
+  unsigned int* mix;              // [P][T] out: bit j of mix[i][t] = row j is in N_i
+  int mixed_out;                  // 1: write the mixed table; 0: zero the table
+};
+
+__global__ void __launch_bounds__(NNM_THREADS) nnm_mix_kernel(const __grid_constant__ NnmMixArgs a) {
+  const int t = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (t >= a.T) return;                                        // whole warps: t is uniform across the warp
+  const int npairs = a.P * (a.P - 1) / 2;
+  double* d2 = a.pair_d2 + (long long)t * npairs;
+  unsigned long long key[KRUM_MAXP];
+  int id[KRUM_MAXP];
+#pragma unroll
+  for (int j = 0; j < KRUM_MAXP; ++j) {
+    key[j] = ~0ull;                                            // self and padding sort after every neighbour
+    id[j] = j;
+    if (j < a.P && lane < a.P && j != lane) {
+      const int lo = lane < j ? lane : j, hi = lane < j ? j : lane;
+      key[j] = dist_key(d2[hi * (hi - 1) / 2 + lo]);
+    }
+  }
+  sort_pairs16(key, id);                                       // the P - 1 neighbours first, nearest first, NaN last
+  const int need = a.P - a.f - 1;                              // neighbours besides row i itself
+  unsigned long long thr = 0;                                  // key of the need-th nearest neighbour
+#pragma unroll
+  for (int x = 0; x < KRUM_MAXP - 1; ++x) if (x < need) thr = key[x];
+  int below = 0;
+#pragma unroll
+  for (int x = 0; x < KRUM_MAXP - 1; ++x) below += x < need && key[x] < thr;
+  unsigned int mask = 1u << lane;
+#pragma unroll
+  for (int x = 0; x < KRUM_MAXP - 1; ++x) {
+    int lower_ties = 0;                                        // neighbours with the threshold key and a lower row index
+#pragma unroll
+    for (int y = 0; y < KRUM_MAXP - 1; ++y) lower_ties += key[y] == thr && id[y] < id[x];
+    const bool in = need > 0 && (key[x] < thr || (key[x] == thr && lower_ties < need - below));
+    if (in) mask |= 1u << id[x];
+  }
+  if (lane >= a.P) mask = 0;
+  if (lane < a.P) a.mix[lane * a.T + t] = mask;
+
+  if (a.mixed_out) {
+    double row[KRUM_MAXP];                                     // row[l] = D[lane][l] (0 on the diagonal and past P)
+#pragma unroll
+    for (int l = 0; l < KRUM_MAXP; ++l) {
+      row[l] = 0.0;
+      if (l < a.P && lane < a.P && l != lane) {
+        const int lo = lane < l ? lane : l, hi = lane < l ? l : lane;
+        row[l] = d2[hi * (hi - 1) / 2 + lo];
+      }
+    }
+    __syncwarp();                                              // every lane has read its row before any lane writes
+    double u[KRUM_MAXP];                                       // u[l] = sum over j in N_lane of D[j][l]
+#pragma unroll
+    for (int l = 0; l < KRUM_MAXP; ++l) u[l] = 0.0;
+#pragma unroll
+    for (int j = 0; j < KRUM_MAXP; ++j) {
+      if (j < a.P) {
+        const bool nb = (mask >> j) & 1u;
+#pragma unroll
+        for (int l = 0; l < KRUM_MAXP; ++l) {
+          const double v = __shfl_sync(0xffffffffu, row[l], j);
+          if (nb && l < a.P) u[l] += v;
+        }
+      }
+    }
+    double self = 0.0;                                         // S_lane = a_lane^T D a_lane
+#pragma unroll
+    for (int l = 0; l < KRUM_MAXP; ++l) if ((mask >> l) & 1u) self += u[l];
+    const double inv = 1.0 / (2.0 * (double)(a.P - a.f) * (double)(a.P - a.f));
+#pragma unroll
+    for (int k = 1; k < KRUM_MAXP; ++k) {
+      const unsigned int mk = __shfl_sync(0xffffffffu, mask, k);
+      const double sk = __shfl_sync(0xffffffffu, self, k);
+      double q = 0.0;                                          // Q_lane,k = a_k^T D a_lane
+#pragma unroll
+      for (int l = 0; l < KRUM_MAXP; ++l) if ((mk >> l) & 1u) q += u[l];
+      if (lane < k && k < a.P) {
+        double v = (2.0 * q - self - sk) * inv;
+        if (v < 0.0) v = 0.0;                                  // cancellation; a NaN fails the test and stays NaN
+        d2[k * (k - 1) / 2 + lane] = v;
+      }
+    }
+  } else {
+    __syncwarp();
+    for (int q = lane; q < npairs; q += 32) d2[q] = 0.0;
+  }
+}
+
+// nnm_fold_kernel: a choice made over the mixed rows, as weights over the raw rows: w_raw[t][j] = (1 / n_mix) sum over i with
+// j in N_i of w_mix[i], summed in fp64.  w_mix is 1/m on the m mixed rows `select` names (Krum m = 1, multi-Krum m = P - f),
+// or the fp32 weights [T][P] of geomed_weights.  aggregate_update MODE 2 (K = P, no row table) then applies w_raw.
+struct NnmFoldArgs {
+  const unsigned int* mix;        // [P][T] neighbour masks from nnm_mix_kernel
+  int T, P, f;
+  const int* select;              // [m][T] mixed rows chosen (uniform weight 1/m), or null: use w_mix
+  int m;
+  const float* w_mix;             // [T][P] weights over the mixed rows (select == null)
+  float* w_raw;                   // [T][P] out
+};
+
+__global__ void nnm_fold_kernel(const __grid_constant__ NnmFoldArgs a) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= a.T * a.P) return;
+  const int t = g / a.P, j = g - t * a.P;
+  double acc = 0.0;
+  if (a.select) {
+    const double w = 1.0 / a.m;
+    for (int r = 0; r < a.m; ++r)
+      if ((a.mix[a.select[r * a.T + t] * a.T + t] >> j) & 1u) acc += w;
+  } else {
+    for (int i = 0; i < a.P; ++i)
+      if ((a.mix[i * a.T + t] >> j) & 1u) acc += (double)a.w_mix[t * a.P + i];
+  }
+  a.w_raw[t * a.P + j] = (float)(acc / (double)(a.P - a.f));
+}
+
+extern "C" int drc_nnm_mix(const NnmMixArgs* args, cudaStream_t stream) {
+  if (args->P < 1 || args->P > KRUM_MAXP || args->f < 0 || args->f >= args->P || !args->mix || !args->pair_d2)
+    return (int)cudaErrorInvalidValue;
+  nnm_mix_kernel<<<(args->T * 32 + NNM_THREADS - 1) / NNM_THREADS, NNM_THREADS, 0, stream>>>(*args);
+  return (int)cudaGetLastError();
+}
+extern "C" int drc_nnm_fold(const NnmFoldArgs* args, cudaStream_t stream) {
+  if (args->P < 1 || args->P > KRUM_MAXP || args->f < 0 || args->f >= args->P || !args->mix || !args->w_raw)
+    return (int)cudaErrorInvalidValue;
+  if (args->select ? (args->m < 1 || args->m > args->P) : !args->w_mix) return (int)cudaErrorInvalidValue;
+  nnm_fold_kernel<<<(args->T * args->P + 127) / 128, 128, 0, stream>>>(*args);
+  return (int)cudaGetLastError();
+}
+
 extern "C" int drc_pair_dist(const PairDistArgs* args, int grid, cudaStream_t stream) {
   // with or without a row table: at most KRUM_MAXP rows (the pair table of one tensor lives in shared memory)
   if (args->P > KRUM_MAXP) return (int)cudaErrorInvalidValue;
@@ -432,3 +584,5 @@ extern "C" int drc_sizeof_GeoMedPrepArgs() { return (int)sizeof(GeoMedPrepArgs);
 extern "C" int drc_sizeof_PairDistArgs() { return (int)sizeof(PairDistArgs); }
 extern "C" int drc_sizeof_KrumSelectArgs() { return (int)sizeof(KrumSelectArgs); }
 extern "C" int drc_sizeof_BulyanSelectArgs() { return (int)sizeof(BulyanSelectArgs); }
+extern "C" int drc_sizeof_NnmMixArgs() { return (int)sizeof(NnmMixArgs); }
+extern "C" int drc_sizeof_NnmFoldArgs() { return (int)sizeof(NnmFoldArgs); }

@@ -75,7 +75,8 @@ class UpdateArgs(C.Structure):
                 ("scale", C.c_float), ("recomb", ptr), ("tv", TileView), ("params", ptr), ("momentum", ptr),
                 ("exp_avg_sq", ptr), ("max_exp_avg_sq", ptr), ("hp", ptr), ("step_ptr", ptr), ("first_step", u64), ("grad_out", ptr), ("mc_params", ptr),
                 ("dst", ptr * MAX_DST), ("ndst", C.c_int), ("done_counter", ptr), ("flags", FlagList),
-                ("tile_begin", C.c_int), ("tile_end", C.c_int), ("trim", C.c_int)]
+                ("tile_begin", C.c_int), ("tile_end", C.c_int), ("trim", C.c_int),
+                ("mix", ptr), ("mixP", C.c_int), ("mix_scale", C.c_float)]
 
 
 class StreamPushArgs(C.Structure):
@@ -131,6 +132,15 @@ class KrumSelectArgs(C.Structure):
 
 class BulyanSelectArgs(C.Structure):
     _fields_ = [("pair_d2", ptr), ("T", C.c_int), ("P", C.c_int), ("f", C.c_int), ("select", ptr), ("rows", ptr)]
+
+
+class NnmMixArgs(C.Structure):
+    _fields_ = [("pair_d2", ptr), ("T", C.c_int), ("P", C.c_int), ("f", C.c_int), ("mix", ptr), ("mixed_out", C.c_int)]
+
+
+class NnmFoldArgs(C.Structure):
+    _fields_ = [("mix", ptr), ("T", C.c_int), ("P", C.c_int), ("f", C.c_int), ("select", ptr), ("m", C.c_int),
+                ("w_mix", ptr), ("w_raw", ptr)]
 
 
 class AttackArgs(C.Structure):
@@ -212,6 +222,8 @@ def cuda() -> C.CDLL:
             "drc_pair_dist": [C.POINTER(PairDistArgs), C.c_int, st],
             "drc_krum_select": [C.POINTER(KrumSelectArgs), st],
             "drc_bulyan_select": [C.POINTER(BulyanSelectArgs), st],
+            "drc_nnm_mix": [C.POINTER(NnmMixArgs), st],
+            "drc_nnm_fold": [C.POINTER(NnmFoldArgs), st],
             "drc_attack_stats": [C.POINTER(AttackArgs), C.c_int, st],
             "drc_attack_solve": [C.POINTER(AttackArgs), st],
             "drc_attack_write": [C.POINTER(AttackArgs), C.c_int, st],

@@ -69,8 +69,11 @@ def geometric_median_weights(slots: np.ndarray, eps: float = 1e-10, max_iter: in
     csrc/cuda/robust.cu).  Every iterate is ``m = w @ X`` with ``sum(w) = 1``, for which
     ``||x_i - m||^2 = (D w)_i - w^T D w / 2`` with ``D_ij = ||x_i - x_j||^2`` -- the data is touched once (for D)."""
     X = np.asarray(slots, dtype=np.float64)
-    P = X.shape[0]
-    D = ((X[:, None, :] - X[None, :, :]) ** 2).sum(axis=2)
+    return _weiszfeld_weights(((X[:, None, :] - X[None, :, :]) ** 2).sum(axis=2), eps, max_iter)
+
+
+def _weiszfeld_weights(D: np.ndarray, eps: float, max_iter: int) -> np.ndarray:
+    P = D.shape[0]
     w = np.full(P, 1.0 / P)
     if D.max() <= 0:
         return w
@@ -101,9 +104,12 @@ def krum_scores(slots: np.ndarray, s: int) -> np.ndarray:
     """score_i of ``krum_index``: the sum of the (P - s - 2) smallest squared distances from row i to the others (NaN
     distances sort last)."""
     X = np.asarray(slots, dtype=np.float64)
-    P = X.shape[0]
+    return _krum_scores_d2(((X[:, None, :] - X[None, :, :]) ** 2).sum(axis=2), s)
+
+
+def _krum_scores_d2(d2: np.ndarray, s: int) -> np.ndarray:
+    P = d2.shape[0]
     keep = max(P - s - 2, 0)
-    d2 = ((X[:, None, :] - X[None, :, :]) ** 2).sum(axis=2)
     return np.array([np.sort(np.delete(d2[i], i))[:keep].sum() for i in range(P)])
 
 
@@ -151,6 +157,11 @@ def bulyan_indices(slots: np.ndarray, f: int) -> List[int]:
         raise ValueError(f"Bulyan needs P >= 4f + 3 rows (got P = {P}, f = {f})")
     with np.errstate(invalid="ignore", over="ignore"):                # Inf - Inf: a NaN distance, which sorts last
         d2 = ((X[:, None, :] - X[None, :, :]) ** 2).sum(axis=2)
+    return _bulyan_rounds(d2, f)
+
+
+def _bulyan_rounds(d2: np.ndarray, f: int) -> List[int]:
+    P = d2.shape[0]
     R, chosen = list(range(P)), []
     for _ in range(P - 2 * f):
         keep = max(len(R) - f - 2, 0)
@@ -199,6 +210,106 @@ def bulyan(slots: np.ndarray, f: int) -> np.ndarray:
     ``nearest_to_median_mean`` over the theta = P - 2f rows ``bulyan_indices`` selects.  With f = 0 it is the mean of all rows."""
     X = np.asarray(slots, dtype=np.float64)
     return nearest_to_median_mean(X[bulyan_indices(X, f)], f)
+
+
+NNM_MODES = ("coordinate_median", "trimmed_mean", "krum", "multi_krum", "geometric_median", "bulyan")
+
+
+def _raw_d2(slots: np.ndarray) -> np.ndarray:
+    """Squared distances between the rows, in fp64 from the (fp32) inputs; the diagonal is 0."""
+    X = np.asarray(slots, dtype=np.float64)
+    with np.errstate(invalid="ignore", over="ignore"):
+        D = ((X[:, None, :] - X[None, :, :]) ** 2).sum(axis=2)
+    np.fill_diagonal(D, 0.0)
+    return D
+
+
+def nnm_neighbours_d2(D: np.ndarray, f: int) -> np.ndarray:
+    """``nnm_neighbours`` from a table of squared distances ``D`` [P, P] (only its off-diagonal entries are read)."""
+    D = np.asarray(D, dtype=np.float64)
+    P = D.shape[0]
+    if not 0 <= f < P:
+        raise ValueError(f"nearest-neighbour mixing needs 0 <= f < P (got P = {P}, f = {f})")
+    A = np.zeros((P, P), dtype=np.int64)
+    for i in range(P):
+        others = np.array([j for j in range(P) if j != i], dtype=np.int64)
+        order = others[np.argsort(D[i, others], kind="stable")]      # ascending, NaN last, ties to the lower row
+        A[i, i] = 1
+        A[i, order[:P - f - 1]] = 1
+    return A
+
+
+def nnm_neighbours(slots: np.ndarray, f: int) -> np.ndarray:
+    """Nearest-neighbour mixing (NNM; Allouah, Farhadkhani, Guerraoui, Gupta, Pinot and Stephan, *Fixing by Mixing: A Recipe
+    for Optimal Byzantine ML under Heterogeneity*, AISTATS 2023), the neighbourhoods: with n_mix = P - f, N_i is row i itself
+    plus the n_mix - 1 rows nearest to it among the others, by squared distance in fp64 from the inputs, ascending, NaN last,
+    ties to the lower row index.  Row i is its own first neighbour even when another row duplicates it.  Returns the P x P 0/1
+    matrix A with A[i, j] = 1 iff j is in N_i."""
+    return nnm_neighbours_d2(_raw_d2(slots), f)
+
+
+def nnm_mix(slots: np.ndarray, f: int) -> np.ndarray:
+    """The mixed rows y_i = (1 / n_mix) sum over j in N_i of x_j (``nnm_neighbours``), in fp64."""
+    X = np.asarray(slots, dtype=np.float64)
+    return _mix_rows(X, nnm_neighbours(X, f), f)
+
+
+def _mix_rows(X: np.ndarray, A: np.ndarray, f: int) -> np.ndarray:
+    """Row i: the sum of the rows in N_i over n_mix (not ``A @ X``, where 0 * NaN would reach the rows that do not take it)."""
+    return np.stack([X[np.flatnonzero(a)].sum(axis=0) for a in A]) / (X.shape[0] - f)
+
+
+def nnm_pair_d2(D: np.ndarray, A: np.ndarray, f: int) -> np.ndarray:
+    """Squared distances between the mixed rows from the raw table ``D`` alone, with no pass over the data: with
+    c = (A[i] - A[k]) / n_mix (which sums to 0), ||y_i - y_k||^2 = -1/2 c^T D c, in fp64 and clamped at 0.  The sum runs over
+    the rows of N_i and N_k and D's diagonal counts as 0, so a NaN distance between any two of those rows makes the result NaN
+    (as it would be for the mixed rows themselves), and the clamp keeps a NaN a NaN."""
+    D = np.array(D, dtype=np.float64)
+    np.fill_diagonal(D, 0.0)
+    A = np.asarray(A, dtype=np.float64)
+    P, n = A.shape[0], A.shape[0] - f
+    out = np.zeros((P, P))
+    for i in range(P):
+        for k in range(P):
+            if i == k:
+                continue
+            u = np.flatnonzero(A[i] + A[k])
+            c = (A[i, u] - A[k, u]) / n
+            v = -0.5 * (c @ D[np.ix_(u, u)] @ c)
+            out[i, k] = v if not v < 0.0 else 0.0
+    return out
+
+
+def nnm(slots: np.ndarray, f: int, mode: str) -> np.ndarray:
+    """NNM, then the robust rule ``mode`` on the mixed rows (``nnm_mix``), per tensor.  The rules that use distances (Krum,
+    multi-Krum, Bulyan's selection, the geometric median's Weiszfeld in weight space) take them from ``nnm_pair_d2``:
+
+    * ``coordinate_median``; * ``trimmed_mean``: trim f;  * ``krum``: s = f;  * ``multi_krum``: s = f, averaging P - f rows;
+    * ``geometric_median``: ``geometric_median_weights`` over the mixed table, applied to the mixed rows;
+    * ``bulyan``: f, for P >= 4f + 3.
+
+    With f = 0 every mixed row is the mean of all rows, and so is the result."""
+    X = np.asarray(slots, dtype=np.float64)
+    P = X.shape[0]
+    D = _raw_d2(X)
+    A = nnm_neighbours_d2(D, f)
+    Y = _mix_rows(X, A, f)
+    if mode == "coordinate_median":
+        return coordinate_median(Y)
+    if mode == "trimmed_mean":
+        return trimmed_mean(Y, f)
+    Dm = nnm_pair_d2(D, A, f)
+    if mode == "krum":
+        return Y[int(np.argsort(_krum_scores_d2(Dm, f), kind="stable")[0])]
+    if mode == "multi_krum":
+        return Y[np.argsort(_krum_scores_d2(Dm, f), kind="stable")[:P - f]].mean(axis=0)
+    if mode == "geometric_median":
+        return _weiszfeld_weights(Dm, 1e-10, 256) @ Y
+    if mode == "bulyan":
+        if P < 4 * f + 3:
+            raise ValueError(f"Bulyan needs P >= 4f + 3 rows (got P = {P}, f = {f})")
+        return nearest_to_median_mean(Y[_bulyan_rounds(Dm, f)], f)
+    raise ValueError(f"NNM has no rule {mode!r}")
 
 
 def captured_group_bound(worker_fail: int, group_size: int) -> int:

@@ -10,9 +10,10 @@ import argparse
 from dataclasses import asdict, dataclass
 from typing import Optional
 
-APPROACHES = ("baseline", "maj_vote", "cyclic", "detox")
+APPROACHES = ("baseline", "maj_vote", "cyclic", "detox", "nnm")
 MODES = ("normal", "geometric_median", "krum", "maj_vote", "coordinate_median", "trimmed_mean", "multi_krum", "bulyan")
 DETOX_MODES = ("coordinate_median", "trimmed_mean", "multi_krum", "geometric_median", "bulyan")
+NNM_MODES = ("coordinate_median", "trimmed_mean", "krum", "multi_krum", "geometric_median", "bulyan")
 ROBUST_MAXP = 16                    # workers the fused coordinate-wise / Krum / Bulyan kernels take (TRIM_MAXP, KRUM_MAXP)
 ERR_MODES = ("rev_grad", "constant", "random", "omniscient", "alie", "minmax", "none")
 TRANSPORTS = ("nvl", "nccl", "nccl_flat", "gloo")
@@ -105,21 +106,15 @@ class JobConfig:
         if self.no_cuda:
             self.transport = "gloo"
         if self.approach == "baseline" and self.mode in ("coordinate_median", "trimmed_mean", "multi_krum", "bulyan"):
-            P, f = self.num_workers, self.worker_fail
-            if self.mode in ("coordinate_median", "trimmed_mean") and 2 * f >= P:
-                raise ValueError(f"--mode {self.mode} trims --worker-fail {f} values at each end of every coordinate: it needs "
-                                 f"num_workers > 2*worker_fail (got {P} workers)")
-            if self.mode == "multi_krum" and P <= 2 * f + 2:
-                raise ValueError(f"--mode multi_krum needs num_workers > 2*worker_fail + 2 (Krum's condition; got {P} workers, "
-                                 f"worker_fail {f})")
-            if self.mode == "bulyan" and P < 4 * f + 3:
-                raise ValueError(f"--mode bulyan needs num_workers >= 4*worker_fail + 3 (Bulyan's condition; got {P} workers, "
-                                 f"worker_fail {f})")
+            P = self.num_workers
+            self._check_rule_bounds(f"--mode {self.mode}")
             if self.transport == "nvl" and P > ROBUST_MAXP:
                 raise ValueError(f"--mode {self.mode} on the nvl transport handles at most {ROBUST_MAXP} workers (got {P}); "
                                  f"use --transport nccl for more")
         if self.approach == "detox":
             self._check_detox()
+        if self.approach == "nnm":
+            self._check_nnm()
         if self.compress and self.transport == "nvl" and self.err_mode == "omniscient":
             raise ValueError("--err-mode omniscient reads the honest slots in PS memory while they arrive; with --compress-grad "
                              "compress they only exist after the PS unpacked them -- pass --compress-grad None")
@@ -159,6 +154,37 @@ class JobConfig:
         """z of the ALIE attack: --attack-z, else z_max(num_workers, worker_fail)."""
         from .codes.adversary import alie_z_max
         return float(self.attack_z) if self.attack_z is not None else alie_z_max(self.num_workers, self.worker_fail)
+
+    def _check_rule_bounds(self, label: str) -> None:
+        """The P / f conditions of the robust rule ``--mode`` over the num_workers rows (``label`` names the flags in errors)."""
+        P, f = self.num_workers, self.worker_fail
+        if self.mode in ("coordinate_median", "trimmed_mean") and 2 * f >= P:
+            raise ValueError(f"{label} trims --worker-fail {f} values at each end of every coordinate: it needs "
+                             f"num_workers > 2*worker_fail (got {P} workers)")
+        if self.mode == "multi_krum" and P <= 2 * f + 2:
+            raise ValueError(f"{label} needs num_workers > 2*worker_fail + 2 (Krum's condition; got {P} workers, "
+                             f"worker_fail {f})")
+        if self.mode == "bulyan" and P < 4 * f + 3:
+            raise ValueError(f"{label} needs num_workers >= 4*worker_fail + 3 (Bulyan's condition; got {P} workers, "
+                             f"worker_fail {f})")
+
+    def _check_nnm(self) -> None:
+        """NNM mixes every worker's row with its num_workers - worker_fail - 1 nearest rows, then runs ``--mode`` on the mixed
+        rows with the same P / f conditions as the baseline rule."""
+        if self.mode not in NNM_MODES:
+            raise ValueError(f"--approach nnm takes --mode {' | '.join(NNM_MODES)} (the rule applied to the mixed rows), got "
+                             f"--mode {self.mode}")
+        P, f = self.num_workers, self.worker_fail
+        if not 0 <= f < P:
+            raise ValueError(f"--approach nnm mixes num_workers - worker_fail rows: it needs 0 <= worker_fail < num_workers "
+                             f"(got worker_fail {f}, {P} workers)")
+        self._check_rule_bounds(f"--approach nnm --mode {self.mode}")
+        if self.transport == "nvl" and P > ROBUST_MAXP:
+            raise ValueError(f"--approach nnm on the nvl transport handles at most {ROBUST_MAXP} workers (got {P}); use "
+                             f"--transport nccl for more")
+        if self.transport == "nccl_flat":
+            raise ValueError("--transport nccl_flat runs the plain mean and the vote only; use --transport nccl for "
+                             "--approach nnm")
 
     def _check_detox(self) -> None:
         """DETOX runs the robust rule across the G group winners, tolerating b_G captured groups in place of f liars."""
@@ -242,7 +268,8 @@ def add_fit_args(parser: argparse.ArgumentParser) -> argparse.ArgumentParser:
            "worker_fail // ceil(group_size / 2)); multi_krum averages the num_workers - worker_fail workers (detox: G - b_G group "
            "winners) with the lowest Krum scores; bulyan picks num_workers - 2 worker_fail workers by repeated Krum, then "
            "averages, per coordinate, the num_workers - 4 worker_fail picked values nearest their median (needs num_workers >= "
-           "4 worker_fail + 3; detox: G and b_G)")
+           "4 worker_fail + 3; detox: G and b_G); coordinate_median | trimmed_mean | krum | multi_krum | geometric_median | "
+           "bulyan (nnm: the rule applied to the mixed rows, with --worker-fail as f)")
     a("--dataset", type=str, default=d.dataset)
     a("--comm-type", type=str, default=d.comm_type)
     a("--err-mode", type=str, default=d.err_mode,
@@ -252,7 +279,8 @@ def add_fit_args(parser: argparse.ArgumentParser) -> argparse.ArgumentParser:
       help="--err-mode alie: the liars send mu - z * sigma (default: z_max = Phi^-1((P - s) / P), s = floor(P/2 + 1) - f)")
     a("--approach", type=str, default=d.approach,
       help="baseline | maj_vote | cyclic | detox (majority vote inside each repetition group, then --mode across the G group "
-           "winners)")
+           "winners) | nnm (nearest-neighbour mixing: every worker's row is replaced, per tensor, by the mean of its "
+           "num_workers - worker_fail nearest rows, itself included, then --mode runs on the mixed rows)")
     a("--num-aggregate", type=int, default=d.num_aggregate)
     a("--eval-freq", type=int, default=d.eval_freq)
     a("--train-dir", type=str, default=d.train_dir)

@@ -131,7 +131,7 @@ def augment_cifar(x_u8: torch.Tensor, seed: int) -> torch.Tensor:
 class BatchPlan:
     """Maps (step, worker rank) to dataset indices for one approach."""
 
-    approach: str                 # baseline | maj_vote | cyclic | detox
+    approach: str                 # baseline | maj_vote | cyclic | detox | nnm
     dataset_size: int
     batch_size: int
     num_workers: int
@@ -162,7 +162,7 @@ class BatchPlan:
         spe = self.steps_per_epoch()
         epoch, pos = divmod(max(step - 1, 0), spe)
         B = self.batch_size
-        if self.approach == "baseline":
+        if self.approach in ("baseline", "nnm"):                  # every worker draws its own batch
             return [self._slice(self._perm(self.seed * 1000003 + rank * 7919 + epoch), pos, B)]
         if self.approach in ("maj_vote", "detox"):
             gseed = self.group_seeds[self.group_of[rank]]

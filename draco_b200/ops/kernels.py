@@ -197,7 +197,8 @@ def aggregate_update(layout: ArenaLayout, grad_in: Addr, slot_stride: int, *, pa
                      recomb: Addr = None, first_step: int = 1, grad_out: Addr = None, mc_params: Addr = None,
                      dst: Sequence[Addr] = (), flags: Sequence[Addr] = (), grid: Optional[int] = None,
                      tile_range: Optional[tuple] = None, weights: Addr = None, exp_avg_sq: Addr = None,
-                     max_exp_avg_sq: Addr = None, trim: Optional[int] = None, near_median: Optional[int] = None) -> None:
+                     max_exp_avg_sq: Addr = None, trim: Optional[int] = None, near_median: Optional[int] = None,
+                     mix: Optional[torch.Tensor] = None, mix_f: Optional[int] = None) -> None:
     """Fused aggregate (select-sum, cyclic recombination, real per-tensor ``weights`` [T, K], -- with ``trim`` -- the
     coordinate-wise trimmed mean of K <= 16 rows that drops ``trim`` values at each end, or -- with ``near_median = f`` --
     Bulyan's coordinate stage: the mean of the K - 2f values nearest the coordinate median of the K <= 16 rows ``select``
@@ -207,7 +208,12 @@ def aggregate_update(layout: ArenaLayout, grad_in: Addr, slot_stride: int, *, pa
 
     ``select``: int32 [K, T] table of the worker slot that row k of tensor t is read from (rows 0..K-1 when None).  It applies to
     the select-sum, to the ``weights`` sum and to the trimmed mean; DETOX passes the vote's ``winner_slot`` so that the rule runs
-    on the group winners."""
+    on the group winners.
+
+    ``mix`` (with ``trim`` or ``near_median``): the int32 [P, T] neighbour masks of ``nnm_mix`` and ``mix_f`` = f.  The trimmed
+    mean / median then runs on the K = P mixed rows (no ``select``), Bulyan's coordinate stage on the K = theta mixed rows that
+    ``select`` names (mixed-row indices from ``bulyan_select``); mixed row i is the fp32 mean of the raw slots in N_i, formed in
+    the kernel (csrc/cuda/aggregate_update.cu, mixed_robust_f4)."""
     a = N.UpdateArgs()
     a.mode = 1 if recomb is not None else (2 if weights is not None else 0)
     if weights is not None:
@@ -235,6 +241,18 @@ def aggregate_update(layout: ArenaLayout, grad_in: Addr, slot_stride: int, *, pa
         if abs(scale * (K - 2 * f) - 1.0) > 1e-6:
             raise ValueError(f"nearest-to-median mean: scale must be 1 / (K - 2 * f) = {1.0 / (K - 2 * f)}, got {scale}")
         a.mode, a.trim = 4, int(f)
+    if mix is not None:
+        if trim is None and near_median is None:
+            raise ValueError("mixing: only the trimmed mean / median (trim=) and Bulyan's stage (near_median=) take mix=")
+        P = mix.shape[0] if mix.dim() == 2 else 0
+        _check_row_table(layout, mix, P)
+        if mix_f is None or not 0 <= mix_f < P:
+            raise ValueError(f"mixing: needs 0 <= mix_f < P = {P} (got {mix_f})")
+        if trim is not None and (K != P or select is not None):
+            raise ValueError(f"mixing: the trimmed mean runs on all P = {P} mixed rows (K = {K}) and takes no select table")
+        if near_median is not None and K > P:
+            raise ValueError(f"mixing: Bulyan's stage takes at most P = {P} mixed rows (K = {K})")
+        a.mix, a.mixP, a.mix_scale = mix.data_ptr(), P, 1.0 / (P - mix_f)
     a.grad_in = addr(grad_in)
     a.slot_stride = slot_stride
     a.select = addr(select)
@@ -373,17 +391,20 @@ GEOMED_FAST_MAXP = 16
 
 def geometric_median_weights(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, pair_d2: torch.Tensor,
                              weights: torch.Tensor, max_iter: int = 256, eps: float = 1e-10,
-                             iters_out: Optional[torch.Tensor] = None, rows: Optional[torch.Tensor] = None) -> torch.Tensor:
+                             iters_out: Optional[torch.Tensor] = None, rows: Optional[torch.Tensor] = None,
+                             filled: bool = False) -> torch.Tensor:
     """Per-tensor geometric median as convex weights: ``median_t = sum_i weights[t, i] * slot_i`` (Weiszfeld run in weight
     space from the pairwise distances -- one pass over the slab; see csrc/cuda/robust.cu).  ``pair_d2``: zeroed fp64
     [T, P(P-1)/2] scratch (left zeroed); ``weights``: fp32 [T, P] out.  ``rows``: optional int32 [P, T] table, row i of tensor t
-    is worker slot ``rows[i, t]`` (the weights stay in row space: pass the same table to ``aggregate_update(select=)``)."""
+    is worker slot ``rows[i, t]`` (the weights stay in row space: pass the same table to ``aggregate_update(select=)``).
+    ``filled``: ``pair_d2`` already holds the distances (``nnm_mix(mixed_out=True)``), so no pair-distance pass is launched."""
     assert P <= GEOMED_FAST_MAXP
     if rows is not None:
         _check_row_table(layout, rows, P)
     lib = N.cuda()
-    pa = N.PairDistArgs(addr(grad_in), slot_stride, P, layout.tile_view(weights.device), pair_d2.data_ptr(), addr(rows))
-    N.check(lib.drc_pair_dist(C.byref(pa), stream_grid(layout, 4), _stream()), "pair_dist")
+    if not filled:
+        pa = N.PairDistArgs(addr(grad_in), slot_stride, P, layout.tile_view(weights.device), pair_d2.data_ptr(), addr(rows))
+        N.check(lib.drc_pair_dist(C.byref(pa), stream_grid(layout, 4), _stream()), "pair_dist")
     wa = N.GeoMedWeightsArgs(pair_d2.data_ptr(), layout.ntensors, P, max_iter, eps, weights.data_ptr(),
                              iters_out.data_ptr() if iters_out is not None else None)
     N.check(lib.drc_geomed_weights(C.byref(wa), _stream()), "geomed_weights")
@@ -391,36 +412,79 @@ def geometric_median_weights(layout: ArenaLayout, grad_in: Addr, slot_stride: in
 
 
 def krum_select(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, s: int, pair_d2: torch.Tensor,
-                select: torch.Tensor, m: int = 1, rows: Optional[torch.Tensor] = None) -> None:
+                select: torch.Tensor, m: int = 1, rows: Optional[torch.Tensor] = None, filled: bool = False) -> None:
     """``pair_d2``: zeroed fp64 [T, P*(P-1)/2] scratch (left zeroed); ``select``: int32 [m, T] out, the ``m`` lowest Krum scores
     per tensor ordered by (score, slot) -- ``m = 1``: the Krum winner, ``m = P - s``: multi-Krum (int32 [T] is fine for m = 1).
-    ``rows``: optional int32 [P, T] table, row i of tensor t is worker slot ``rows[i, t]``; ``select`` then holds worker slots."""
+    ``rows``: optional int32 [P, T] table, row i of tensor t is worker slot ``rows[i, t]``; ``select`` then holds worker slots.
+    ``filled``: ``pair_d2`` already holds the distances (``nnm_mix(mixed_out=True)``), so no pair-distance pass is launched."""
     assert 1 <= m <= P and select.numel() >= m * layout.ntensors
     if rows is not None:
         _check_row_table(layout, rows, P)
     lib = N.cuda()
-    pa = N.PairDistArgs(addr(grad_in), slot_stride, P, layout.tile_view(select.device), pair_d2.data_ptr(), addr(rows))
-    N.check(lib.drc_pair_dist(C.byref(pa), stream_grid(layout, 4), _stream()), "pair_dist")
+    if not filled:
+        pa = N.PairDistArgs(addr(grad_in), slot_stride, P, layout.tile_view(select.device), pair_d2.data_ptr(), addr(rows))
+        N.check(lib.drc_pair_dist(C.byref(pa), stream_grid(layout, 4), _stream()), "pair_dist")
     ka = N.KrumSelectArgs(pair_d2.data_ptr(), layout.ntensors, P, s, m, select.data_ptr(), addr(rows))
     N.check(lib.drc_krum_select(C.byref(ka), _stream()), "krum_select")
 
 
 def bulyan_select(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, f: int, pair_d2: torch.Tensor,
-                  select: torch.Tensor, rows: Optional[torch.Tensor] = None) -> None:
+                  select: torch.Tensor, rows: Optional[torch.Tensor] = None, filled: bool = False) -> None:
     """Bulyan's selection stage per tensor (``oracle.bulyan_indices``): theta = P - 2f rounds of Krum over the rows not chosen
     yet, for P >= 4f + 3 rows.  ``pair_d2``: zeroed fp64 [T, P*(P-1)/2] scratch (left zeroed); ``select``: int32 [theta, T] out,
     the worker slot chosen in round k at ``select[k, t]`` -- pass it to ``aggregate_update(K=theta, near_median=f, select=)``.
-    ``rows``: optional int32 [P, T] table, row i of tensor t is worker slot ``rows[i, t]`` (DETOX: the vote's winner_slot)."""
+    ``rows``: optional int32 [P, T] table, row i of tensor t is worker slot ``rows[i, t]`` (DETOX: the vote's winner_slot).
+    ``filled``: ``pair_d2`` already holds the distances (``nnm_mix(mixed_out=True)``), so no pair-distance pass is launched."""
     if not (f >= 0 and 4 * f + 3 <= P <= ROW_TABLE_MAXROWS):
         raise ValueError(f"bulyan_select: needs 4 * f + 3 <= P <= {ROW_TABLE_MAXROWS} (got P = {P}, f = {f})")
     _check_row_table(layout, select, P - 2 * f)
     if rows is not None:
         _check_row_table(layout, rows, P)
     lib = N.cuda()
-    pa = N.PairDistArgs(addr(grad_in), slot_stride, P, layout.tile_view(select.device), pair_d2.data_ptr(), addr(rows))
-    N.check(lib.drc_pair_dist(C.byref(pa), stream_grid(layout, 4), _stream()), "pair_dist")
+    if not filled:
+        pa = N.PairDistArgs(addr(grad_in), slot_stride, P, layout.tile_view(select.device), pair_d2.data_ptr(), addr(rows))
+        N.check(lib.drc_pair_dist(C.byref(pa), stream_grid(layout, 4), _stream()), "pair_dist")
     ba = N.BulyanSelectArgs(pair_d2.data_ptr(), layout.ntensors, P, f, select.data_ptr(), addr(rows))
     N.check(lib.drc_bulyan_select(C.byref(ba), _stream()), "bulyan_select")
+
+
+def nnm_mix(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, f: int, pair_d2: torch.Tensor, mix: torch.Tensor,
+            mixed_out: bool) -> None:
+    """Nearest-neighbour mixing per tensor (``oracle.nnm_neighbours`` / ``oracle.nnm_pair_d2``): the pair-distance pass over the
+    P raw slots, then ``nnm_mix_kernel`` (csrc/cuda/robust.cu).  ``mix``: int32 [P, T] out, bit j of ``mix[i, t]`` = slot j is
+    one of the n_mix = P - f rows row i is mixed from.  ``pair_d2``: zeroed fp64 [T, P*(P-1)/2] scratch.  ``mixed_out``: leave
+    the mixed rows' distances in it for ``krum_select`` / ``bulyan_select`` / ``geometric_median_weights`` with ``filled=True``
+    (which zero it); otherwise it is left zeroed."""
+    if not (0 <= f < P <= ROW_TABLE_MAXROWS):
+        raise ValueError(f"nnm_mix: needs 0 <= f < P <= {ROW_TABLE_MAXROWS} (got P = {P}, f = {f})")
+    _check_row_table(layout, mix, P)
+    lib = N.cuda()
+    pa = N.PairDistArgs(addr(grad_in), slot_stride, P, layout.tile_view(mix.device), pair_d2.data_ptr(), None)
+    N.check(lib.drc_pair_dist(C.byref(pa), stream_grid(layout, 4), _stream()), "pair_dist")
+    na = N.NnmMixArgs(pair_d2.data_ptr(), layout.ntensors, P, f, mix.data_ptr(), int(bool(mixed_out)))
+    N.check(lib.drc_nnm_mix(C.byref(na), _stream()), "nnm_mix")
+
+
+def nnm_fold(layout: ArenaLayout, P: int, f: int, mix: torch.Tensor, w_raw: torch.Tensor, *, select: Optional[torch.Tensor] = None,
+             m: int = 1, w_mix: Optional[torch.Tensor] = None) -> None:
+    """A choice over the mixed rows as fp32 weights over the raw slots: ``w_raw[t] = A_t^T w_mix[t] / (P - f)`` (fp64 sums),
+    with w_mix = 1/m on the m mixed rows ``select[:m, t]`` names (Krum, multi-Krum) or the fp32 [T, P] ``w_mix`` (geometric
+    median).  Pass ``w_raw`` to ``aggregate_update(K=P, scale=1, weights=w_raw)``."""
+    T = layout.ntensors
+    if not (0 <= f < P <= ROW_TABLE_MAXROWS):
+        raise ValueError(f"nnm_fold: needs 0 <= f < P <= {ROW_TABLE_MAXROWS} (got P = {P}, f = {f})")
+    _check_row_table(layout, mix, P)
+    if (select is None) == (w_mix is None):
+        raise ValueError("nnm_fold: pass exactly one of select= and w_mix=")
+    if select is not None:
+        if not 1 <= m <= P:
+            raise ValueError(f"nnm_fold: needs 1 <= m <= P = {P} (got m = {m})")
+        _check_row_table(layout, select, m)
+    for name, w in (("w_mix", w_mix), ("w_raw", w_raw)):
+        if w is not None and (w.dtype != torch.float32 or not w.is_cuda or not w.is_contiguous() or tuple(w.shape) != (T, P)):
+            raise ValueError(f"nnm_fold: {name} must be a contiguous fp32 CUDA tensor of shape ({T}, {P})")
+    fa = N.NnmFoldArgs(mix.data_ptr(), T, P, f, addr(select), m, addr(w_mix), w_raw.data_ptr())
+    N.check(N.cuda().drc_nnm_fold(C.byref(fa), _stream()), "nnm_fold")
 
 
 # ------------------------------------------------------------------------------------------------ GEMM (K10)

@@ -30,24 +30,29 @@ def select_rule(cfg: JobConfig) -> str:
     (rep_master.py:118-129); baseline approach -> mean / geometric median / Krum by ``--mode`` (baseline_master.py:118-129), plus
     three rules beyond the reference: coordinate-wise median, coordinate-wise trimmed mean and multi-Krum.  The detox approach
     (beyond the reference too) votes inside every group and runs ``--mode`` across the group winners: ``detox_*`` rules.  Bulyan
-    (``--mode bulyan``) is beyond the reference as well."""
+    (``--mode bulyan``) is beyond the reference as well, and so is the nnm approach: nearest-neighbour mixing of the worker rows,
+    then ``--mode`` on the mixed rows (``nnm_*`` rules)."""
     if cfg.approach == "cyclic":
         return "cyclic"
     if cfg.approach == "maj_vote":
         return "vote" if cfg.mode == "maj_vote" else "mean"
     if cfg.approach == "detox":
         return DETOX_RULES[cfg.mode]
+    if cfg.approach == "nnm":
+        return NNM_RULES[cfg.mode]
     return {"normal": "mean", "geometric_median": "geomedian", "krum": "krum", "coordinate_median": "median",
             "trimmed_mean": "trimmed_mean", "multi_krum": "multi_krum", "bulyan": "bulyan"}.get(cfg.mode, "mean")
 
 
 DETOX_RULES = {"coordinate_median": "detox_median", "trimmed_mean": "detox_trimmed_mean", "multi_krum": "detox_multi_krum",
                "geometric_median": "detox_geomedian", "bulyan": "detox_bulyan"}
+NNM_RULES = {"coordinate_median": "nnm_median", "trimmed_mean": "nnm_trimmed_mean", "krum": "nnm_krum",
+             "multi_krum": "nnm_multi_krum", "geometric_median": "nnm_geomedian", "bulyan": "nnm_bulyan"}
 
 
 def coordinate_trim(cfg: JobConfig) -> int:
     """Values dropped at each end of every coordinate: (P - 1) // 2 for the median, ``--worker-fail`` for the trimmed mean."""
-    return (cfg.num_workers - 1) // 2 if select_rule(cfg) == "median" else cfg.worker_fail
+    return (cfg.num_workers - 1) // 2 if select_rule(cfg) in ("median", "nnm_median") else cfg.worker_fail
 
 
 # rules the fused PS applies bucket by bucket while the workers still push (nothing in them needs the whole tensor at once)
@@ -127,6 +132,22 @@ class FusedPS:
             self.theta = rows - 2 * self.f                 # rows selected per tensor; their worker slots go in `select`
             self.pair_d2 = torch.zeros(T, rows * (rows - 1) // 2, dtype=torch.float64, device=device)
             self.select = torch.zeros(self.theta, T, dtype=torch.int32, device=device)
+        elif self.rule.startswith("nnm_"):                # mixing masks; the rule then runs on the mixed rows
+            P, self.f = self.P, cfg.worker_fail
+            self.mix = torch.zeros(P, T, dtype=torch.int32, device=device)
+            self.pair_d2 = torch.zeros(T, P * (P - 1) // 2, dtype=torch.float64, device=device)
+            if self.rule in ("nnm_median", "nnm_trimmed_mean"):
+                self.trim = coordinate_trim(cfg)
+            elif self.rule == "nnm_bulyan":               # select holds the mixed rows Bulyan keeps
+                self.theta = P - 2 * self.f
+                self.select = torch.zeros(self.theta, T, dtype=torch.int32, device=device)
+            else:                                         # a choice over the mixed rows, folded into raw-slot weights
+                if self.rule == "nnm_geomedian":
+                    self.gm_weights = torch.zeros(T, P, dtype=torch.float32, device=device)
+                else:
+                    self.m = 1 if self.rule == "nnm_krum" else P - self.f
+                    self.select = torch.zeros(self.m, T, dtype=torch.int32, device=device)
+                self.w_raw = torch.zeros(T, P, dtype=torch.float32, device=device)
         elif self.rule == "krum":
             self.pair_d2 = torch.zeros(T, self.P * (self.P - 1) // 2, dtype=torch.float64, device=device)
             self.select = torch.zeros(T, dtype=torch.int32, device=device)
@@ -237,6 +258,25 @@ class FusedPS:
             else:
                 _update(L, self.grad_in, self.slot_stride, K=G, scale=1.0 / (G - 2 * self.trim), trim=self.trim, select=win,
                         **common); n += 1
+        elif self.rule.startswith("nnm_"):
+            P, f = self.P, self.f
+            coordinate = self.rule in ("nnm_median", "nnm_trimmed_mean")
+            K.nnm_mix(L, self.grad_in, self.slot_stride, P, f, self.pair_d2, self.mix, mixed_out=not coordinate); n += 2
+            if coordinate:
+                _update(L, self.grad_in, self.slot_stride, K=P, scale=1.0 / (P - 2 * self.trim), trim=self.trim, mix=self.mix,
+                        mix_f=f, **common); n += 1
+            elif self.rule == "nnm_bulyan":
+                K.bulyan_select(L, self.grad_in, self.slot_stride, P, f, self.pair_d2, self.select, filled=True); n += 1
+                _update(L, self.grad_in, self.slot_stride, K=self.theta, scale=1.0 / (self.theta - 2 * f), near_median=f,
+                        select=self.select, mix=self.mix, mix_f=f, **common); n += 1
+            else:
+                if self.rule == "nnm_geomedian":
+                    K.geometric_median_weights(L, self.grad_in, self.slot_stride, P, self.pair_d2, self.gm_weights, filled=True)
+                    K.nnm_fold(L, P, f, self.mix, self.w_raw, w_mix=self.gm_weights); n += 2
+                else:
+                    K.krum_select(L, self.grad_in, self.slot_stride, P, f, self.pair_d2, self.select, m=self.m, filled=True)
+                    K.nnm_fold(L, P, f, self.mix, self.w_raw, select=self.select, m=self.m); n += 2
+                _update(L, self.grad_in, self.slot_stride, K=P, scale=1.0, weights=self.w_raw, **common); n += 1
         elif self.rule == "krum":
             K.krum_select(L, self.grad_in, self.slot_stride, self.P, self.cfg.worker_fail, self.pair_d2, self.select); n += 2
             _update(L, self.grad_in, self.slot_stride, K=1, scale=1.0, select=self.select, **common); n += 1
@@ -289,7 +329,7 @@ class TorchPS:
             g = torch.Generator().manual_seed(cfg.seed + 4242)
             f = (torch.randn(layout.total, generator=g) + 1.0) * torch.from_numpy(layout.valid_mask()).float()
             self.f = f.to(device)
-        self.trim = coordinate_trim(cfg) if self.rule in ("median", "trimmed_mean") else 0
+        self.trim = coordinate_trim(cfg) if self.rule in ("median", "trimmed_mean", "nnm_median", "nnm_trimmed_mean") else 0
         if self.rule in ("detox_median", "detox_trimmed_mean"):
             self.trim = detox_trim(cfg)
         self.last_info: Dict[str, object] = {}
@@ -427,6 +467,23 @@ class TorchPS:
             acc += S.gather(0, (s + k)[None]).squeeze(0)
         return acc * (1.0 / beta)
 
+    def _nnm_mix_tensor(self, X: torch.Tensor, f: int) -> torch.Tensor:
+        """Nearest-neighbour mixing (``oracle.nnm_mix``): row i becomes the mean of itself and its P - f - 1 nearest rows
+        (squared distances in fp64, NaN last, ties to the lower row), formed in fp32 as the fused kernel does: from +0, add the
+        neighbours in ascending row order, then multiply once by fp32(1 / (P - f))."""
+        P = X.shape[0]
+        d2 = torch.cdist(X.double(), X.double()).pow(2)
+        d2.fill_diagonal_(-1.0)                            # row i is its own first neighbour
+        nbrs = d2.argsort(dim=1, stable=True)[:, :P - f].sort(dim=1).values.tolist()
+        scale = torch.tensor(1.0 / (P - f), dtype=torch.float32, device=X.device)
+        Y = torch.empty_like(X)
+        for i in range(P):
+            y = torch.zeros_like(X[0])
+            for j in nbrs[i]:
+                y = y + X[j]
+            Y[i] = y * scale
+        return Y
+
     def _cyclic_tensor(self, R: torch.Tensor, f: torch.Tensor) -> torch.Tensor:
         """R: [n, d] complex64 -> Re(v^T R) / n with v from the C++ locator (N1 replacement)."""
         n, s = self.P, self.cfg.worker_fail
@@ -464,6 +521,19 @@ class TorchPS:
                 g = self._geomedian_tensor(X)
             elif self.rule == "bulyan":
                 g = self._bulyan_tensor(X, self.cfg.worker_fail)
+            elif self.rule.startswith("nnm_"):            # the rule's own helper on the mixed rows
+                f = self.cfg.worker_fail
+                Y = self._nnm_mix_tensor(X, f)
+                if self.rule == "nnm_krum":
+                    g = Y[self._krum_tensor(Y)]
+                elif self.rule == "nnm_multi_krum":
+                    g = self._multi_krum_tensor(Y, f, self.P - f)
+                elif self.rule == "nnm_geomedian":
+                    g = self._geomedian_tensor(Y)
+                elif self.rule == "nnm_bulyan":
+                    g = self._bulyan_tensor(Y, f)
+                else:
+                    g = self._trimmed_mean_tensor(Y)
             elif self.rule.startswith("detox"):
                 winners = []                               # stage 1: the vote inside every group
                 for grp in self.groups.groups:
@@ -493,7 +563,8 @@ class TorchPS:
         mode = {"mean": "normal", "vote": "maj_vote", "krum": "krum", "geomedian": "geometric_median", "cyclic": "cyclic",
                 "median": "coordinate_median", "trimmed_mean": "trimmed_mean", "multi_krum": "multi_krum",
                 "detox_median": "coordinate_median", "detox_trimmed_mean": "trimmed_mean", "detox_multi_krum": "multi_krum",
-                "detox_geomedian": "geometric_median", "bulyan": "bulyan", "detox_bulyan": "bulyan"}[self.rule]
+                "detox_geomedian": "geometric_median", "bulyan": "bulyan", "detox_bulyan": "bulyan",
+                **{rule: mode for mode, rule in NNM_RULES.items()}}[self.rule]
         self.optimizer.step(grads=grads, mode=mode)
 
 

@@ -19,8 +19,14 @@ each launch on its own and as the chain the PS runs after the last bucket: the p
 (the beta = theta - 2f values nearest the coordinate median of theta rows) against mode 0 over the P - f multi-Krum rows and
 mode 3 over the same theta rows (the f-trimmed mean: the same sort, without the median and the window walk).
 
+With --nnm-workers it times nearest-neighbour mixing (NNM) on the same arena, f = (P - 3) // 4 (P = 7: f = 1, P = 15: f = 3):
+``nnm_mix`` (neighbour masks plus the mixed rows' distance table, csrc/cuda/robust.cu) and ``nnm_fold`` (a multi-Krum choice over
+the mixed rows as raw-slot weights) alone; the update kernel's mode 3 (coordinate-wise median) and mode 4 (Bulyan's coordinate
+stage) with mixing against the same modes without it, over the same rows; and the whole chains the PS runs after the last
+bucket -- NNM + multi-Krum and NNM + Bulyan against plain multi-Krum and plain Bulyan.
+
     python tools/bench_aggregate.py [--workers 7 16] [--groups 3 5 8] [--attack-workers 7 15] [--bulyan-workers 7 15]
-                                    [--iters 200] [--rounds 3] [--out FILE]
+                                    [--nnm-workers 7 15] [--iters 200] [--rounds 3] [--out FILE]
 """
 from __future__ import annotations
 
@@ -134,6 +140,74 @@ def bulyan_arm(K, L, P, iters, rounds, dev, update) -> list:
              "us_rounds": [round(t, 2) for t in ts]} for name, ts in times.items()]
 
 
+def nnm_arm(K, L, P, iters, rounds, dev, update) -> list:
+    """NNM's launches alone and chained, against the unmixed rules (see the module docstring)."""
+    import ctypes as C
+
+    import torch
+    from draco_b200 import _native as N
+    f = (P - 3) // 4
+    theta, m, T, D = P - 2 * f, P - f, L.ntensors, L.total
+    med = (P - 1) // 2
+    slab = torch.randn(P, D, device=dev) * 1e-3
+    pair = torch.zeros(T, P * (P - 1) // 2, dtype=torch.float64, device=dev)
+    mix = torch.zeros(P, T, dtype=torch.int32, device=dev)
+    sel_b = torch.zeros(theta, T, dtype=torch.int32, device=dev)
+    sel_k = torch.zeros(m, T, dtype=torch.int32, device=dev)
+    w_raw = torch.zeros(T, P, device=dev)
+    K.nnm_mix(L, slab, D, P, f, pair, mix, mixed_out=True)
+    K.bulyan_select(L, slab, D, P, f, pair, sel_b, filled=True)
+    lib = N.cuda()
+    na = N.NnmMixArgs(pair.data_ptr(), T, P, f, mix.data_ptr(), 0)     # alone: zeroes the (already zero) table after the masks
+    na_out = N.NnmMixArgs(pair.data_ptr(), T, P, f, mix.data_ptr(), 1)
+    fa = N.NnmFoldArgs(mix.data_ptr(), T, P, f, sel_k.data_ptr(), m, None, w_raw.data_ptr())
+
+    def mix_then_zero():                                                # the mixed table, then zeroed as a select kernel would
+        lib.drc_nnm_mix(C.byref(na_out), K._stream())
+        pair.zero_()
+    arms = {
+        "nnm_mix_masks": lambda: lib.drc_nnm_mix(C.byref(na), K._stream()),
+        "nnm_mix_table_plus_zero": mix_then_zero,
+        "table_zero_alone": pair.zero_,
+        "nnm_fold_select": lambda: lib.drc_nnm_fold(C.byref(fa), K._stream()),
+        "mode3_median_mixed": lambda: update(slab, dict(K=P, scale=1.0 / (P - 2 * med), trim=med, mix=mix, mix_f=f)),
+        "mode3_median": lambda: update(slab, dict(K=P, scale=1.0 / (P - 2 * med), trim=med)),
+        "mode4_near_median_mixed": lambda: update(slab, dict(K=theta, scale=1.0 / (theta - 2 * f), near_median=f, select=sel_b,
+                                                             mix=mix, mix_f=f)),
+        "mode4_near_median": lambda: update(slab, dict(K=theta, scale=1.0 / (theta - 2 * f), near_median=f, select=sel_b)),
+        "nnm_multi_krum_chain": lambda: (K.nnm_mix(L, slab, D, P, f, pair, mix, mixed_out=True),
+                                         K.krum_select(L, slab, D, P, f, pair, sel_k, m=m, filled=True),
+                                         K.nnm_fold(L, P, f, mix, w_raw, select=sel_k, m=m),
+                                         update(slab, dict(K=P, scale=1.0, weights=w_raw))),
+        "multi_krum_chain": lambda: (K.krum_select(L, slab, D, P, f, pair, sel_k, m=m),
+                                     update(slab, dict(K=m, scale=1.0 / m, select=sel_k))),
+        "nnm_median_chain": lambda: (K.nnm_mix(L, slab, D, P, f, pair, mix, mixed_out=False),
+                                     update(slab, dict(K=P, scale=1.0 / (P - 2 * med), trim=med, mix=mix, mix_f=f))),
+        "nnm_bulyan_chain": lambda: (K.nnm_mix(L, slab, D, P, f, pair, mix, mixed_out=True),
+                                     K.bulyan_select(L, slab, D, P, f, pair, sel_b, filled=True),
+                                     update(slab, dict(K=theta, scale=1.0 / (theta - 2 * f), near_median=f, select=sel_b, mix=mix,
+                                                       mix_f=f))),
+        "bulyan_chain": lambda: (K.bulyan_select(L, slab, D, P, f, pair, sel_b),
+                                 update(slab, dict(K=theta, scale=1.0 / (theta - 2 * f), near_median=f, select=sel_b))),
+    }
+    for fn in arms.values():
+        for _ in range(20):
+            fn()
+    torch.cuda.synchronize()
+    times = {name: [] for name in arms}
+    for _ in range(rounds):
+        for name, fn in arms.items():
+            s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            s.record()
+            for _ in range(iters):
+                fn()
+            e.record()
+            e.synchronize()
+            times[name].append(s.elapsed_time(e) * 1e3 / iters)
+    return [{"P": P, "f": f, "theta": theta, "arm": name, "us_per_call": round(sorted(ts)[len(ts) // 2], 2),
+             "us_rounds": [round(t, 2) for t in ts]} for name, ts in times.items()]
+
+
 def main() -> int:
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--workers", type=int, nargs="*", default=[7, 16])
@@ -143,6 +217,7 @@ def main() -> int:
     ap.add_argument("--attack-workers", type=int, nargs="*", default=[], help="P of the ALIE / min-max kernel arm (none: skipped)")
     ap.add_argument("--attack-fail", type=int, default=3, help="liar slots of the attack arm")
     ap.add_argument("--bulyan-workers", type=int, nargs="*", default=[], help="P of the Bulyan / multi-Krum arm (none: skipped)")
+    ap.add_argument("--nnm-workers", type=int, nargs="*", default=[], help="P of the NNM arm (none: skipped)")
     ap.add_argument("--iters", type=int, default=200)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--out", type=str, default=None, help="also append the JSON lines to this file")
@@ -217,6 +292,8 @@ def main() -> int:
         K.aggregate_update(L, slab, D, params=params, momentum=mom, hp=hp, step_ptr=step, done_counter=cnt[0:1], **kw)
     for P in a.bulyan_workers:
         lines += bulyan_arm(K, L, P, a.iters, a.rounds, dev, update)
+    for P in a.nnm_workers:
+        lines += nnm_arm(K, L, P, a.iters, a.rounds, dev, update)
     for ln in lines:
         print(json.dumps(ln), flush=True)
     if a.out:
