@@ -32,6 +32,12 @@ struct PushArgs {
   // Zero-copy mode: instead of arenas, a device table [R][ntensors] of pointers to each parameter's gradient tensor
   // exactly where autograd left it (bf16 or fp32 per TensorMeta.is_bf16).  No gather / accumulate pass exists at all.
   const void* const* src_table;
+  // Worker-side momentum (push_encode_wmom_kernel only): this worker's fp32 state arena, in the slot's element layout.  Each
+  // pushed element becomes m' = rn(rn(wm_beta * m) + rn(wm_scale * g)) (wm_beta = fp32(beta), wm_scale = fp32(1 - beta)),
+  // m' is stored back, and the adversary hook acts on a copy of m': a liar's state always follows its true gradient.
+  float* wmom;
+  float wm_beta;
+  float wm_scale;
 };
 
 // counter-based normal generator (Philox-lite: 2 rounds of a 64-bit mix, Box-Muller) keyed by (seed, step, worker, idx)
@@ -71,7 +77,9 @@ __device__ __forceinline__ float4 load_grad4(const PushArgs& a, int k, int tenso
   return ld_stream_f4(reinterpret_cast<const float4*>(a.g32[k] + idx));
 }
 
-__global__ void __launch_bounds__(DRC_THREADS) push_encode_kernel(const __grid_constant__ PushArgs a) {
+// The tile loop of the push; returns the step it pushed.  WMOM: the worker-momentum build.
+template <bool WMOM>
+__device__ __forceinline__ unsigned long long push_encode_tiles(const PushArgs& a) {
   const unsigned long long step = *a.step_ptr;
   const bool lie = a.attack != 0 && a.adv_len > 0 &&
                    ((a.adv_bitmap[step % (unsigned long long)a.adv_len] >> a.worker) & 1u);
@@ -87,9 +95,20 @@ __global__ void __launch_bounds__(DRC_THREADS) push_encode_kernel(const __grid_c
     const int is_bf16 = a.tv.meta[tensor].is_bf16;
     const long long idx = (long long)tile * DRC_TILE + threadIdx.x * 4;
     const int lane_valid = valid - (int)threadIdx.x * 4;      // elements of this thread that are real
-    if (!a.cyclic) {
+    if (WMOM || !a.cyclic) {   // the momentum build has no cyclic path
       if (a.src_table && lane_valid <= 0) continue;             // padding of the slab stays zero, nothing to send
       float4 g = load_grad4(a, 0, tensor, is_bf16, idx, lane_valid);
+      if constexpr (WMOM) {
+        // no FMA: the library-op PS and the oracle (codes/oracle.py worker_momentum) round the two products separately
+        float4* mp = reinterpret_cast<float4*>(a.wmom + idx);
+        float4 m = *mp;
+        m.x = __fadd_rn(__fmul_rn(a.wm_beta, m.x), __fmul_rn(a.wm_scale, g.x));
+        m.y = __fadd_rn(__fmul_rn(a.wm_beta, m.y), __fmul_rn(a.wm_scale, g.y));
+        m.z = __fadd_rn(__fmul_rn(a.wm_beta, m.z), __fmul_rn(a.wm_scale, g.z));
+        m.w = __fadd_rn(__fmul_rn(a.wm_beta, m.w), __fmul_rn(a.wm_scale, g.w));
+        *mp = m;
+        g = m;
+      }
       if (lie) {
         if (a.attack == 1) { g.x *= a.magnitude; g.y *= a.magnitude; g.z *= a.magnitude; g.w *= a.magnitude; }
         else if (a.attack == 2) { g = make_float4(a.magnitude, a.magnitude, a.magnitude, a.magnitude); }
@@ -108,7 +127,7 @@ __global__ void __launch_bounds__(DRC_THREADS) push_encode_kernel(const __grid_c
       }
       st_f4(reinterpret_cast<float4*>(a.dst + idx), g);
       if (a.local_copy) *reinterpret_cast<float4*>(a.local_copy + idx) = g;
-    } else {
+    } else if constexpr (!WMOM) {
       if (a.src_table && lane_valid <= 0) continue;
       float4 re = make_float4(0.f, 0.f, 0.f, 0.f), im = re, plain = re;
 #pragma unroll 1
@@ -141,13 +160,31 @@ __global__ void __launch_bounds__(DRC_THREADS) push_encode_kernel(const __grid_c
       st_f4(d + 1, make_float4(re.z, im.z, re.w, im.w));
     }
   }
+  return step;
+}
+
+__global__ void __launch_bounds__(DRC_THREADS) push_encode_kernel(const __grid_constant__ PushArgs a) {
+  const unsigned long long step = push_encode_tiles<false>(a);
+  if (grid_last_cta(a.done_counter)) {
+    if (threadIdx.x == 0 && a.flag) st_release_sys(a.flag, step);
+  }
+}
+
+// the momentum build of the non-cyclic push (the cyclic code keeps no worker state)
+__global__ void __launch_bounds__(DRC_THREADS) push_encode_wmom_kernel(const __grid_constant__ PushArgs a) {
+  const unsigned long long step = push_encode_tiles<true>(a);
   if (grid_last_cta(a.done_counter)) {
     if (threadIdx.x == 0 && a.flag) st_release_sys(a.flag, step);
   }
 }
 
 extern "C" int drc_push_encode(const PushArgs* args, int grid, cudaStream_t stream) {
-  push_encode_kernel<<<grid, DRC_THREADS, 0, stream>>>(*args);
+  if (args->wmom) {
+    if (args->cyclic) return (int)cudaErrorInvalidValue;
+    push_encode_wmom_kernel<<<grid, DRC_THREADS, 0, stream>>>(*args);
+  } else {
+    push_encode_kernel<<<grid, DRC_THREADS, 0, stream>>>(*args);
+  }
   return (int)cudaGetLastError();
 }
 

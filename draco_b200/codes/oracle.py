@@ -4,6 +4,8 @@ They define the semantics the CUDA kernels (csrc/cuda/*.cu) and the C++ host twi
 (csrc/host/*.cpp) are tested against, tensor by tensor -- the reference applies every rule
 *per parameter tensor*, never on the concatenated model (src/master/rep_master.py:154-168,
 src/master/baseline_master.py:271-296).
+
+``worker_momentum`` is the one worker-side rule here, and it is fp32 on purpose: every path must produce its exact bits.
 """
 from __future__ import annotations
 
@@ -359,3 +361,21 @@ def sgd_momentum_step(p: np.ndarray, buf: np.ndarray, g: np.ndarray, lr: float, 
         buf = d_p.copy() if first_step else momentum * buf + (1.0 - dampening) * d_p
         d_p = d_p + momentum * buf if nesterov else buf
     return p - lr * d_p, buf
+
+
+def worker_momentum_coefficients(beta: float) -> Tuple[float, float]:
+    """(b, c) of worker momentum as fp32 values: b = fp32(beta), c = fp32(1 - beta) with 1 - beta formed in fp64 and rounded
+    once.  Every path (push kernel, library-op PS, this oracle) multiplies by exactly these two numbers."""
+    return float(np.float32(beta)), float(np.float32(1.0 - float(beta)))
+
+
+def worker_momentum(m: np.ndarray, g: np.ndarray, beta: float) -> np.ndarray:
+    """One step of worker-side momentum, dampened form (Karimireddy, He and Jaggi, ICML 2021; Allouah et al., AISTATS 2023):
+    m' = b m + c g in fp32, each product rounded, then the sum rounded (no fused multiply-add).  The state starts at zero and
+    there is no first-step copy.  bf16 gradients widen to fp32 exactly before the update."""
+    b, c = worker_momentum_coefficients(beta)
+    m32 = np.asarray(m, dtype=np.float32)
+    g32 = np.asarray(g, dtype=np.float32)
+    bm = np.multiply(np.float32(b), m32, dtype=np.float32)
+    cg = np.multiply(np.float32(c), g32, dtype=np.float32)
+    return np.add(bm, cg, dtype=np.float32)

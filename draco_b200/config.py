@@ -80,6 +80,7 @@ class JobConfig:
     worker_streams: int = 4         # >1: logical workers sharing a GPU run on (up to) this many concurrent CUDA streams
     zero_copy_grads: bool = True    # push reads gradients where autograd left them (pointer table), no flat gather
     attack_z: Optional[float] = None  # --err-mode alie: z of mu - z * sigma (None: Baruch et al.'s z_max for P and f)
+    worker_momentum: float = 0.0    # beta of worker-side momentum: every worker pushes m <- beta m + (1 - beta) g (0: off)
 
     # ---- derived --------------------------------------------------------------------------
     def resolve(self, world_size: int) -> "JobConfig":
@@ -121,6 +122,7 @@ class JobConfig:
         if self.compress and self.transport == "nccl_flat":
             raise ValueError("--transport nccl_flat is the uncompressed library comparator: pass --compress-grad None")
         self._check_ps_attack()
+        self._check_worker_momentum()
         if self.transport == "gloo":
             self.dtype = "fp32"
             self.cuda_graphs = False
@@ -148,6 +150,25 @@ class JobConfig:
         if m == "alie" and self.attack_z is None and alie_s(self.num_workers, self.worker_fail) < 1:
             raise ValueError(f"--err-mode alie: z_max = Phi^-1((P - s) / P) with s = floor(P/2 + 1) - f is undefined for "
                              f"{self.num_workers} workers and worker_fail {self.worker_fail} (s < 1); pass --attack-z")
+
+    def _check_worker_momentum(self) -> None:
+        """--worker-momentum beta: every worker keeps its own momentum and pushes it in place of its gradient."""
+        beta = self.worker_momentum
+        if not 0.0 <= beta < 1.0:
+            raise ValueError(f"--worker-momentum must lie in [0, 1) (0 = off; got {beta}): at 1 the gradient would never enter "
+                             f"the state")
+        if beta == 0.0:
+            return
+        if self.approach == "cyclic":
+            raise ValueError("--worker-momentum has no meaning under --approach cyclic: its decode recovers the exact sum of the "
+                             "gradients, so worker momentum would only re-derive the PS momentum (--momentum), and the codeword "
+                             "would need complex state")
+        if self.transport == "nccl_flat":
+            raise ValueError("--transport nccl_flat pushes the raw gradient buckets and keeps no worker state: use "
+                             "--transport nvl or nccl for --worker-momentum")
+        if self.err_mode == "omniscient":
+            raise ValueError("--err-mode omniscient replaces the liars' push with a row read from the PS, so their momentum "
+                             "could never advance: pick another --err-mode for --worker-momentum")
 
     @property
     def alie_z(self) -> float:
@@ -277,6 +298,11 @@ def add_fit_args(parser: argparse.ArgumentParser) -> argparse.ArgumentParser:
            "inverse-std direction) are applied by the PS per tensor from the honest workers' mean and standard deviation")
     a("--attack-z", type=float, default=None,
       help="--err-mode alie: the liars send mu - z * sigma (default: z_max = Phi^-1((P - s) / P), s = floor(P/2 + 1) - f)")
+    a("--worker-momentum", type=float, default=d.worker_momentum,
+      help="beta of worker-side momentum (0 = off): every worker keeps m <- beta m + (1 - beta) g and pushes m instead of its "
+           "gradient, which shrinks the honest workers' spread before the robust rule sees it (Karimireddy et al. 2021, El "
+           "Mhamdi et al. 2021).  --momentum still applies at the PS on top; the papers' recipe is --worker-momentum 0.9 "
+           "--momentum 0")
     a("--approach", type=str, default=d.approach,
       help="baseline | maj_vote | cyclic | detox (majority vote inside each repetition group, then --mode across the G group "
            "winners) | nnm (nearest-neighbour mixing: every worker's row is replaced, per tensor, by the mean of its "

@@ -57,9 +57,16 @@ def push_encode(layout: ArenaLayout, g32: Sequence[Addr], g16: Sequence[Addr], d
                 worker: int, done_counter: Addr, flag: Addr = None, coef: Optional[Sequence[complex]] = None,
                 adv_bitmap: Addr = None, adv_len: int = 0, attack: int = 0, magnitude: float = -100.0, seed: int = 428,
                 local_copy: Addr = None, grid: Optional[int] = None, tile_range: Optional[tuple] = None,
-                src_table: Addr = None) -> None:
+                src_table: Addr = None, wmom: Addr = None, wm_beta: float = 0.0) -> None:
     """Fused encode + adversary + store into ``dst`` (a peer pointer) + release flag.  ``coef`` given => cyclic encode
-    of ``len(coef)`` gradient streams into an interleaved complex64 slot.  ``tile_range=(t0, t1)`` pushes one bucket."""
+    of ``len(coef)`` gradient streams into an interleaved complex64 slot.  ``tile_range=(t0, t1)`` pushes one bucket.
+    ``wmom``: this worker's fp32 momentum arena; the push then advances it, m <- fp32(wm_beta) m + fp32(1 - wm_beta) g
+    (codes/oracle.py ``worker_momentum``), and sends m (through the adversary hook) instead of g."""
+    if wmom is not None:
+        if coef is not None:
+            raise ValueError("worker momentum is not defined for the cyclic encode (coef)")
+        if not 0.0 <= wm_beta < 1.0:
+            raise ValueError(f"worker momentum beta must lie in [0, 1), got {wm_beta}")
     a = N.PushArgs()
     if src_table is not None:
         # zero-copy mode: `src_table` is a device int64 [R, ntensors] table of per-tensor gradient pointers
@@ -94,6 +101,10 @@ def push_encode(layout: ArenaLayout, g32: Sequence[Addr], g16: Sequence[Addr], d
     a.done_counter = addr(done_counter)
     a.flag = addr(flag)
     a.local_copy = addr(local_copy)
+    if wmom is not None:
+        from ..codes.oracle import worker_momentum_coefficients
+        a.wmom = addr(wmom)
+        a.wm_beta, a.wm_scale = worker_momentum_coefficients(wm_beta)
     ntiles = layout.ntiles
     if tile_range is not None:
         a.tile_begin, a.tile_end = int(tile_range[0]), int(tile_range[1])

@@ -20,6 +20,7 @@ import torch
 import torch.distributed as dist
 
 from ..codes.adversary import PS_ATTACKS, generate_schedule
+from ..codes.oracle import worker_momentum_coefficients
 from ..config import JobConfig
 from ..data import TensorDataset
 from ..utils.codec import compress, decompress
@@ -60,6 +61,10 @@ class CollectiveEngine:
         self.use_adv = cfg.err_mode != "none" and cfg.worker_fail > 0
         wire = torch.complex64 if self.cyclic else torch.float32
         self.sendbuf = {w: torch.zeros(self.layout.total, dtype=wire, device=self.device) for w in self.local_workers}
+        # --worker-momentum: each local worker's fp32 state, advanced in _encode with the push kernel's roundings
+        self.worker_momentum: Dict[int, torch.Tensor] = (
+            {w: self.layout.new_arena(self.device) for w in self.local_workers} if cfg.worker_momentum > 0 else {})
+        self._wm_b, self._wm_c = worker_momentum_coefficients(cfg.worker_momentum)
         self.ps: Optional[TorchPS] = None
         if self.is_ps:
             self.slots = torch.zeros(self.P, self.layout.total, dtype=wire, device=self.device)
@@ -103,6 +108,13 @@ class CollectiveEngine:
             buf.zero_()
             for k in range(wc.R):
                 buf.add_(wc.flat_gradient(k).to(torch.complex64), alpha=complex(coef[k]))
+        elif self.worker_momentum:
+            # m <- b m + c g as two rounded fp32 products and a rounded sum (no FMA), like the push kernel; a liar's state
+            # follows its true gradient, the attack below acts on the copy it sends
+            m = self.worker_momentum[w]
+            m.mul_(self._wm_b)
+            m.add_(wc.flat_gradient(0) * self._wm_c)
+            buf.copy_(m)
         else:
             buf.copy_(wc.flat_gradient(0))
         if self.use_adv and self.schedule.is_adversary(w, step):

@@ -178,6 +178,10 @@ class FusedEngine:
             # the PS process also builds the model: its initial parameters are the job's initial parameters
             self.worker = WorkerCompute(cfg, device, self.local_workers, plan, dataset, self.layout, self.params_f32, model)
             self.worker.step_dev = self.step_dev       # dropout masks are keyed by the device step (graph replays advance it)
+        # --worker-momentum: one fp32 state arena per local logical worker, in the slot's element layout.  The push kernel
+        # advances it and sends it in place of the gradient (no extra launch); it starts at zero.
+        self.worker_momentum: Dict[int, torch.Tensor] = (
+            {w: self.layout.new_arena(device) for w in self.local_workers} if cfg.worker_momentum > 0 else {})
         if self.is_ps:
             self.ps = FusedPS(cfg, self.layout, device, self.params_f32, self.grad_in, self.groups, self.code,
                               adv_bitmap=self.adv_bitmap, adv_len=len(sched.ranks))
@@ -190,8 +194,10 @@ class FusedEngine:
     # ------------------------------------------------------------------ transport self-check
     def _dbg_loopback(self, w: int, g32, g16, push_kw) -> None:
         """Re-run the worker's encode + adversary into a LOCAL buffer and keep its 64-bit checksum (sum of the 32-bit
-        words): what the PS must find in slot ``w`` if every peer store of the real push landed."""
-        K.push_encode(self.layout, g32, g16, self._dbg_buf.data_ptr(), flag=None, **push_kw)
+        words): what the PS must find in slot ``w`` if every peer store of the real push landed.  With worker momentum a
+        second run would advance the state twice: the real push wrote what it sent into this buffer (``local_copy``)."""
+        if push_kw.get("wmom") is None:
+            K.push_encode(self.layout, g32, g16, self._dbg_buf.data_ptr(), flag=None, **push_kw)
         self._dbg_sums[w] = self._dbg_buf.view(torch.int32).sum(dtype=torch.int64)
 
     def _verify_checksums(self, step: int) -> None:
@@ -395,6 +401,9 @@ class FusedEngine:
                        attack=self.attack if self.attack < ATTACK_OMNISCIENT else 0,    # 4..6: not the worker's doing
                        magnitude=cfg.attack_magnitude, seed=cfg.seed,
                        src_table=wc.ptr_dev[w] if wc.zero_copy else None)
+        if self.worker_momentum:
+            push_kw.update(wmom=self.worker_momentum[w], wm_beta=cfg.worker_momentum,
+                           local_copy=self._dbg_buf if self.debug_checksum else None)
         if self.overlap_push and not lying_now:
             # bucketed push on a side stream, overlapped with the rest of the backward pass
             state = {"done": 0}

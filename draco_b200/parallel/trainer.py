@@ -21,7 +21,8 @@ import torch.distributed as dist
 
 from ..config import JobConfig
 from ..data import TensorDataset, load_dataset
-from ..utils.checkpoint import (checkpoint_path, load_checkpoint, model_buffers, restore_into, save_checkpoint)
+from ..utils.checkpoint import (arena_tensors, check_worker_momentum, checkpoint_path, load_checkpoint, model_buffers,
+                                restore_into, restore_worker_momentum, save_checkpoint)
 from ..utils.metrics import MetricsLogger
 
 
@@ -175,15 +176,34 @@ class Trainer:
                 pass
             dist.broadcast_object_list(box, src=self.eval_rank)
             bufs = box[0]
+        wmom = self._gather_worker_momentum() if self.cfg.worker_momentum > 0 else None
         if self.is_ps:
             ps = getattr(eng, "ps", None)
             mom = getattr(ps, "momentum", None)
             save_checkpoint(checkpoint_path(self.cfg.train_dir, step), eng.layout, eng.master_params(), mom, step,
-                            self.cfg, bufs, opt_state=getattr(ps, "opt_state", None))
+                            self.cfg, bufs, opt_state=getattr(ps, "opt_state", None), worker_momentum=wmom)
 
+    def _gather_worker_momentum(self) -> Dict[int, Dict[str, torch.Tensor]]:
+        """Every logical worker's momentum, per tensor on the CPU (complete on the PS).  Each process converts its local
+        workers'; in a multi-process job every worker process then broadcasts them, the way the BatchNorm statistics travel
+        (every process takes part in each broadcast)."""
+        eng = self.engine
+        out = {w: arena_tensors(eng.layout, m) for w, m in eng.worker_momentum.items()}
+        if self.world > 1:
+            for p in range(1, self.world):
+                if not eng.place.local_workers(p):
+                    continue
+                box = [out if self.rank == p else None]
+                dist.broadcast_object_list(box, src=p)
+                if self.rank == 0:
+                    out.update(box[0])
+        return out
     def resume(self, step: int) -> None:
         blob = load_checkpoint(checkpoint_path(self.cfg.train_dir, step))
+        check_worker_momentum(blob, self.cfg.worker_momentum)
         eng = self.engine
+        if self.cfg.worker_momentum > 0:
+            restore_worker_momentum(blob, eng.layout, eng.worker_momentum)       # every process: its own local workers
         ps = getattr(eng, "ps", None)
         if self.is_ps and hasattr(ps, "load_momentum"):
             # library-op PS: the momentum lives in the optimizer's state, rebuild it from the checkpoint

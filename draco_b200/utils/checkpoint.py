@@ -8,7 +8,8 @@ optimizer state (baseline_master.py:54-57).
 Here one file per checkpoint, same naming (``<train_dir>model_step_<N>``), containing logical (NCHW) parameter tensors,
 the momentum buffers, the step, the BatchNorm statistics of the evaluating worker (the PS never runs a forward pass, so
 its own BN statistics would be meaningless -- the reason the reference refuses to save ResNets on the PS) and the job
-config.  Resume works for every approach and restores optimizer state.
+config.  Resume works for every approach and restores optimizer state.  With ``--worker-momentum`` the blob also holds
+every logical worker's momentum (``"worker_momentum": {w: {tensor name: fp32 tensor}}``); the key is absent otherwise.
 """
 from __future__ import annotations
 
@@ -27,9 +28,11 @@ def checkpoint_path(train_dir: str, step: int) -> str:
 
 def save_checkpoint(path: str, layout: ArenaLayout, params: torch.Tensor, momentum: Optional[torch.Tensor], step: int,
                     cfg: JobConfig, buffers: Optional[Dict[str, torch.Tensor]] = None,
-                    opt_state: Optional[Dict[str, torch.Tensor]] = None) -> None:
+                    opt_state: Optional[Dict[str, torch.Tensor]] = None,
+                    worker_momentum: Optional[Dict[int, Dict[str, torch.Tensor]]] = None) -> None:
     """``momentum``: SGD momentum buffer / Adam first moment arena; ``opt_state``: further optimizer arenas by name
-    (Adam: ``exp_avg_sq``, AMSGrad: ``max_exp_avg_sq``) -- all saved per parameter tensor."""
+    (Adam: ``exp_avg_sq``, AMSGrad: ``max_exp_avg_sq``) -- all saved per parameter tensor.  ``worker_momentum``: every
+    logical worker's state as ``arena_tensors`` gives it (None: no worker momentum, no key)."""
     d = os.path.dirname(path)
     if d:
         os.makedirs(d, exist_ok=True)
@@ -43,9 +46,39 @@ def save_checkpoint(path: str, layout: ArenaLayout, params: torch.Tensor, moment
                     for i in range(layout.ntensors)} for name, arena in (opt_state or {}).items() if arena is not None}
     blob = {"format": "draco_b200/1", "step": int(step), "state_dict": state, "momentum": mom, "opt_state": extra,
             "buffers": {k: v.detach().cpu().clone() for k, v in (buffers or {}).items()}, "config": cfg.to_dict()}
+    if worker_momentum is not None:
+        blob["worker_momentum"] = {int(w): dict(t) for w, t in sorted(worker_momentum.items())}
     tmp = path + ".tmp"
     torch.save(blob, tmp)
     os.replace(tmp, path)
+
+
+def arena_tensors(layout: ArenaLayout, arena: torch.Tensor) -> Dict[str, torch.Tensor]:
+    """{tensor name: fp32 CPU tensor in the logical (NCHW) shape} of one arena."""
+    return {layout.specs[i].name: layout.view(arena, i).detach().float().cpu().contiguous().clone()
+            for i in range(layout.ntensors)}
+
+
+def check_worker_momentum(blob: dict, beta: float) -> None:
+    """A job resumes only from a checkpoint of the same kind: with worker momentum iff the job runs with it."""
+    has = "worker_momentum" in blob
+    if beta > 0 and not has:
+        raise ValueError(f"--worker-momentum {beta}: the checkpoint holds no worker momentum (it was written by a job without "
+                         f"--worker-momentum), so the workers' state cannot be restored")
+    if beta == 0 and has:
+        raise ValueError("the checkpoint holds worker momentum (it was written with --worker-momentum): resume it with the same "
+                         "--worker-momentum, or the workers' state would be dropped")
+
+
+def restore_worker_momentum(blob: dict, layout: ArenaLayout, arenas: Dict[int, torch.Tensor]) -> None:
+    """Copy the saved state of every worker in ``arenas`` (this process's local workers) into its arena."""
+    saved = blob["worker_momentum"]
+    with torch.no_grad():
+        for w, arena in arenas.items():
+            if w not in saved:
+                raise ValueError(f"the checkpoint holds no worker momentum for worker {w} (it has workers {sorted(saved)})")
+            for i, spec in enumerate(layout.specs):
+                layout.view(arena, i).copy_(saved[w][spec.name])
 
 
 def load_checkpoint(path: str) -> dict:
