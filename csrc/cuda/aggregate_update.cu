@@ -90,8 +90,7 @@ template <> __device__ __forceinline__ void sort_net<16>(unsigned int (&k)[16]) 
 }
 #undef CX
 
-// One coordinate of mode 3 (trimmed_sum) and of mode 4 (near_median_sum) for the mixed path: the same steps as the loops of
-// trimmed_mean_f4 and near_median_mean_f4, which keep their own copies so that the unmixed kernels compile as before.
+// One coordinate of mode 3: sort the K keys (padded to N) and sum the K - 2 trim in the middle in ascending order
 template <int N>
 __device__ __forceinline__ float trimmed_sum(unsigned int (&k)[N], int K, int trim) {
   sort_net<N>(k);
@@ -100,33 +99,6 @@ __device__ __forceinline__ float trimmed_sum(unsigned int (&k)[N], int K, int tr
   for (int r = 0; r < N; ++r)
     if (r >= trim && r < K - trim) s += key_float(k[r]);
   return s;
-}
-
-// SEL: row r of `tensor` is worker slot select[r][tensor] instead of slot r
-template <int N, bool SEL>
-__device__ __forceinline__ float4 trimmed_mean_f4(const UpdateArgs& a, long long idx, int tensor) {
-  unsigned int k[4][N];
-#pragma unroll
-  for (int r = 0; r < N; ++r) {
-    if (r < a.K) {
-      const int slot = SEL ? a.select[r * a.tv.ntensors + tensor] : r;
-      const float4 v = ld_f4(reinterpret_cast<const float4*>(a.grad_in + slot * a.slot_stride + idx));
-      k[0][r] = float_key(v.x); k[1][r] = float_key(v.y); k[2][r] = float_key(v.z); k[3][r] = float_key(v.w);
-    } else {
-      k[0][r] = k[1][r] = k[2][r] = k[3][r] = 0xFFFFFFFFu;
-    }
-  }
-  float out[4];
-#pragma unroll
-  for (int e = 0; e < 4; ++e) {
-    sort_net<N>(k[e]);
-    float s = 0.f;
-#pragma unroll
-    for (int r = 0; r < N; ++r)
-      if (r >= a.trim && r < a.K - a.trim) s += key_float(k[e][r]);
-    out[e] = s;
-  }
-  return make_float4(out[0], out[1], out[2], out[3]);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -188,50 +160,25 @@ __device__ __forceinline__ float near_median_sum(unsigned int (&k)[N], int K, in
   return sum;
 }
 
-template <int N>
-__device__ __forceinline__ float4 near_median_mean_f4(const UpdateArgs& a, long long idx, int tensor) {
+// Modes 3 and 4 on raw rows: the thread loads its 4 coordinates of the K rows as keys (row r of `tensor` is worker slot
+// select[r][tensor] with SEL, slot r without), then reduces every coordinate with trimmed_sum or near_median_sum.
+template <int MODE, int N, bool SEL>
+__device__ __forceinline__ float4 raw_robust_f4(const UpdateArgs& a, long long idx, int tensor) {
+  const int K = a.K, trim = a.trim;
   unsigned int k[4][N];
 #pragma unroll
   for (int r = 0; r < N; ++r) {
     if (r < a.K) {
-      const int slot = a.select[r * a.tv.ntensors + tensor];
+      const int slot = SEL ? a.select[r * a.tv.ntensors + tensor] : r;
       const float4 v = ld_f4(reinterpret_cast<const float4*>(a.grad_in + slot * a.slot_stride + idx));
       k[0][r] = float_key(v.x); k[1][r] = float_key(v.y); k[2][r] = float_key(v.z); k[3][r] = float_key(v.w);
     } else {
       k[0][r] = k[1][r] = k[2][r] = k[3][r] = 0xFFFFFFFFu;
     }
   }
-  const int beta = a.K - 2 * a.trim, span = 2 * a.trim;
   float out[4];
 #pragma unroll
-  for (int e = 0; e < 4; ++e) {
-    sort_net<N>(k[e]);
-    unsigned int md[N];                                        // md[0], md[1] = k[e][(K - 1) / 2], k[e][(K - 1) / 2 + 1]
-#pragma unroll
-    for (int j = 0; j < N; ++j) md[j] = k[e][j];
-    barrel_shift<N, 1>(md, (a.K - 1) / 2);
-    const float lo = key_float(md[0]), hi = key_float(md[1]);
-    const float m = (a.K & 1) ? lo : __fadd_rn(__fmul_rn(0.5f, lo), __fmul_rn(0.5f, hi));
-    unsigned int sh[N];                                        // sh[j] = k[e][j + beta]
-#pragma unroll
-    for (int j = 0; j < N; ++j) sh[j] = k[e][j];
-    barrel_shift<N, 1>(sh, beta);
-    int s = 0;
-    bool moving = true;
-#pragma unroll
-    for (int j = 0; j < N - 1; ++j) {
-      if (j < span && moving) {
-        const float vin = key_float(sh[j]), vout = key_float(k[e][j]);
-        moving = nearer(fabsf(__fsub_rn(vin, m)), fabsf(__fsub_rn(vout, m))) || vin == vout || (vin != vin && vout != vout);
-        s += moving;
-      }
-    }
-    float sum = 0.f;
-#pragma unroll
-    for (int r = 0; r < N; ++r)
-      if (r >= s && r < s + beta) sum += key_float(k[e][r]);
-    out[e] = sum;
-  }
+  for (int e = 0; e < 4; ++e) out[e] = MODE == 3 ? trimmed_sum<N>(k[e], K, trim) : near_median_sum<N>(k[e], K, trim);
   return make_float4(out[0], out[1], out[2], out[3]);
 }
 
@@ -241,8 +188,9 @@ __device__ __forceinline__ float4 near_median_mean_f4(const UpdateArgs& a, long 
 //     y = +0.0f;  for j = 0, 1, ..., mixP - 1 in ascending order: if bit j of mask_i is set, y = y + x_j  (round to nearest);
 //     y = y * mix_scale  (one rounded multiply, mix_scale = fp32(1 / n_mix)),
 // with mask_i = mix[i][t] for mode 3 (the K = mixP mixed rows) and mask_r = mix[select[r][t]][t] for mode 4 (the K = theta
-// mixed rows bulyan_select chose).  The K mixed values are then sorted and reduced exactly as modes 3 and 4 do without
-// mixing.  The raw rows stay in registers (N = SORT_N >= mixP float4s); the keys are built one coordinate at a time.
+// mixed rows bulyan_select chose).  The K mixed values are then reduced by trimmed_sum / near_median_sum as in raw_robust_f4.
+// The raw rows stay in registers (N = SORT_N >= mixP float4s); the keys are built one coordinate at a time, which holds the
+// registers down where raw_robust_f4 keeps the keys of all 4 coordinates.
 // ---------------------------------------------------------------------------------------------
 template <int MODE, int N>
 __device__ __forceinline__ float4 mixed_robust_f4(const UpdateArgs& a, long long idx, int tensor) {
@@ -273,11 +221,11 @@ __device__ __forceinline__ float4 mixed_robust_f4(const UpdateArgs& a, long long
   return make_float4(out[0], out[1], out[2], out[3]);
 }
 
-// SORT_N: modes 3 and 4, the sorting-network size (4, 8 or 16 >= K).  Each size is its own instantiation so that a launch pays the
-// registers of its own network (4 x SORT_N keys per thread), not those of the largest one.  SEL: mode 3 only, rows come through
-// the `select` table (DETOX); a separate instantiation, so the launches without a table run the code they always ran.  Mode 4
-// always reads through the table and is instantiated as <4, N, true>.  MIX: modes 3 and 4 over nearest-neighbour mixed rows
-// (mixed_robust_f4), instantiated as <3, N, false, true> and <4, N, true, true> with N >= mixP.
+// SORT_N: modes 3 and 4, the sorting-network size (4, 8 or 16 >= K, or >= mixP with MIX).  Each size is its own instantiation so
+// that a launch pays the registers of its own network (4 x SORT_N keys per thread), not those of the largest one.  SEL: rows come
+// through the `select` table (DETOX's winners, Bulyan's choice); mode 3 without a table is its own instantiation, mode 4 always
+// has one.  MIX: modes 3 and 4 over nearest-neighbour mixed rows (mixed_robust_f4), instantiated as <3, N, false, true> and
+// <4, N, true, true>.
 template <int MODE, int SORT_N = 0, bool SEL = false, bool MIX = false>
 __global__ void __launch_bounds__(DRC_THREADS) aggregate_update_kernel(const __grid_constant__ UpdateArgs a) {
   const HyperParams hp = *a.hp;
@@ -311,10 +259,8 @@ __global__ void __launch_bounds__(DRC_THREADS) aggregate_update_kernel(const __g
       }
     } else if constexpr (MIX) {
       g = mixed_robust_f4<MODE, SORT_N>(a, idx, tensor);
-    } else if constexpr (MODE == 3) {
-      g = trimmed_mean_f4<SORT_N, SEL>(a, idx, tensor);
-    } else if constexpr (MODE == 4) {
-      g = near_median_mean_f4<SORT_N>(a, idx, tensor);
+    } else if constexpr (MODE == 3 || MODE == 4) {
+      g = raw_robust_f4<MODE, SORT_N, SEL>(a, idx, tensor);
     } else {
       for (int k = 0; k < a.K; ++k) {
         const float2 v = a.recomb[tensor * a.K + k];
@@ -376,50 +322,38 @@ __global__ void __launch_bounds__(DRC_THREADS) aggregate_update_kernel(const __g
   }
 }
 
-template <int N>
-static void launch_trimmed_mean(const UpdateArgs* args, int grid, cudaStream_t stream) {
-  if (args->select) aggregate_update_kernel<3, N, true><<<grid, DRC_THREADS, 0, stream>>>(*args);
-  else aggregate_update_kernel<3, N, false><<<grid, DRC_THREADS, 0, stream>>>(*args);
-}
-
-template <int MODE>
-static void launch_mixed(const UpdateArgs* args, int grid, cudaStream_t stream) {
-  if (args->mixP <= 4) aggregate_update_kernel<MODE, 4, MODE == 4, true><<<grid, DRC_THREADS, 0, stream>>>(*args);
-  else if (args->mixP <= 8) aggregate_update_kernel<MODE, 8, MODE == 4, true><<<grid, DRC_THREADS, 0, stream>>>(*args);
-  else aggregate_update_kernel<MODE, 16, MODE == 4, true><<<grid, DRC_THREADS, 0, stream>>>(*args);
+// modes 3 and 4: the instantiation with the smallest sorting network that holds `rows` (K, or mixP with mixing)
+template <int MODE, bool SEL, bool MIX>
+static void launch_sorted(const UpdateArgs* args, int rows, int grid, cudaStream_t stream) {
+  if (rows <= 4) aggregate_update_kernel<MODE, 4, SEL, MIX><<<grid, DRC_THREADS, 0, stream>>>(*args);
+  else if (rows <= 8) aggregate_update_kernel<MODE, 8, SEL, MIX><<<grid, DRC_THREADS, 0, stream>>>(*args);
+  else aggregate_update_kernel<MODE, 16, SEL, MIX><<<grid, DRC_THREADS, 0, stream>>>(*args);
 }
 
 extern "C" int drc_aggregate_update(const UpdateArgs* args, int grid, cudaStream_t stream) {
+  const int mode = args->mode, K = args->K;
   if (args->ndst > DRC_MAX_DST || args->flags.n > DRC_MAX_DST) return (int)cudaErrorInvalidValue;
+  // modes 3 and 4 sort K <= TRIM_MAXP rows per coordinate and keep K - 2 trim of them; mode 4 reads its K = theta rows
+  // through the table bulyan_select filled
+  if ((mode == 3 || mode == 4) && (K < 1 || K > TRIM_MAXP || args->trim < 0 || 2 * args->trim >= K))
+    return (int)cudaErrorInvalidValue;
+  if (mode == 4 && !args->select) return (int)cudaErrorInvalidValue;
   // nearest-neighbour mixing: modes 3 (K = mixP mixed rows, no row table) and 4 (K = theta mixed rows named by `select`)
   if (args->mix) {
-    if (args->mixP < 1 || args->mixP > TRIM_MAXP || !(args->mix_scale > 0.f) || args->trim < 0 || 2 * args->trim >= args->K)
-      return (int)cudaErrorInvalidValue;
-    if (args->mode == 3 && args->K == args->mixP && !args->select) launch_mixed<3>(args, grid, stream);
-    else if (args->mode == 4 && args->K >= 1 && args->K <= args->mixP && args->select) launch_mixed<4>(args, grid, stream);
+    if (args->mixP < 1 || args->mixP > TRIM_MAXP || !(args->mix_scale > 0.f)) return (int)cudaErrorInvalidValue;
+    if (mode == 3 && K == args->mixP && !args->select) launch_sorted<3, false, true>(args, args->mixP, grid, stream);
+    else if (mode == 4 && K <= args->mixP) launch_sorted<4, true, true>(args, args->mixP, grid, stream);
     else return (int)cudaErrorInvalidValue;
     return (int)cudaGetLastError();
   }
-  if (args->mode == 3 && (args->K < 1 || args->K > TRIM_MAXP || args->trim < 0 || 2 * args->trim >= args->K))
-    return (int)cudaErrorInvalidValue;
   // a row table names at most TRIM_MAXP rows under the weighted sum (the weight-space geometric median's limit); the cyclic
   // recombination reads every worker's slot and has no use for one
-  if (args->select && (args->mode == 1 || (args->mode == 2 && (args->K < 1 || args->K > TRIM_MAXP))))
-    return (int)cudaErrorInvalidValue;
-  // mode 4 reads its K = theta rows through the table bulyan_select filled
-  if (args->mode == 4) {
-    if (args->K < 1 || args->K > TRIM_MAXP || args->trim < 0 || 2 * args->trim >= args->K || !args->select)
-      return (int)cudaErrorInvalidValue;
-    if (args->K <= 4) aggregate_update_kernel<4, 4, true><<<grid, DRC_THREADS, 0, stream>>>(*args);
-    else if (args->K <= 8) aggregate_update_kernel<4, 8, true><<<grid, DRC_THREADS, 0, stream>>>(*args);
-    else aggregate_update_kernel<4, 16, true><<<grid, DRC_THREADS, 0, stream>>>(*args);
-    return (int)cudaGetLastError();
-  }
-  if (args->mode == 0) aggregate_update_kernel<0><<<grid, DRC_THREADS, 0, stream>>>(*args);
-  else if (args->mode == 2) aggregate_update_kernel<2><<<grid, DRC_THREADS, 0, stream>>>(*args);
-  else if (args->mode == 3 && args->K <= 4) launch_trimmed_mean<4>(args, grid, stream);
-  else if (args->mode == 3 && args->K <= 8) launch_trimmed_mean<8>(args, grid, stream);
-  else if (args->mode == 3) launch_trimmed_mean<16>(args, grid, stream);
+  if (args->select && (mode == 1 || (mode == 2 && (K < 1 || K > TRIM_MAXP)))) return (int)cudaErrorInvalidValue;
+  if (mode == 0) aggregate_update_kernel<0><<<grid, DRC_THREADS, 0, stream>>>(*args);
+  else if (mode == 2) aggregate_update_kernel<2><<<grid, DRC_THREADS, 0, stream>>>(*args);
+  else if (mode == 3 && args->select) launch_sorted<3, true, false>(args, K, grid, stream);
+  else if (mode == 3) launch_sorted<3, false, false>(args, K, grid, stream);
+  else if (mode == 4) launch_sorted<4, true, false>(args, K, grid, stream);
   else aggregate_update_kernel<1><<<grid, DRC_THREADS, 0, stream>>>(*args);
   return (int)cudaGetLastError();
 }

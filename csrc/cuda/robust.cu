@@ -197,6 +197,12 @@ __global__ void __launch_bounds__(DRC_THREADS) pair_dist_kernel(const __grid_con
   }
 }
 
+// Entry (i, j), i != j, of one tensor's pair table: pair (lo < hi) sits at hi * (hi - 1) / 2 + lo
+__device__ __forceinline__ double pair_at(const double* d2, int i, int j) {
+  const int lo = i < j ? i : j, hi = i < j ? j : i;
+  return d2[hi * (hi - 1) / 2 + lo];
+}
+
 struct KrumSelectArgs {
   double* pair_d2;                // consumed and zeroed
   int T, P, s;
@@ -223,8 +229,7 @@ __global__ void krum_select_kernel(const __grid_constant__ KrumSelectArgs a) {
     double nb[KRUM_MAXP]; int c = 0;
     for (int j = 0; j < a.P; ++j) {
       if (j == i) continue;
-      int lo = i < j ? i : j, hi = i < j ? j : i;
-      nb[c++] = d2[hi * (hi - 1) / 2 + lo];
+      nb[c++] = pair_at(d2, i, j);
     }
     for (int x = 1; x < c; ++x) { double k = nb[x]; int y = x - 1; while (y >= 0 && less_nan_last(k, nb[y])) { nb[y + 1] = nb[y]; --y; } nb[y + 1] = k; }
     double score = 0.0;
@@ -302,8 +307,7 @@ __global__ void __launch_bounds__(BULYAN_SELECT_THREADS) bulyan_select_kernel(co
     key[j] = ~0ull;
     id[j] = lane;
     if (j < a.P && lane < a.P && j != lane) {
-      const int lo = lane < j ? lane : j, hi = lane < j ? j : lane;
-      key[j] = dist_key(d2[hi * (hi - 1) / 2 + lo]);
+      key[j] = dist_key(pair_at(d2, lane, j));
       id[j] = j;
     }
   }
@@ -378,10 +382,7 @@ __global__ void __launch_bounds__(NNM_THREADS) nnm_mix_kernel(const __grid_const
   for (int j = 0; j < KRUM_MAXP; ++j) {
     key[j] = ~0ull;                                            // self and padding sort after every neighbour
     id[j] = j;
-    if (j < a.P && lane < a.P && j != lane) {
-      const int lo = lane < j ? lane : j, hi = lane < j ? j : lane;
-      key[j] = dist_key(d2[hi * (hi - 1) / 2 + lo]);
-    }
+    if (j < a.P && lane < a.P && j != lane) key[j] = dist_key(pair_at(d2, lane, j));
   }
   sort_pairs16(key, id);                                       // the P - 1 neighbours first, nearest first, NaN last
   const int need = a.P - a.f - 1;                              // neighbours besides row i itself
@@ -408,10 +409,7 @@ __global__ void __launch_bounds__(NNM_THREADS) nnm_mix_kernel(const __grid_const
 #pragma unroll
     for (int l = 0; l < KRUM_MAXP; ++l) {
       row[l] = 0.0;
-      if (l < a.P && lane < a.P && l != lane) {
-        const int lo = lane < l ? lane : l, hi = lane < l ? l : lane;
-        row[l] = d2[hi * (hi - 1) / 2 + lo];
-      }
+      if (l < a.P && lane < a.P && l != lane) row[l] = pair_at(d2, lane, l);
     }
     __syncwarp();                                              // every lane has read its row before any lane writes
     double u[KRUM_MAXP];                                       // u[l] = sum over j in N_lane of D[j][l]
@@ -534,8 +532,7 @@ __global__ void geomed_weights_kernel(const __grid_constant__ GeoMedWeightsArgs 
   for (int j = 0; j < KRUM_MAXP; ++j) {
     row[j] = 0.0;
     if (j < a.P && lane < a.P && j != lane) {
-      const int lo = lane < j ? lane : j, hi = lane < j ? j : lane;
-      row[j] = d2[hi * (hi - 1) / 2 + lo];
+      row[j] = pair_at(d2, lane, j);
       maxd = fmax(maxd, row[j]);
     }
   }

@@ -232,26 +232,18 @@ def aggregate_update(layout: ArenaLayout, grad_in: Addr, slot_stride: int, *, pa
         if select is not None:
             _check_row_table(layout, select, K)
         recomb = weights
-    if trim is not None:
-        assert recomb is None
+    if trim is not None or near_median is not None:       # modes 3 and 4 sort K <= 16 rows and drop 2 * trim of them
+        assert recomb is None and (trim is None or near_median is None)
+        name, var, t = ("trimmed mean", "trim", trim) if trim is not None else ("nearest-to-median mean", "f", near_median)
+        if near_median is not None and select is None:
+            raise ValueError("nearest-to-median mean: needs the select table of the rows bulyan_select chose")
         if select is not None:
             _check_row_table(layout, select, K)
-        if not (1 <= K <= 16 and 0 <= 2 * trim < K):
-            raise ValueError(f"trimmed mean: K = {K} rows (at most 16) must exceed 2 * trim = {2 * trim}")
-        if abs(scale * (K - 2 * trim) - 1.0) > 1e-6:
-            raise ValueError(f"trimmed mean: scale must be 1 / (K - 2 * trim) = {1.0 / (K - 2 * trim)}, got {scale}")
-        a.mode, a.trim = 3, int(trim)
-    if near_median is not None:
-        assert recomb is None and trim is None
-        if select is None:
-            raise ValueError("nearest-to-median mean: needs the select table of the rows bulyan_select chose")
-        _check_row_table(layout, select, K)
-        f = near_median
-        if not (1 <= K <= 16 and 0 <= 2 * f < K):
-            raise ValueError(f"nearest-to-median mean: K = {K} rows (at most 16) must exceed 2 * f = {2 * f}")
-        if abs(scale * (K - 2 * f) - 1.0) > 1e-6:
-            raise ValueError(f"nearest-to-median mean: scale must be 1 / (K - 2 * f) = {1.0 / (K - 2 * f)}, got {scale}")
-        a.mode, a.trim = 4, int(f)
+        if not (1 <= K <= 16 and 0 <= 2 * t < K):
+            raise ValueError(f"{name}: K = {K} rows (at most 16) must exceed 2 * {var} = {2 * t}")
+        if abs(scale * (K - 2 * t) - 1.0) > 1e-6:
+            raise ValueError(f"{name}: scale must be 1 / (K - 2 * {var}) = {1.0 / (K - 2 * t)}, got {scale}")
+        a.mode, a.trim = 3 if trim is not None else 4, int(t)
     if mix is not None:
         if trim is None and near_median is None:
             raise ValueError("mixing: only the trimmed mean / median (trim=) and Bulyan's stage (near_median=) take mix=")
@@ -400,6 +392,14 @@ def geometric_median(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: in
 GEOMED_FAST_MAXP = 16
 
 
+def _pair_dist(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, pair_d2: torch.Tensor,
+               rows: Optional[torch.Tensor]) -> None:
+    """One pass over the slab: the squared distances between the P rows of every tensor, added into the zeroed fp64
+    ``pair_d2`` [T, P(P-1)/2] (row i of tensor t is worker slot ``rows[i, t]``, or slot i without a table)."""
+    pa = N.PairDistArgs(addr(grad_in), slot_stride, P, layout.tile_view(pair_d2.device), pair_d2.data_ptr(), addr(rows))
+    N.check(N.cuda().drc_pair_dist(C.byref(pa), stream_grid(layout, 4), _stream()), "pair_dist")
+
+
 def geometric_median_weights(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, pair_d2: torch.Tensor,
                              weights: torch.Tensor, max_iter: int = 256, eps: float = 1e-10,
                              iters_out: Optional[torch.Tensor] = None, rows: Optional[torch.Tensor] = None,
@@ -412,13 +412,11 @@ def geometric_median_weights(layout: ArenaLayout, grad_in: Addr, slot_stride: in
     assert P <= GEOMED_FAST_MAXP
     if rows is not None:
         _check_row_table(layout, rows, P)
-    lib = N.cuda()
     if not filled:
-        pa = N.PairDistArgs(addr(grad_in), slot_stride, P, layout.tile_view(weights.device), pair_d2.data_ptr(), addr(rows))
-        N.check(lib.drc_pair_dist(C.byref(pa), stream_grid(layout, 4), _stream()), "pair_dist")
+        _pair_dist(layout, grad_in, slot_stride, P, pair_d2, rows)
     wa = N.GeoMedWeightsArgs(pair_d2.data_ptr(), layout.ntensors, P, max_iter, eps, weights.data_ptr(),
                              iters_out.data_ptr() if iters_out is not None else None)
-    N.check(lib.drc_geomed_weights(C.byref(wa), _stream()), "geomed_weights")
+    N.check(N.cuda().drc_geomed_weights(C.byref(wa), _stream()), "geomed_weights")
     return weights
 
 
@@ -431,12 +429,10 @@ def krum_select(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, s:
     assert 1 <= m <= P and select.numel() >= m * layout.ntensors
     if rows is not None:
         _check_row_table(layout, rows, P)
-    lib = N.cuda()
     if not filled:
-        pa = N.PairDistArgs(addr(grad_in), slot_stride, P, layout.tile_view(select.device), pair_d2.data_ptr(), addr(rows))
-        N.check(lib.drc_pair_dist(C.byref(pa), stream_grid(layout, 4), _stream()), "pair_dist")
+        _pair_dist(layout, grad_in, slot_stride, P, pair_d2, rows)
     ka = N.KrumSelectArgs(pair_d2.data_ptr(), layout.ntensors, P, s, m, select.data_ptr(), addr(rows))
-    N.check(lib.drc_krum_select(C.byref(ka), _stream()), "krum_select")
+    N.check(N.cuda().drc_krum_select(C.byref(ka), _stream()), "krum_select")
 
 
 def bulyan_select(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, f: int, pair_d2: torch.Tensor,
@@ -451,12 +447,10 @@ def bulyan_select(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, 
     _check_row_table(layout, select, P - 2 * f)
     if rows is not None:
         _check_row_table(layout, rows, P)
-    lib = N.cuda()
     if not filled:
-        pa = N.PairDistArgs(addr(grad_in), slot_stride, P, layout.tile_view(select.device), pair_d2.data_ptr(), addr(rows))
-        N.check(lib.drc_pair_dist(C.byref(pa), stream_grid(layout, 4), _stream()), "pair_dist")
+        _pair_dist(layout, grad_in, slot_stride, P, pair_d2, rows)
     ba = N.BulyanSelectArgs(pair_d2.data_ptr(), layout.ntensors, P, f, select.data_ptr(), addr(rows))
-    N.check(lib.drc_bulyan_select(C.byref(ba), _stream()), "bulyan_select")
+    N.check(N.cuda().drc_bulyan_select(C.byref(ba), _stream()), "bulyan_select")
 
 
 def nnm_mix(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, f: int, pair_d2: torch.Tensor, mix: torch.Tensor,
@@ -469,11 +463,9 @@ def nnm_mix(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, f: int
     if not (0 <= f < P <= ROW_TABLE_MAXROWS):
         raise ValueError(f"nnm_mix: needs 0 <= f < P <= {ROW_TABLE_MAXROWS} (got P = {P}, f = {f})")
     _check_row_table(layout, mix, P)
-    lib = N.cuda()
-    pa = N.PairDistArgs(addr(grad_in), slot_stride, P, layout.tile_view(mix.device), pair_d2.data_ptr(), None)
-    N.check(lib.drc_pair_dist(C.byref(pa), stream_grid(layout, 4), _stream()), "pair_dist")
+    _pair_dist(layout, grad_in, slot_stride, P, pair_d2, None)
     na = N.NnmMixArgs(pair_d2.data_ptr(), layout.ntensors, P, f, mix.data_ptr(), int(bool(mixed_out)))
-    N.check(lib.drc_nnm_mix(C.byref(na), _stream()), "nnm_mix")
+    N.check(N.cuda().drc_nnm_mix(C.byref(na), _stream()), "nnm_mix")
 
 
 def nnm_fold(layout: ArenaLayout, P: int, f: int, mix: torch.Tensor, w_raw: torch.Tensor, *, select: Optional[torch.Tensor] = None,

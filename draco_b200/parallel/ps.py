@@ -11,6 +11,7 @@ src/master/*.py):
 """
 from __future__ import annotations
 
+from dataclasses import dataclass
 from typing import Dict, List, Optional, Sequence
 
 import numpy as np
@@ -50,28 +51,44 @@ NNM_RULES = {"coordinate_median": "nnm_median", "trimmed_mean": "nnm_trimmed_mea
              "multi_krum": "nnm_multi_krum", "geometric_median": "nnm_geomedian", "bulyan": "nnm_bulyan"}
 
 
-def coordinate_trim(cfg: JobConfig) -> int:
-    """Values dropped at each end of every coordinate: (P - 1) // 2 for the median, ``--worker-fail`` for the trimmed mean."""
-    return (cfg.num_workers - 1) // 2 if select_rule(cfg) in ("median", "nnm_median") else cfg.worker_fail
-
-
 # rules the fused PS applies bucket by bucket while the workers still push (nothing in them needs the whole tensor at once)
 PIPELINED_RULES = ("mean", "vote", "median", "trimmed_mean", "detox_median", "detox_trimmed_mean")
 
-
-def detox_trim(cfg: JobConfig) -> int:
-    """DETOX's ``coordinate_trim`` over the G group winners: (G - 1) // 2 for the median, b_G for the trimmed mean."""
-    return (cfg.num_groups - 1) // 2 if select_rule(cfg) == "detox_median" else cfg.captured_group_bound
-
-
-def multi_krum_m(cfg: JobConfig) -> int:
-    """Rows multi-Krum averages: P - f."""
-    return cfg.num_workers - cfg.worker_fail
+# the optimizer's mode string for each base rule (SGDModified / AdamModified.step(mode=))
+_OPT_MODE = {"mean": "normal", "vote": "maj_vote", "cyclic": "cyclic", "median": "coordinate_median", "trimmed_mean": "trimmed_mean",
+             "krum": "krum", "multi_krum": "multi_krum", "geomedian": "geometric_median", "bulyan": "bulyan"}
 
 
-def bulyan_f(cfg: JobConfig) -> int:
-    """Bulyan's tolerance: ``--worker-fail`` over the P workers, b_G over the G group winners under DETOX."""
-    return cfg.captured_group_bound if select_rule(cfg) == "detox_bulyan" else cfg.worker_fail
+@dataclass(frozen=True)
+class RulePlan:
+    """A job's aggregation rule as a row source and a base rule, with every parameter worked out once."""
+    rule: str           # select_rule's name
+    source: str         # raw: the P worker slots | detox: the G group winners of the vote | nnm: the P mixed rows
+    base: str           # mean | vote | cyclic | median | trimmed_mean | krum | multi_krum | geomedian | bulyan
+    rows: int           # rows the base rule runs on: P, or G over the group winners
+    f: int              # rows it tolerates: worker_fail, or b_G over the group winners
+    trim: int           # median / trimmed mean: values dropped at each end of a coordinate
+    m: int              # Krum / multi-Krum: rows averaged
+    theta: int          # Bulyan: rows selected
+    opt_mode: str       # the optimizer's mode string
+    pipelined: bool     # the fused PS may apply it bucket by bucket (PIPELINED_RULES)
+
+
+def rule_plan(cfg: JobConfig) -> RulePlan:
+    """The row source and base rule of ``select_rule(cfg)``: the vote is the mean of the group winners, ``detox_*`` runs the
+    rule across them (f = b_G), ``nnm_*`` on the mixed rows."""
+    rule = select_rule(cfg)
+    source, base = "raw", rule
+    if rule == "vote" or rule.startswith("detox_"):
+        source, base = "detox", rule.removeprefix("detox_")
+    elif rule.startswith("nnm_"):
+        source, base = "nnm", rule.removeprefix("nnm_")
+    rows = cfg.num_groups if source == "detox" else cfg.num_workers
+    f = cfg.captured_group_bound if source == "detox" else cfg.worker_fail
+    trim = {"median": (rows - 1) // 2, "trimmed_mean": f}.get(base, 0)
+    m = {"krum": 1, "multi_krum": rows - f}.get(base, 0)
+    return RulePlan(rule, source, base, rows, f, trim, m, rows - 2 * f if base == "bulyan" else 0, _OPT_MODE[base],
+                    rule in PIPELINED_RULES)
 
 
 def hyperparams_tensor(cfg: JobConfig, device) -> torch.Tensor:
@@ -103,68 +120,38 @@ class FusedPS:
         T = layout.ntensors
         self.cyclic = cfg.approach == "cyclic"
         self.slot_stride = layout.total
-        self.rule = select_rule(cfg)
+        self.plan = plan = rule_plan(cfg)
+        self.rule = plan.rule
         # --err-mode alie | minmax: the liar slots of each bucket are overwritten after its flags and before its decode
         self.attack = attack_code(cfg.err_mode) if cfg.err_mode in PS_ATTACKS and adv_bitmap is not None else 0
         self.adv_bitmap, self.adv_len = adv_bitmap, adv_len
         self.attack_z = cfg.alie_z if self.attack == ATTACK_ALIE else 0.0
         self.attack_ws = K.AttackWorkspace(layout, self.P, device) if self.attack == ATTACK_MINMAX else None
-        if self.rule == "vote" or self.rule.startswith("detox"):
+        # row source.  DETOX: the rule runs on the G rows the vote's winner_slot table names, inside the kernels that read the
+        # slab anyway.  NNM: the mixing masks; the rule then runs on the mixed rows.
+        if plan.source == "detox":
             self.group_table = torch.from_numpy(groups.as_table()).to(device)
             G = self.group_table.shape[0]
             self.neq_mask = torch.zeros(G, T, dtype=torch.int32, device=device)
             self.winner_slot = torch.zeros(G, T, dtype=torch.int32, device=device)
             self.winner_member = torch.zeros(G, T, dtype=torch.int32, device=device)
-        # DETOX: the rule runs on the G rows the vote's winner_slot table names, inside the kernels that read the slab anyway
-        if self.rule in ("detox_median", "detox_trimmed_mean"):
-            self.trim = detox_trim(cfg)
-        elif self.rule == "detox_multi_krum":
-            self.b = cfg.captured_group_bound
-            self.m = G - self.b
-            self.pair_d2 = torch.zeros(T, G * (G - 1) // 2, dtype=torch.float64, device=device)
-            self.select = torch.zeros(self.m, T, dtype=torch.int32, device=device)
-        elif self.rule == "detox_geomedian":
-            self.pair_d2 = torch.zeros(T, G * (G - 1) // 2, dtype=torch.float64, device=device)
-            self.gm_weights = torch.zeros(T, G, dtype=torch.float32, device=device)
-        elif self.rule in ("bulyan", "detox_bulyan"):
-            rows = G if self.rule == "detox_bulyan" else self.P
-            self.f = bulyan_f(cfg)
-            self.theta = rows - 2 * self.f                 # rows selected per tensor; their worker slots go in `select`
+        elif plan.source == "nnm":
+            self.mix = torch.zeros(self.P, T, dtype=torch.int32, device=device)
+        # base rule.  The geometric median of more than GEOMED_FAST_MAXP rows streams over the slab once per Weiszfeld iteration;
+        # every other choice starts from the table of pairwise distances between the rows
+        rows = plan.rows
+        self.gm = K.GeoMedianWorkspace(layout, rows, device) if plan.base == "geomedian" and rows > K.GEOMED_FAST_MAXP else None
+        if self.gm is None and (plan.base in ("krum", "multi_krum", "geomedian", "bulyan") or plan.source == "nnm"):
             self.pair_d2 = torch.zeros(T, rows * (rows - 1) // 2, dtype=torch.float64, device=device)
-            self.select = torch.zeros(self.theta, T, dtype=torch.int32, device=device)
-        elif self.rule.startswith("nnm_"):                # mixing masks; the rule then runs on the mixed rows
-            P, self.f = self.P, cfg.worker_fail
-            self.mix = torch.zeros(P, T, dtype=torch.int32, device=device)
-            self.pair_d2 = torch.zeros(T, P * (P - 1) // 2, dtype=torch.float64, device=device)
-            if self.rule in ("nnm_median", "nnm_trimmed_mean"):
-                self.trim = coordinate_trim(cfg)
-            elif self.rule == "nnm_bulyan":               # select holds the mixed rows Bulyan keeps
-                self.theta = P - 2 * self.f
-                self.select = torch.zeros(self.theta, T, dtype=torch.int32, device=device)
-            else:                                         # a choice over the mixed rows, folded into raw-slot weights
-                if self.rule == "nnm_geomedian":
-                    self.gm_weights = torch.zeros(T, P, dtype=torch.float32, device=device)
-                else:
-                    self.m = 1 if self.rule == "nnm_krum" else P - self.f
-                    self.select = torch.zeros(self.m, T, dtype=torch.int32, device=device)
-                self.w_raw = torch.zeros(T, P, dtype=torch.float32, device=device)
-        elif self.rule == "krum":
-            self.pair_d2 = torch.zeros(T, self.P * (self.P - 1) // 2, dtype=torch.float64, device=device)
-            self.select = torch.zeros(T, dtype=torch.int32, device=device)
-        elif self.rule == "multi_krum":
-            self.m = multi_krum_m(cfg)
-            self.pair_d2 = torch.zeros(T, self.P * (self.P - 1) // 2, dtype=torch.float64, device=device)
-            self.select = torch.zeros(self.m, T, dtype=torch.int32, device=device)
-        elif self.rule in ("median", "trimmed_mean"):
-            self.trim = coordinate_trim(cfg)
-        elif self.rule == "geomedian":
-            if self.P <= K.GEOMED_FAST_MAXP:      # weight-space Weiszfeld: 2 passes over the slab in total
-                self.gm = None
-                self.pair_d2 = torch.zeros(T, self.P * (self.P - 1) // 2, dtype=torch.float64, device=device)
-                self.gm_weights = torch.zeros(T, self.P, dtype=torch.float32, device=device)
-            else:
-                self.gm = K.GeoMedianWorkspace(layout, self.P, device)
-        elif self.rule == "cyclic":
+        if plan.base in ("krum", "multi_krum", "bulyan"):    # the rows each tensor keeps (worker slots, or mixed rows under NNM)
+            kept = plan.theta if plan.base == "bulyan" else plan.m
+            self.select = torch.zeros((T,) if plan.source == "raw" and plan.base == "krum" else (kept, T), dtype=torch.int32,
+                                      device=device)
+        if self.gm is None and plan.base == "geomedian":
+            self.gm_weights = torch.zeros(T, rows, dtype=torch.float32, device=device)
+        if plan.source == "nnm" and plan.base in ("krum", "multi_krum", "geomedian"):
+            self.w_raw = torch.zeros(T, self.P, dtype=torch.float32, device=device)   # the choice, folded into raw-slot weights
+        if plan.base == "cyclic":
             self.code = code
             self.E = torch.zeros(T, self.P, 2, dtype=torch.float64, device=device)
             self.recomb = torch.zeros(T, self.P, 2, dtype=torch.float32, device=device)
@@ -187,119 +174,72 @@ class FusedPS:
         With ``buckets`` (the workers' push buckets, in arrival order) and ``wait_bucket(b)`` the PS is pipelined: bucket
         ``b`` is voted on, applied and broadcast as soon as every worker has pushed it, while the workers are still
         back-propagating / pushing the later buckets; only the last bucket is on the critical path."""
-        K, L = self.K, self.layout
+        K, L, plan = self.K, self.layout, self.plan
         before_update = before_update or (lambda: 0)      # called right before the (last) fused update + broadcast kernel
         common = dict(params=self.params, momentum=self.momentum, exp_avg_sq=self.exp_avg_sq, max_exp_avg_sq=self.max_exp_avg_sq,
                       hp=self.hp, step_ptr=step_ptr,
                       done_counter=self.counters[0:1], first_step=1, grad_out=grad_out, mc_params=mc_params, dst=dst)
+        pipelined = buckets is not None and plan.pipelined
+        # (tile range, tensor range) of every bucket; None: the whole arena
+        ranges = [((t0, t1), (min(idxs), max(idxs) + 1)) for t0, t1, idxs in buckets] if pipelined else [(None, None)]
+        nnm = plan.source == "nnm"
         n = 0
-
-        def attack(tile_range=None, tensor_range=None) -> int:
-            if not self.attack:
-                return 0
-            return K.ps_attack(L, self.grad_in, self.slot_stride, self.P, self.attack, adv_bitmap=self.adv_bitmap,
-                               adv_len=self.adv_len, step_ptr=step_ptr, z=self.attack_z, ws=self.attack_ws,
-                               tile_range=tile_range, tensor_range=tensor_range)
-        if buckets is not None and self.rule in PIPELINED_RULES:
-            for bi, (t0, t1, idxs) in enumerate(buckets):
+        for bi, (tiles, tensors) in enumerate(ranges):
+            last = bi == len(ranges) - 1
+            if pipelined:
                 n += wait_bucket(bi)
-                n += attack((t0, t1), (min(idxs), max(idxs) + 1))
-                fl = flags if bi == len(buckets) - 1 else []
-                if self.rule in ("vote", "detox_median", "detox_trimmed_mean"):
-                    K.vote(L, self.grad_in, self.slot_stride, self.group_table, self.neq_mask, self.winner_slot,
-                           self.winner_member, tile_range=(t0, t1), tensor_range=(min(idxs), max(idxs) + 1)); n += 2
-                    G = self.group_table.shape[0]
-                    if bi == len(buckets) - 1:
-                        n += before_update()
-                    if self.rule == "vote":
-                        K.aggregate_update(L, self.grad_in, self.slot_stride, K=G, scale=1.0 / G, select=self.winner_slot,
-                                           tile_range=(t0, t1), flags=fl, **common); n += 1
-                    else:                                  # DETOX: the coordinate-wise rule across the bucket's group winners
-                        K.aggregate_update(L, self.grad_in, self.slot_stride, K=G, scale=1.0 / (G - 2 * self.trim), trim=self.trim,
-                                           select=self.winner_slot, tile_range=(t0, t1), flags=fl, **common); n += 1
-                elif self.rule == "mean":
-                    if bi == len(buckets) - 1:
-                        n += before_update()
-                    K.aggregate_update(L, self.grad_in, self.slot_stride, K=self.P, scale=1.0 / self.P,
-                                       tile_range=(t0, t1), flags=fl, **common); n += 1
-                else:                                      # coordinate-wise rules: element by element, nothing per tensor
-                    if bi == len(buckets) - 1:
-                        n += before_update()
-                    K.aggregate_update(L, self.grad_in, self.slot_stride, K=self.P, scale=1.0 / (self.P - 2 * self.trim),
-                                       trim=self.trim, tile_range=(t0, t1), flags=fl, **common); n += 1
-            return n
-        common["flags"] = flags
-        n += attack()
-        _agg = K.aggregate_update
-
-        def _update(*a, **kw):                             # every rule below ends in exactly one fused update kernel
-            nonlocal n
-            n += before_update()
-            _agg(*a, **kw)
-        if self.rule == "mean":
-            _update(L, self.grad_in, self.slot_stride, K=self.P, scale=1.0 / self.P, **common); n += 1
-        elif self.rule == "vote":
-            K.vote(L, self.grad_in, self.slot_stride, self.group_table, self.neq_mask, self.winner_slot, self.winner_member); n += 2
-            G = self.group_table.shape[0]
-            _update(L, self.grad_in, self.slot_stride, K=G, scale=1.0 / G, select=self.winner_slot, **common); n += 1
-        elif self.rule.startswith("detox"):
-            K.vote(L, self.grad_in, self.slot_stride, self.group_table, self.neq_mask, self.winner_slot, self.winner_member); n += 2
-            G, win = self.group_table.shape[0], self.winner_slot
-            if self.rule == "detox_multi_krum":          # select holds the worker slots of the m best winners
-                K.krum_select(L, self.grad_in, self.slot_stride, G, self.b, self.pair_d2, self.select, m=self.m, rows=win); n += 2
-                _update(L, self.grad_in, self.slot_stride, K=self.m, scale=1.0 / self.m, select=self.select, **common); n += 1
-            elif self.rule == "detox_geomedian":         # weights in row space, applied through the same winner table
-                K.geometric_median_weights(L, self.grad_in, self.slot_stride, G, self.pair_d2, self.gm_weights, rows=win); n += 2
-                _update(L, self.grad_in, self.slot_stride, K=G, scale=1.0, weights=self.gm_weights, select=win, **common); n += 1
-            elif self.rule == "detox_bulyan":            # select holds the worker slots of the theta winners Bulyan keeps
-                K.bulyan_select(L, self.grad_in, self.slot_stride, G, self.f, self.pair_d2, self.select, rows=win); n += 2
-                _update(L, self.grad_in, self.slot_stride, K=self.theta, scale=1.0 / (self.theta - 2 * self.f), near_median=self.f,
-                        select=self.select, **common); n += 1
-            else:
-                _update(L, self.grad_in, self.slot_stride, K=G, scale=1.0 / (G - 2 * self.trim), trim=self.trim, select=win,
-                        **common); n += 1
-        elif self.rule.startswith("nnm_"):
-            P, f = self.P, self.f
-            coordinate = self.rule in ("nnm_median", "nnm_trimmed_mean")
-            K.nnm_mix(L, self.grad_in, self.slot_stride, P, f, self.pair_d2, self.mix, mixed_out=not coordinate); n += 2
-            if coordinate:
-                _update(L, self.grad_in, self.slot_stride, K=P, scale=1.0 / (P - 2 * self.trim), trim=self.trim, mix=self.mix,
-                        mix_f=f, **common); n += 1
-            elif self.rule == "nnm_bulyan":
-                K.bulyan_select(L, self.grad_in, self.slot_stride, P, f, self.pair_d2, self.select, filled=True); n += 1
-                _update(L, self.grad_in, self.slot_stride, K=self.theta, scale=1.0 / (self.theta - 2 * f), near_median=f,
-                        select=self.select, mix=self.mix, mix_f=f, **common); n += 1
-            else:
-                if self.rule == "nnm_geomedian":
-                    K.geometric_median_weights(L, self.grad_in, self.slot_stride, P, self.pair_d2, self.gm_weights, filled=True)
-                    K.nnm_fold(L, P, f, self.mix, self.w_raw, w_mix=self.gm_weights); n += 2
+            if self.attack:
+                n += K.ps_attack(L, self.grad_in, self.slot_stride, self.P, self.attack, adv_bitmap=self.adv_bitmap,
+                                 adv_len=self.adv_len, step_ptr=step_ptr, z=self.attack_z, ws=self.attack_ws,
+                                 tile_range=tiles, tensor_range=tensors)
+            # row source: `rows` is the table of the worker slots the base rule reads (None: slot i is row i)
+            rows = None
+            if plan.source == "detox":
+                K.vote(L, self.grad_in, self.slot_stride, self.group_table, self.neq_mask, self.winner_slot, self.winner_member,
+                       tile_range=tiles, tensor_range=tensors); n += 2
+                rows = self.winner_slot
+            elif nnm:                                      # the choices below read the mixed rows' distances (filled=True)
+                K.nnm_mix(L, self.grad_in, self.slot_stride, self.P, plan.f, self.pair_d2, self.mix,
+                          mixed_out=plan.base not in ("median", "trimmed_mean")); n += 2
+            # selection, then the arguments of the one fused update
+            src, agg = self.grad_in, dict(K=plan.rows, select=rows)
+            if plan.base in ("mean", "vote"):
+                agg.update(scale=1.0 / plan.rows)
+            elif plan.base == "cyclic":
+                K.cyclic_project(L, self.grad_in, self.slot_stride, self.P, self.f, self.E); n += 1
+                K.cyclic_locate(self.E, self.P, self.cfg.worker_fail, self.recomb, self.healthy, self.flagged); n += 1
+                agg.update(scale=1.0 / self.P, recomb=self.recomb)
+            elif plan.base in ("median", "trimmed_mean"):   # coordinate-wise: element by element, nothing per tensor
+                agg.update(scale=1.0 / (plan.rows - 2 * plan.trim), trim=plan.trim)
+            elif plan.base == "bulyan":                    # select holds the rows Bulyan keeps
+                K.bulyan_select(L, self.grad_in, self.slot_stride, plan.rows, plan.f, self.pair_d2, self.select, rows=rows,
+                                filled=nnm); n += 1 if nnm else 2
+                agg.update(K=plan.theta, scale=1.0 / (plan.theta - 2 * plan.f), near_median=plan.f, select=self.select)
+            elif self.gm is not None:
+                iters = 48
+                K.geometric_median(L, self.grad_in, self.slot_stride, plan.rows, self.gm, iters=iters); n += 2 * iters + 1
+                src = self.gm.median
+                agg.update(K=1, scale=1.0)
+            else:                                          # geometric median weights, or the m best Krum rows
+                if plan.base == "geomedian":
+                    K.geometric_median_weights(L, self.grad_in, self.slot_stride, plan.rows, self.pair_d2, self.gm_weights,
+                                               rows=rows, filled=nnm)
+                    choice = dict(w_mix=self.gm_weights)
+                    agg.update(scale=1.0, weights=self.gm_weights)
                 else:
-                    K.krum_select(L, self.grad_in, self.slot_stride, P, f, self.pair_d2, self.select, m=self.m, filled=True)
-                    K.nnm_fold(L, P, f, self.mix, self.w_raw, select=self.select, m=self.m); n += 2
-                _update(L, self.grad_in, self.slot_stride, K=P, scale=1.0, weights=self.w_raw, **common); n += 1
-        elif self.rule == "krum":
-            K.krum_select(L, self.grad_in, self.slot_stride, self.P, self.cfg.worker_fail, self.pair_d2, self.select); n += 2
-            _update(L, self.grad_in, self.slot_stride, K=1, scale=1.0, select=self.select, **common); n += 1
-        elif self.rule == "multi_krum":
-            K.krum_select(L, self.grad_in, self.slot_stride, self.P, self.cfg.worker_fail, self.pair_d2, self.select, m=self.m); n += 2
-            _update(L, self.grad_in, self.slot_stride, K=self.m, scale=1.0 / self.m, select=self.select, **common); n += 1
-        elif self.rule == "bulyan":
-            K.bulyan_select(L, self.grad_in, self.slot_stride, self.P, self.f, self.pair_d2, self.select); n += 2
-            _update(L, self.grad_in, self.slot_stride, K=self.theta, scale=1.0 / (self.theta - 2 * self.f), near_median=self.f,
-                    select=self.select, **common); n += 1
-        elif self.rule in ("median", "trimmed_mean"):
-            _update(L, self.grad_in, self.slot_stride, K=self.P, scale=1.0 / (self.P - 2 * self.trim), trim=self.trim, **common); n += 1
-        elif self.rule == "geomedian" and self.gm is None:
-            K.geometric_median_weights(L, self.grad_in, self.slot_stride, self.P, self.pair_d2, self.gm_weights); n += 2
-            _update(L, self.grad_in, self.slot_stride, K=self.P, scale=1.0, weights=self.gm_weights, **common); n += 1
-        elif self.rule == "geomedian":
-            iters = 48
-            K.geometric_median(L, self.grad_in, self.slot_stride, self.P, self.gm, iters=iters); n += 2 * iters + 1
-            _update(L, self.gm.median, self.slot_stride, K=1, scale=1.0, **common); n += 1
-        elif self.rule == "cyclic":
-            K.cyclic_project(L, self.grad_in, self.slot_stride, self.P, self.f, self.E); n += 1
-            K.cyclic_locate(self.E, self.P, self.cfg.worker_fail, self.recomb, self.healthy, self.flagged); n += 1
-            _update(L, self.grad_in, self.slot_stride, K=self.P, scale=1.0 / self.P, recomb=self.recomb, **common); n += 1
+                    K.krum_select(L, self.grad_in, self.slot_stride, plan.rows, plan.f, self.pair_d2, self.select, m=plan.m,
+                                  rows=rows, filled=nnm)
+                    choice = dict(select=self.select, m=plan.m)
+                    agg.update(K=plan.m, scale=1.0 / plan.m, select=self.select)
+                n += 1 if nnm else 2
+                if nnm:                                    # a choice over the mixed rows, as weights over the raw slots
+                    K.nnm_fold(L, self.P, plan.f, self.mix, self.w_raw, **choice); n += 1
+                    agg = dict(K=self.P, scale=1.0, weights=self.w_raw)
+            if nnm and plan.base in ("median", "trimmed_mean", "bulyan"):
+                agg.update(mix=self.mix, mix_f=plan.f)
+            if last:
+                n += before_update()
+            K.aggregate_update(L, src, self.slot_stride, tile_range=tiles, flags=flags if last else [], **agg, **common); n += 1
         return n
 
 
@@ -315,7 +255,8 @@ class TorchPS:
         self.cfg, self.layout, self.device, self.params = cfg, layout, device, params
         self.P = cfg.num_workers
         self.groups, self.code = groups, code
-        self.rule = select_rule(cfg)
+        self.plan = rule_plan(cfg)
+        self.rule = self.plan.rule
         # flat per-tensor views in arena element order (the optimizer is element-wise, so order is irrelevant)
         views = [params[s.offset: s.offset + s.numel] for s in layout.specs]
         self._views = views
@@ -325,13 +266,10 @@ class TorchPS:
         else:
             self.optimizer = SGDModified(views, lr=cfg.lr, momentum=cfg.momentum, weight_decay=cfg.weight_decay,
                                          dampening=cfg.dampening, nesterov=cfg.nesterov)
-        if self.rule == "cyclic":
+        if self.plan.base == "cyclic":
             g = torch.Generator().manual_seed(cfg.seed + 4242)
             f = (torch.randn(layout.total, generator=g) + 1.0) * torch.from_numpy(layout.valid_mask()).float()
             self.f = f.to(device)
-        self.trim = coordinate_trim(cfg) if self.rule in ("median", "trimmed_mean", "nnm_median", "nnm_trimmed_mean") else 0
-        if self.rule in ("detox_median", "detox_trimmed_mean"):
-            self.trim = detox_trim(cfg)
         self.last_info: Dict[str, object] = {}
 
     # --- optimizer state for checkpoints (the reference saves none: src/master/baseline_master.py:237-243) ----------
@@ -421,7 +359,7 @@ class TorchPS:
         return d2.sort(dim=1).values[:, :keep].sum(1)
 
     def _krum_tensor(self, X: torch.Tensor) -> int:
-        return int(torch.argsort(self._krum_scores(X, self.cfg.worker_fail), stable=True)[0])      # NaN scores last, like the kernel
+        return int(torch.argsort(self._krum_scores(X, self.plan.f), stable=True)[0])      # NaN scores last, like the kernel
 
     def _multi_krum_tensor(self, X: torch.Tensor, s: int, m: int) -> torch.Tensor:
         best = torch.argsort(self._krum_scores(X, s), stable=True)[:m]
@@ -429,7 +367,7 @@ class TorchPS:
 
     def _trimmed_mean_tensor(self, X: torch.Tensor) -> torch.Tensor:
         """Sort every coordinate (NaN sorts last), drop ``trim`` values at each end, sum the rest in ascending order."""
-        P, b = X.shape[0], self.trim
+        P, b = X.shape[0], self.plan.trim
         S = X.sort(0).values
         acc = S[b].clone()
         for k in range(b + 1, P - b):
@@ -497,62 +435,41 @@ class TorchPS:
 
     # --- step -----------------------------------------------------------------------------------
     def aggregate(self, slots: torch.Tensor) -> List[torch.Tensor]:
-        """``slots``: [P, D] fp32 (or [P, D] complex64 for cyclic).  Returns the per-tensor aggregated gradients."""
-        L = self.layout
+        """``slots``: [P, D] fp32 (or [P, D] complex64 for cyclic).  Returns the per-tensor aggregated gradients: per tensor the
+        rows of the row source (the worker slots, the group winners of the vote, or the mixed rows), then the base rule's helper
+        on them."""
+        plan = self.plan
         self.last_info = {}
         out = []
-        for i, spec in enumerate(L.specs):
+        for spec in self.layout.specs:
             X = slots[:, spec.offset: spec.offset + spec.numel]
-            if self.rule == "mean":
-                g = X.sum(0) / self.P
-            elif self.rule == "vote":
-                acc = torch.zeros(spec.numel, dtype=torch.float32, device=X.device)
-                for grp in self.groups.groups:
-                    rows = [X[w - 1] for w in grp]
-                    acc += rows[self._vote_tensor(rows)]
-                g = acc / float(self.groups.num_groups)
-            elif self.rule == "krum":
-                g = X[self._krum_tensor(X)]
-            elif self.rule == "multi_krum":
-                g = self._multi_krum_tensor(X, self.cfg.worker_fail, multi_krum_m(self.cfg))
-            elif self.rule in ("median", "trimmed_mean"):
-                g = self._trimmed_mean_tensor(X)
-            elif self.rule == "geomedian":
-                g = self._geomedian_tensor(X)
-            elif self.rule == "bulyan":
-                g = self._bulyan_tensor(X, self.cfg.worker_fail)
-            elif self.rule.startswith("nnm_"):            # the rule's own helper on the mixed rows
-                f = self.cfg.worker_fail
-                Y = self._nnm_mix_tensor(X, f)
-                if self.rule == "nnm_krum":
-                    g = Y[self._krum_tensor(Y)]
-                elif self.rule == "nnm_multi_krum":
-                    g = self._multi_krum_tensor(Y, f, self.P - f)
-                elif self.rule == "nnm_geomedian":
-                    g = self._geomedian_tensor(Y)
-                elif self.rule == "nnm_bulyan":
-                    g = self._bulyan_tensor(Y, f)
-                else:
-                    g = self._trimmed_mean_tensor(Y)
-            elif self.rule.startswith("detox"):
-                winners = []                               # stage 1: the vote inside every group
+            if plan.source == "detox":                   # the vote inside every group
+                winners = []
                 for grp in self.groups.groups:
                     rows = [X[w - 1] for w in grp]
                     winners.append(rows[self._vote_tensor(rows)])
-                W = torch.stack(winners)                   # stage 2: the rule across the G winners
-                if self.rule == "detox_multi_krum":
-                    b = self.cfg.captured_group_bound
-                    g = self._multi_krum_tensor(W, b, W.shape[0] - b)
-                elif self.rule == "detox_geomedian":
-                    g = self._geomedian_tensor(W)
-                elif self.rule == "detox_bulyan":
-                    g = self._bulyan_tensor(W, self.cfg.captured_group_bound)
-                else:
-                    g = self._trimmed_mean_tensor(W)
-            elif self.rule == "cyclic":
-                g = self._cyclic_tensor(X, self.f[spec.offset: spec.offset + spec.numel])
+                X = torch.stack(winners)
+            elif plan.source == "nnm":
+                X = self._nnm_mix_tensor(X, plan.f)
+            if plan.base == "mean":
+                g = X.sum(0) / plan.rows
+            elif plan.base == "vote":                    # the winners summed in group order, then divided by G
+                g = torch.zeros_like(X[0])
+                for w in X:
+                    g += w
+                g = g / float(plan.rows)
+            elif plan.base == "krum":
+                g = X[self._krum_tensor(X)]
+            elif plan.base == "multi_krum":
+                g = self._multi_krum_tensor(X, plan.f, plan.m)
+            elif plan.base in ("median", "trimmed_mean"):
+                g = self._trimmed_mean_tensor(X)
+            elif plan.base == "geomedian":
+                g = self._geomedian_tensor(X)
+            elif plan.base == "bulyan":
+                g = self._bulyan_tensor(X, plan.f)
             else:
-                raise ValueError(self.rule)
+                g = self._cyclic_tensor(X, self.f[spec.offset: spec.offset + spec.numel])
             out.append(g)
         return out
 
@@ -560,12 +477,7 @@ class TorchPS:
         self.apply(self.aggregate(slots))
 
     def apply(self, grads: List[torch.Tensor]) -> None:
-        mode = {"mean": "normal", "vote": "maj_vote", "krum": "krum", "geomedian": "geometric_median", "cyclic": "cyclic",
-                "median": "coordinate_median", "trimmed_mean": "trimmed_mean", "multi_krum": "multi_krum",
-                "detox_median": "coordinate_median", "detox_trimmed_mean": "trimmed_mean", "detox_multi_krum": "multi_krum",
-                "detox_geomedian": "geometric_median", "bulyan": "bulyan", "detox_bulyan": "bulyan",
-                **{rule: mode for mode, rule in NNM_RULES.items()}}[self.rule]
-        self.optimizer.step(grads=grads, mode=mode)
+        self.optimizer.step(grads=grads, mode=self.plan.opt_mode)
 
 
 def build_codes(cfg: JobConfig):
