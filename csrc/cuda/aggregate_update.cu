@@ -15,7 +15,8 @@ struct UpdateArgs {
   // gradient source ---------------------------------------------------------------------------
   int mode;                       // 0: select-sum over `select` table; 1: cyclic recombination; 2: real per-tensor weights;
                                   // 3: coordinate-wise trimmed mean over K rows (see `trim`);
-                                  // 4: Bulyan's average of the K - 2 trim values nearest the coordinate median of K rows
+                                  // 4: Bulyan's average of the K - 2 trim values nearest the coordinate median of K rows;
+                                  // 5: centered clipping, v + sum_k w[tensor][k] (g_k - v) around the centre `center`
   const float* grad_in;           // mode 0: [P][slot_stride] fp32 ; mode 1: [n][2*slot_stride] complex64
   long long slot_stride;          // elements (fp32 words for mode 0, complex elements for mode 1)
   const int* select;              // modes 0, 2, 3: [K][T] worker slot to read for (k, tensor); null -> rows 0..K-1 for all
@@ -47,6 +48,8 @@ struct UpdateArgs {
   const unsigned int* mix;        // [mixP][T] neighbour masks of nnm_mix (bit j = raw row j is in N_i), or null: no mixing
   int mixP;                       // raw rows P (slots 0..P-1); mode 3 sorts K = P mixed rows, mode 4 the K = theta of `select`
   float mix_scale;                // fp32(1 / n_mix), n_mix = P - f
+  // centered clipping (mode 5; appended) ------------------------------------------------------------------------------------
+  float* center;                  // [D] the centre v, replaced by the aggregate g; weights in `recomb` as float [T][K]
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -221,6 +224,29 @@ __device__ __forceinline__ float4 mixed_robust_f4(const UpdateArgs& a, long long
   return make_float4(out[0], out[1], out[2], out[3]);
 }
 
+// ---------------------------------------------------------------------------------------------
+// Mode 5: centered clipping (clip.cu; codes/oracle.py::centered_clip).  Per coordinate, from acc = +0 and for the rows k in
+// ascending order whose weight w_k = w[tensor][k] (cc_weights_kernel) is not zero: acc = fma_rn(w_k, rn(x_k - v), acc); then
+// g = rn(v + acc), stored back as the next step's centre.  A zero weight (a NaN or +Inf distance) skips the row's load, so
+// such a row never reaches g through 0 * NaN.
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ float4 centered_clip_f4(const UpdateArgs& a, long long idx, int tensor) {
+  const float* wts = reinterpret_cast<const float*>(a.recomb);
+  const float4 v = *reinterpret_cast<const float4*>(a.center + idx);
+  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int k = 0; k < a.K; ++k) {
+    const float w = wts[tensor * a.K + k];
+    if (w == 0.f) continue;
+    const int slot = a.select ? a.select[k * a.tv.ntensors + tensor] : k;
+    const float4 x = ld_f4(reinterpret_cast<const float4*>(a.grad_in + slot * a.slot_stride + idx));
+    acc.x = __fmaf_rn(w, __fsub_rn(x.x, v.x), acc.x); acc.y = __fmaf_rn(w, __fsub_rn(x.y, v.y), acc.y);
+    acc.z = __fmaf_rn(w, __fsub_rn(x.z, v.z), acc.z); acc.w = __fmaf_rn(w, __fsub_rn(x.w, v.w), acc.w);
+  }
+  const float4 g = make_float4(__fadd_rn(v.x, acc.x), __fadd_rn(v.y, acc.y), __fadd_rn(v.z, acc.z), __fadd_rn(v.w, acc.w));
+  *reinterpret_cast<float4*>(a.center + idx) = g;
+  return g;
+}
+
 // SORT_N: modes 3 and 4, the sorting-network size (4, 8 or 16 >= K, or >= mixP with MIX).  Each size is its own instantiation so
 // that a launch pays the registers of its own network (4 x SORT_N keys per thread), not those of the largest one.  SEL: rows come
 // through the `select` table (DETOX's winners, Bulyan's choice); mode 3 without a table is its own instantiation, mode 4 always
@@ -261,6 +287,8 @@ __global__ void __launch_bounds__(DRC_THREADS) aggregate_update_kernel(const __g
       g = mixed_robust_f4<MODE, SORT_N>(a, idx, tensor);
     } else if constexpr (MODE == 3 || MODE == 4) {
       g = raw_robust_f4<MODE, SORT_N, SEL>(a, idx, tensor);
+    } else if constexpr (MODE == 5) {
+      g = centered_clip_f4(a, idx, tensor);
     } else {
       for (int k = 0; k < a.K; ++k) {
         const float2 v = a.recomb[tensor * a.K + k];
@@ -273,7 +301,7 @@ __global__ void __launch_bounds__(DRC_THREADS) aggregate_update_kernel(const __g
         g.w += v.x * c1.z - v.y * c1.w;
       }
     }
-    g.x *= a.scale; g.y *= a.scale; g.z *= a.scale; g.w *= a.scale;
+    if constexpr (MODE != 5) { g.x *= a.scale; g.y *= a.scale; g.z *= a.scale; g.w *= a.scale; }
     if (a.grad_out) *reinterpret_cast<float4*>(a.grad_out + idx) = g;
 
     float4 p = *reinterpret_cast<const float4*>(a.params + idx);
@@ -338,6 +366,12 @@ extern "C" int drc_aggregate_update(const UpdateArgs* args, int grid, cudaStream
   if ((mode == 3 || mode == 4) && (K < 1 || K > TRIM_MAXP || args->trim < 0 || 2 * args->trim >= K))
     return (int)cudaErrorInvalidValue;
   if (mode == 4 && !args->select) return (int)cudaErrorInvalidValue;
+  // centered clipping: K <= TRIM_MAXP rows (through `select` or slots 0..K-1), their weights and the centre
+  if (mode == 5) {
+    if (K < 1 || K > TRIM_MAXP || !args->recomb || !args->center || args->mix) return (int)cudaErrorInvalidValue;
+    aggregate_update_kernel<5><<<grid, DRC_THREADS, 0, stream>>>(*args);
+    return (int)cudaGetLastError();
+  }
   // nearest-neighbour mixing: modes 3 (K = mixP mixed rows, no row table) and 4 (K = theta mixed rows named by `select`)
   if (args->mix) {
     if (args->mixP < 1 || args->mixP > TRIM_MAXP || !(args->mix_scale > 0.f)) return (int)cudaErrorInvalidValue;

@@ -77,7 +77,7 @@ class UpdateArgs(C.Structure):
                 ("exp_avg_sq", ptr), ("max_exp_avg_sq", ptr), ("hp", ptr), ("step_ptr", ptr), ("first_step", u64), ("grad_out", ptr), ("mc_params", ptr),
                 ("dst", ptr * MAX_DST), ("ndst", C.c_int), ("done_counter", ptr), ("flags", FlagList),
                 ("tile_begin", C.c_int), ("tile_end", C.c_int), ("trim", C.c_int),
-                ("mix", ptr), ("mixP", C.c_int), ("mix_scale", C.c_float)]
+                ("mix", ptr), ("mixP", C.c_int), ("mix_scale", C.c_float), ("center", ptr)]
 
 
 class StreamPushArgs(C.Structure):
@@ -149,6 +149,12 @@ class AttackArgs(C.Structure):
                 ("adv_bitmap", ptr), ("adv_len", C.c_int), ("step_ptr", ptr), ("z", C.c_double), ("stats", ptr),
                 ("partials", ptr), ("gamma", ptr), ("tile_begin", C.c_int), ("tile_end", C.c_int), ("t_begin", C.c_int),
                 ("t_end", C.c_int)]
+
+
+class CcArgs(C.Structure):
+    _fields_ = [("grad_in", ptr), ("slot_stride", i64), ("n", C.c_int), ("rows", ptr), ("tv", TileView), ("center", ptr),
+                ("partials", ptr), ("weights", ptr), ("tau", C.c_double), ("tile_begin", C.c_int), ("tile_end", C.c_int),
+                ("t_begin", C.c_int), ("t_end", C.c_int)]
 
 
 def _maybe_build() -> None:
@@ -228,6 +234,8 @@ def cuda() -> C.CDLL:
             "drc_attack_stats": [C.POINTER(AttackArgs), C.c_int, st],
             "drc_attack_solve": [C.POINTER(AttackArgs), st],
             "drc_attack_write": [C.POINTER(AttackArgs), C.c_int, st],
+            "drc_cc_dist": [C.POINTER(CcArgs), C.c_int, st],
+            "drc_cc_weights": [C.POINTER(CcArgs), st],
             "drc_gemm_bf16": [ptr, i64, C.c_int, ptr, i64, C.c_int, ptr, i64, C.c_int, C.c_int, C.c_int, C.c_int, ptr, ptr,
                               C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, st],
             "drc_rt_init": [C.c_int],

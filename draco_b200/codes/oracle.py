@@ -6,9 +6,11 @@ They define the semantics the CUDA kernels (csrc/cuda/*.cu) and the C++ host twi
 src/master/baseline_master.py:271-296).
 
 ``worker_momentum`` is the one worker-side rule here, and it is fp32 on purpose: every path must produce its exact bits.
+``centered_clip`` is fp64 where it measures (the distances, the weights) and fp32 where it combines rows, for the same reason.
 """
 from __future__ import annotations
 
+import math
 from typing import List, Sequence, Tuple
 
 import numpy as np
@@ -379,3 +381,58 @@ def worker_momentum(m: np.ndarray, g: np.ndarray, beta: float) -> np.ndarray:
     bm = np.multiply(np.float32(b), m32, dtype=np.float32)
     cg = np.multiply(np.float32(c), g32, dtype=np.float32)
     return np.add(bm, cg, dtype=np.float32)
+
+
+def fma_f32(a, b, c) -> np.ndarray:
+    """fp32 fused multiply-add, rn(a * b + c) with one rounding, element-wise.  The product of two fp32 values is exact in fp64;
+    the sum is formed exactly as s + err (TwoSum), rounded to odd in fp64, then rounded once to fp32 (53 >= 24 + 2 bits makes
+    the second rounding exact).  Non-finite sums are rounded as they are."""
+    a64 = np.asarray(a, dtype=np.float32).astype(np.float64)
+    b64 = np.asarray(b, dtype=np.float32).astype(np.float64)
+    c64 = np.asarray(c, dtype=np.float32).astype(np.float64)
+    p = a64 * b64
+    with np.errstate(invalid="ignore", over="ignore"):
+        s = p + c64
+        bb = s - p
+        err = (p - (s - bb)) + (c64 - bb)
+    s, err = np.broadcast_to(s, np.broadcast(s, err).shape).copy(), np.broadcast_to(err, s.shape)
+    odd = np.isfinite(s) & (err != 0) & ((s.view(np.int64) & 1) == 0)
+    s[odd] = np.nextafter(s[odd], np.where(err[odd] > 0, np.inf, -np.inf))
+    return s.astype(np.float32)
+
+
+def centered_clip_weights(rows: np.ndarray, center: np.ndarray, tau: float) -> np.ndarray:
+    """The fp32 weights of one centered-clipping step over one tensor: d_i = sum_e ((double)x_ie - (double)v_e)^2 in fp64,
+    w_i = fp32(min(1, tau / sqrt(d_i)) / n) formed in fp64 and rounded once; d_i = 0 gives fp32(1 / n), and a NaN or +Inf d_i
+    gives 0 (the row is then never read)."""
+    X = np.asarray(rows, dtype=np.float32).astype(np.float64)
+    v = np.asarray(center, dtype=np.float32).astype(np.float64)
+    n = X.shape[0]
+    with np.errstate(invalid="ignore", over="ignore"):
+        d = ((X - v[None, :]) ** 2).sum(axis=1)
+    return np.array([centered_clip_weight(float(di), tau, n) for di in d], dtype=np.float32)
+
+
+def centered_clip_weight(d: float, tau: float, n: int) -> float:
+    """One row's fp32 weight from its fp64 squared distance ``d`` to the centre (see ``centered_clip_weights``)."""
+    if not d < math.inf:
+        return 0.0
+    return float(np.float32(1.0 / n)) if d == 0.0 else float(np.float32(min(1.0, tau / math.sqrt(d)) / n))
+
+
+def centered_clip(rows: np.ndarray, center: np.ndarray, tau: float, weights=None) -> np.ndarray:
+    """Centered clipping (Karimireddy, He and Jaggi, ICML 2021), one iteration on one tensor:
+    g = v + (1/n) sum_i (x_i - v) min(1, tau / ||x_i - v||), with the n fp32 rows x_i and the fp32 centre v (the previous
+    aggregate of this tensor, +0 at the start).  The weights come from ``centered_clip_weights`` (or ``weights``); then per
+    coordinate acc = +0, acc = fma_rn(w_i, rn(x_i - v), acc) for i ascending with w_i != 0, and g = rn(v + acc), all fp32 with
+    no other contraction.  g is both the aggregated gradient and the next centre.  The norm and tau are per tensor, where the
+    paper clips the whole model's vector."""
+    X = np.asarray(rows, dtype=np.float32)
+    v = np.asarray(center, dtype=np.float32)
+    w = centered_clip_weights(X, v, tau) if weights is None else np.asarray(weights, dtype=np.float32)
+    acc = np.zeros_like(v)
+    with np.errstate(invalid="ignore", over="ignore"):
+        for i in range(X.shape[0]):
+            if w[i] != 0:
+                acc = fma_f32(w[i], np.subtract(X[i], v, dtype=np.float32), acc)
+        return np.add(v, acc, dtype=np.float32)

@@ -7,12 +7,14 @@ logging, ``--no-cuda`` forces the CPU/Gloo path) -- see DESIGN.md "flag semantic
 from __future__ import annotations
 
 import argparse
+import math
 from dataclasses import asdict, dataclass
 from typing import Optional
 
 APPROACHES = ("baseline", "maj_vote", "cyclic", "detox", "nnm")
-MODES = ("normal", "geometric_median", "krum", "maj_vote", "coordinate_median", "trimmed_mean", "multi_krum", "bulyan")
-DETOX_MODES = ("coordinate_median", "trimmed_mean", "multi_krum", "geometric_median", "bulyan")
+MODES = ("normal", "geometric_median", "krum", "maj_vote", "coordinate_median", "trimmed_mean", "multi_krum", "bulyan",
+         "centered_clip")
+DETOX_MODES = ("coordinate_median", "trimmed_mean", "multi_krum", "geometric_median", "bulyan", "centered_clip")
 NNM_MODES = ("coordinate_median", "trimmed_mean", "krum", "multi_krum", "geometric_median", "bulyan")
 ROBUST_MAXP = 16                    # workers the fused coordinate-wise / Krum / Bulyan kernels take (TRIM_MAXP, KRUM_MAXP)
 ERR_MODES = ("rev_grad", "constant", "random", "omniscient", "alie", "minmax", "none")
@@ -81,6 +83,7 @@ class JobConfig:
     zero_copy_grads: bool = True    # push reads gradients where autograd left them (pointer table), no flat gather
     attack_z: Optional[float] = None  # --err-mode alie: z of mu - z * sigma (None: Baruch et al.'s z_max for P and f)
     worker_momentum: float = 0.0    # beta of worker-side momentum: every worker pushes m <- beta m + (1 - beta) g (0: off)
+    clip_tau: Optional[float] = None  # --mode centered_clip: the clipping radius tau, per tensor, in the gradient's units
 
     # ---- derived --------------------------------------------------------------------------
     def resolve(self, world_size: int) -> "JobConfig":
@@ -123,6 +126,7 @@ class JobConfig:
             raise ValueError("--transport nccl_flat is the uncompressed library comparator: pass --compress-grad None")
         self._check_ps_attack()
         self._check_worker_momentum()
+        self._check_centered_clip()
         if self.transport == "gloo":
             self.dtype = "fp32"
             self.cuda_graphs = False
@@ -169,6 +173,33 @@ class JobConfig:
         if self.err_mode == "omniscient":
             raise ValueError("--err-mode omniscient replaces the liars' push with a row read from the PS, so their momentum "
                              "could never advance: pick another --err-mode for --worker-momentum")
+
+    def _check_centered_clip(self) -> None:
+        """--mode centered_clip --clip-tau tau: the PS clips every row's distance to last step's aggregate at tau, per tensor."""
+        cc = self.mode == "centered_clip"
+        if self.clip_tau is not None and not (cc and self.approach in ("baseline", "detox")):
+            raise ValueError(f"--clip-tau sets centered clipping's radius: it needs --approach baseline | detox with --mode "
+                             f"centered_clip (got --approach {self.approach} --mode {self.mode})")
+        if not cc:
+            return
+        if self.approach not in ("baseline", "detox"):
+            raise ValueError(f"--mode centered_clip runs under --approach baseline (over the workers) or detox (over the group "
+                             f"winners), got --approach {self.approach}")
+        if self.clip_tau is None or not (math.isfinite(self.clip_tau) and self.clip_tau > 0):
+            raise ValueError(f"--mode centered_clip needs --clip-tau, a finite radius > 0 (got {self.clip_tau}): tau is in the "
+                             f"gradient's own units, per tensor, so no default would mean anything")
+        detox = self.approach == "detox"
+        n, f = (self.num_groups, self.captured_group_bound) if detox else (self.num_workers, self.worker_fail)
+        what = f"{n} groups, b_G = {f}" if detox else f"{n} workers, worker_fail {f}"
+        if 2 * f >= n:
+            raise ValueError(f"--mode centered_clip averages every row around the centre: it needs the honest rows to be a strict "
+                             f"majority, {'groups > 2*b_G' if detox else 'num_workers > 2*worker_fail'} (got {what})")
+        if self.transport == "nvl" and n > ROBUST_MAXP:
+            raise ValueError(f"--mode centered_clip on the nvl transport handles at most {ROBUST_MAXP} rows (got {n}); use "
+                             f"{'a larger --group-size or ' if detox else ''}--transport nccl for more")
+        if self.transport == "nccl_flat":
+            raise ValueError("--transport nccl_flat runs the plain mean and the vote only; use --transport nccl for "
+                             "--mode centered_clip")
 
     @property
     def alie_z(self) -> float:
@@ -290,7 +321,9 @@ def add_fit_args(parser: argparse.ArgumentParser) -> argparse.ArgumentParser:
            "winners) with the lowest Krum scores; bulyan picks num_workers - 2 worker_fail workers by repeated Krum, then "
            "averages, per coordinate, the num_workers - 4 worker_fail picked values nearest their median (needs num_workers >= "
            "4 worker_fail + 3; detox: G and b_G); coordinate_median | trimmed_mean | krum | multi_krum | geometric_median | "
-           "bulyan (nnm: the rule applied to the mixed rows, with --worker-fail as f)")
+           "bulyan (nnm: the rule applied to the mixed rows, with --worker-fail as f).  centered_clip (baseline, detox; needs "
+           "--clip-tau): one step of centered clipping around last step's aggregate v, g = v + (1/n) sum_i (x_i - v) min(1, "
+           "tau / ||x_i - v||) per tensor, and g becomes the next v")
     a("--dataset", type=str, default=d.dataset)
     a("--comm-type", type=str, default=d.comm_type)
     a("--err-mode", type=str, default=d.err_mode,
@@ -303,6 +336,9 @@ def add_fit_args(parser: argparse.ArgumentParser) -> argparse.ArgumentParser:
            "gradient, which shrinks the honest workers' spread before the robust rule sees it (Karimireddy et al. 2021, El "
            "Mhamdi et al. 2021).  --momentum still applies at the PS on top; the papers' recipe is --worker-momentum 0.9 "
            "--momentum 0")
+    a("--clip-tau", type=float, default=None,
+      help="--mode centered_clip: the clipping radius tau, per tensor, in the gradient's own units (required; the papers' "
+           "recipe pairs it with --worker-momentum 0.9 --momentum 0)")
     a("--approach", type=str, default=d.approach,
       help="baseline | maj_vote | cyclic | detox (majority vote inside each repetition group, then --mode across the G group "
            "winners) | nnm (nearest-neighbour mixing: every worker's row is replaced, per tensor, by the mean of its "

@@ -7,6 +7,7 @@ library is missing the call raises (see ``_native.cuda``).
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 from typing import Optional, Sequence, Union
 
@@ -256,6 +257,16 @@ def aggregate_update(layout: ArenaLayout, grad_in: Addr, slot_stride: int, *, pa
         if near_median is not None and K > P:
             raise ValueError(f"mixing: Bulyan's stage takes at most P = {P} mixed rows (K = {K})")
         a.mix, a.mixP, a.mix_scale = mix.data_ptr(), P, 1.0 / (P - mix_f)
+    _launch_update(a, layout, grad_in, slot_stride, select=select, K=K, scale=scale, recomb=recomb, params=params,
+                   momentum=momentum, exp_avg_sq=exp_avg_sq, max_exp_avg_sq=max_exp_avg_sq, hp=hp, step_ptr=step_ptr,
+                   first_step=first_step, grad_out=grad_out, mc_params=mc_params, dst=dst, done_counter=done_counter, flags=flags,
+                   tile_range=tile_range, grid=grid)
+
+
+def _launch_update(a: N.UpdateArgs, layout: ArenaLayout, grad_in: Addr, slot_stride: int, *, select, K, scale, recomb, params,
+                   momentum, exp_avg_sq, max_exp_avg_sq, hp, step_ptr, first_step, grad_out, mc_params, dst, done_counter, flags,
+                   tile_range, grid) -> None:
+    """Fill the fields every mode of ``UpdateArgs`` shares and launch the fused update (``a`` holds the mode's own fields)."""
     a.grad_in = addr(grad_in)
     a.slot_stride = slot_stride
     a.select = addr(select)
@@ -284,6 +295,84 @@ def aggregate_update(layout: ArenaLayout, grad_in: Addr, slot_stride: int, *, pa
         a.tile_begin, a.tile_end = int(tile_range[0]), int(tile_range[1])
         ntiles = a.tile_end - a.tile_begin
     N.check(N.cuda().drc_aggregate_update(C.byref(a), grid or max(1, min(ntiles, sm_count() * 8)), _stream()), "aggregate_update")
+
+
+# ------------------------------------------------------------------------------------------------ centered clipping (C13)
+CC_MAXROWS = 16
+
+
+def _check_buffer(what: str, t, dtype: torch.dtype, shape: tuple) -> None:
+    if (not isinstance(t, torch.Tensor) or t.dtype != dtype or not t.is_cuda or not t.is_contiguous()
+            or tuple(t.shape) != tuple(shape)):
+        got = (tuple(t.shape), t.dtype) if isinstance(t, torch.Tensor) else type(t).__name__
+        raise ValueError(f"{what}: expected a contiguous {dtype} CUDA tensor of shape {tuple(shape)}, got {got}")
+
+
+def _check_cc_rows(what: str, n: int) -> None:
+    if not 1 <= n <= CC_MAXROWS:
+        raise ValueError(f"{what}: takes 1..{CC_MAXROWS} rows, got {n}")
+
+
+def centered_clip_dist(layout: ArenaLayout, grad_in: Addr, slot_stride: int, n: int, center: torch.Tensor,
+                       partials: torch.Tensor, *, rows: Optional[torch.Tensor] = None, tile_range: Optional[tuple] = None,
+                       grid: Optional[int] = None) -> None:
+    """Centered clipping's distances (csrc/cuda/clip.cu): for every tile of ``tile_range`` (one bucket; None: the arena) and
+    each of the ``n`` rows, the fp64 sum of ((double)x - (double)v)^2 over the tile's real elements into ``partials``
+    [ntiles, n] fp64.  ``center``: the fp32 arena v.  ``rows``: optional int32 [n, T] table, row i of tensor t is worker slot
+    ``rows[i, t]`` (DETOX: the vote's winner_slot); slot i without one."""
+    _check_cc_rows("centered_clip_dist", n)
+    if rows is not None:
+        _check_row_table(layout, rows, n)
+    _check_buffer("centered_clip_dist: center", center, torch.float32, (layout.total,))
+    _check_buffer("centered_clip_dist: partials", partials, torch.float64, (layout.ntiles, n))
+    a = N.CcArgs()
+    a.grad_in, a.slot_stride, a.n, a.rows = addr(grad_in), slot_stride, n, addr(rows)
+    a.tv = layout.tile_view(center.device)
+    a.center, a.partials = center.data_ptr(), partials.data_ptr()
+    ntiles = layout.ntiles
+    if tile_range is not None:
+        a.tile_begin, a.tile_end = int(tile_range[0]), int(tile_range[1])
+        ntiles = a.tile_end - a.tile_begin
+    N.check(N.cuda().drc_cc_dist(C.byref(a), grid or max(1, min(ntiles, sm_count() * 8)), _stream()), "cc_dist")
+
+
+def centered_clip_weights(layout: ArenaLayout, n: int, tau: float, partials: torch.Tensor, weights: torch.Tensor, *,
+                          tensor_range: Optional[tuple] = None) -> None:
+    """Fold ``centered_clip_dist``'s partials per tensor in tile order into d_i and write ``weights`` [T, n] fp32:
+    fp32(min(1, tau / sqrt(d_i)) / n), fp32(1 / n) for d_i = 0 and 0 for a NaN or +Inf d_i (codes/oracle.py
+    ``centered_clip_weights``).  ``tensor_range``: the tensors of one bucket (None: every tensor)."""
+    _check_cc_rows("centered_clip_weights", n)
+    if not (math.isfinite(tau) and tau > 0):
+        raise ValueError(f"centered_clip_weights: tau must be finite and > 0, got {tau}")
+    _check_buffer("centered_clip_weights: partials", partials, torch.float64, (layout.ntiles, n))
+    _check_buffer("centered_clip_weights: weights", weights, torch.float32, (layout.ntensors, n))
+    a = N.CcArgs()
+    a.n, a.tv = n, layout.tile_view(weights.device)
+    a.partials, a.weights, a.tau = partials.data_ptr(), weights.data_ptr(), float(tau)
+    if tensor_range is not None:
+        a.t_begin, a.t_end = int(tensor_range[0]), int(tensor_range[1])
+    N.check(N.cuda().drc_cc_weights(C.byref(a), _stream()), "cc_weights")
+
+
+def centered_clip_update(layout: ArenaLayout, grad_in: Addr, slot_stride: int, *, center: torch.Tensor, weights: torch.Tensor,
+                         K: int, params: Addr, momentum: Addr, hp: Addr, step_ptr: Addr, done_counter: Addr,
+                         select: Optional[torch.Tensor] = None, first_step: int = 1, grad_out: Addr = None,
+                         mc_params: Addr = None, dst: Sequence[Addr] = (), flags: Sequence[Addr] = (), grid: Optional[int] = None,
+                         tile_range: Optional[tuple] = None, exp_avg_sq: Addr = None, max_exp_avg_sq: Addr = None) -> None:
+    """The fused update in mode 5 (csrc/cuda/aggregate_update.cu): g = v + sum_k w[t, k] (x_k - v) in fp32 over the K rows with
+    a non-zero weight, stored back into ``center`` as the next step's v, then the optimizer step, broadcast and flags of
+    ``aggregate_update``.  ``weights``: centered_clip_weights's fp32 [T, K]; ``select``: optional int32 [K, T] row table."""
+    _check_cc_rows("centered_clip_update", K)
+    if select is not None:
+        _check_row_table(layout, select, K)
+    _check_buffer("centered_clip_update: center", center, torch.float32, (layout.total,))
+    _check_buffer("centered_clip_update: weights", weights, torch.float32, (layout.ntensors, K))
+    a = N.UpdateArgs()
+    a.mode, a.center = 5, center.data_ptr()
+    _launch_update(a, layout, grad_in, slot_stride, select=select, K=K, scale=1.0, recomb=weights, params=params,
+                   momentum=momentum, exp_avg_sq=exp_avg_sq, max_exp_avg_sq=max_exp_avg_sq, hp=hp, step_ptr=step_ptr,
+                   first_step=first_step, grad_out=grad_out, mc_params=mc_params, dst=dst, done_counter=done_counter, flags=flags,
+                   tile_range=tile_range, grid=grid)
 
 
 def stream_push(src: Addr, dst: Addr, nbytes: Addr, nbytes_out: Addr = None, *, step_ptr: Addr, done_counter: Addr, flag: Addr = None,

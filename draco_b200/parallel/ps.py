@@ -11,6 +11,7 @@ src/master/*.py):
 """
 from __future__ import annotations
 
+import math
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Sequence
 
@@ -20,6 +21,7 @@ import torch
 from .. import _native as N
 from ..codes.adversary import ATTACK_ALIE, ATTACK_MINMAX, PS_ATTACKS, attack_code
 from ..codes.cyclic import CyclicCode, search_w
+from ..codes.oracle import centered_clip_weight
 from ..codes.repetition import GroupPlan
 from ..config import JobConfig
 from .arena import ArenaLayout
@@ -31,8 +33,9 @@ def select_rule(cfg: JobConfig) -> str:
     (rep_master.py:118-129); baseline approach -> mean / geometric median / Krum by ``--mode`` (baseline_master.py:118-129), plus
     three rules beyond the reference: coordinate-wise median, coordinate-wise trimmed mean and multi-Krum.  The detox approach
     (beyond the reference too) votes inside every group and runs ``--mode`` across the group winners: ``detox_*`` rules.  Bulyan
-    (``--mode bulyan``) is beyond the reference as well, and so is the nnm approach: nearest-neighbour mixing of the worker rows,
-    then ``--mode`` on the mixed rows (``nnm_*`` rules)."""
+    (``--mode bulyan``) is beyond the reference as well, and so are centered clipping (``--mode centered_clip``, one step around
+    last step's aggregate) and the nnm approach: nearest-neighbour mixing of the worker rows, then ``--mode`` on the mixed rows
+    (``nnm_*`` rules)."""
     if cfg.approach == "cyclic":
         return "cyclic"
     if cfg.approach == "maj_vote":
@@ -42,21 +45,26 @@ def select_rule(cfg: JobConfig) -> str:
     if cfg.approach == "nnm":
         return NNM_RULES[cfg.mode]
     return {"normal": "mean", "geometric_median": "geomedian", "krum": "krum", "coordinate_median": "median",
-            "trimmed_mean": "trimmed_mean", "multi_krum": "multi_krum", "bulyan": "bulyan"}.get(cfg.mode, "mean")
+            "trimmed_mean": "trimmed_mean", "multi_krum": "multi_krum", "bulyan": "bulyan",
+            "centered_clip": "centered_clip"}.get(cfg.mode, "mean")
 
 
 DETOX_RULES = {"coordinate_median": "detox_median", "trimmed_mean": "detox_trimmed_mean", "multi_krum": "detox_multi_krum",
-               "geometric_median": "detox_geomedian", "bulyan": "detox_bulyan"}
+               "geometric_median": "detox_geomedian", "bulyan": "detox_bulyan",
+               "centered_clip": "detox_centered_clip"}
 NNM_RULES = {"coordinate_median": "nnm_median", "trimmed_mean": "nnm_trimmed_mean", "krum": "nnm_krum",
              "multi_krum": "nnm_multi_krum", "geometric_median": "nnm_geomedian", "bulyan": "nnm_bulyan"}
 
 
-# rules the fused PS applies bucket by bucket while the workers still push (nothing in them needs the whole tensor at once)
-PIPELINED_RULES = ("mean", "vote", "median", "trimmed_mean", "detox_median", "detox_trimmed_mean")
+# rules the fused PS applies bucket by bucket while the workers still push (nothing in them reaches beyond the bucket's
+# tensors: buckets hold whole tensors, and centered clipping's centre is known before the step starts)
+PIPELINED_RULES = ("mean", "vote", "median", "trimmed_mean", "detox_median", "detox_trimmed_mean", "centered_clip",
+                   "detox_centered_clip")
 
 # the optimizer's mode string for each base rule (SGDModified / AdamModified.step(mode=))
 _OPT_MODE = {"mean": "normal", "vote": "maj_vote", "cyclic": "cyclic", "median": "coordinate_median", "trimmed_mean": "trimmed_mean",
-             "krum": "krum", "multi_krum": "multi_krum", "geomedian": "geometric_median", "bulyan": "bulyan"}
+             "krum": "krum", "multi_krum": "multi_krum", "geomedian": "geometric_median", "bulyan": "bulyan",
+             "centered_clip": "centered_clip"}
 
 
 @dataclass(frozen=True)
@@ -64,7 +72,7 @@ class RulePlan:
     """A job's aggregation rule as a row source and a base rule, with every parameter worked out once."""
     rule: str           # select_rule's name
     source: str         # raw: the P worker slots | detox: the G group winners of the vote | nnm: the P mixed rows
-    base: str           # mean | vote | cyclic | median | trimmed_mean | krum | multi_krum | geomedian | bulyan
+    base: str           # mean | vote | cyclic | median | trimmed_mean | krum | multi_krum | geomedian | bulyan | centered_clip
     rows: int           # rows the base rule runs on: P, or G over the group winners
     f: int              # rows it tolerates: worker_fail, or b_G over the group winners
     trim: int           # median / trimmed mean: values dropped at each end of a coordinate
@@ -149,6 +157,10 @@ class FusedPS:
                                       device=device)
         if self.gm is None and plan.base == "geomedian":
             self.gm_weights = torch.zeros(T, rows, dtype=torch.float32, device=device)
+        if plan.base == "centered_clip":                  # the centre v (last step's aggregate, +0 at the start) is PS state
+            self.cc_center = layout.new_arena(device)
+            self.cc_partials = torch.zeros(layout.ntiles, rows, dtype=torch.float64, device=device)
+            self.cc_weights = torch.zeros(T, rows, dtype=torch.float32, device=device)
         if plan.source == "nnm" and plan.base in ("krum", "multi_krum", "geomedian"):
             self.w_raw = torch.zeros(T, self.P, dtype=torch.float32, device=device)   # the choice, folded into raw-slot weights
         if plan.base == "cyclic":
@@ -164,8 +176,12 @@ class FusedPS:
 
     @property
     def opt_state(self) -> Dict[str, Optional[torch.Tensor]]:
-        """Optimizer arenas beyond ``momentum`` (Adam second moment, AMSGrad maximum) for checkpoints."""
-        return {"exp_avg_sq": self.exp_avg_sq, "max_exp_avg_sq": self.max_exp_avg_sq}
+        """Optimizer arenas beyond ``momentum`` (Adam second moment, AMSGrad maximum) for checkpoints, and centered clipping's
+        centre (``cc_center``, only under that rule)."""
+        state = {"exp_avg_sq": self.exp_avg_sq, "max_exp_avg_sq": self.max_exp_avg_sq}
+        if self.plan.base == "centered_clip":
+            state["cc_center"] = self.cc_center
+        return state
 
     def enqueue_step(self, step_ptr: torch.Tensor, *, mc_params: Optional[int], dst: Sequence[int], flags: Sequence[int],
                      grad_out: Optional[torch.Tensor] = None, buckets=None, wait_bucket=None, before_update=None) -> int:
@@ -211,6 +227,11 @@ class FusedPS:
                 agg.update(scale=1.0 / self.P, recomb=self.recomb)
             elif plan.base in ("median", "trimmed_mean"):   # coordinate-wise: element by element, nothing per tensor
                 agg.update(scale=1.0 / (plan.rows - 2 * plan.trim), trim=plan.trim)
+            elif plan.base == "centered_clip":             # per tensor, from the n distances to the centre: bucket by bucket
+                K.centered_clip_dist(L, self.grad_in, self.slot_stride, plan.rows, self.cc_center, self.cc_partials, rows=rows,
+                                     tile_range=tiles)
+                K.centered_clip_weights(L, plan.rows, self.cfg.clip_tau, self.cc_partials, self.cc_weights,
+                                        tensor_range=tensors); n += 2
             elif plan.base == "bulyan":                    # select holds the rows Bulyan keeps
                 K.bulyan_select(L, self.grad_in, self.slot_stride, plan.rows, plan.f, self.pair_d2, self.select, rows=rows,
                                 filled=nnm); n += 1 if nnm else 2
@@ -239,7 +260,12 @@ class FusedPS:
                 agg.update(mix=self.mix, mix_f=plan.f)
             if last:
                 n += before_update()
-            K.aggregate_update(L, src, self.slot_stride, tile_range=tiles, flags=flags if last else [], **agg, **common); n += 1
+            if plan.base == "centered_clip":               # the update reads and replaces the centre
+                K.centered_clip_update(L, src, self.slot_stride, center=self.cc_center, weights=self.cc_weights, K=plan.rows,
+                                       select=rows, tile_range=tiles, flags=flags if last else [], **common)
+            else:
+                K.aggregate_update(L, src, self.slot_stride, tile_range=tiles, flags=flags if last else [], **agg, **common)
+            n += 1
         return n
 
 
@@ -266,6 +292,8 @@ class TorchPS:
         else:
             self.optimizer = SGDModified(views, lr=cfg.lr, momentum=cfg.momentum, weight_decay=cfg.weight_decay,
                                          dampening=cfg.dampening, nesterov=cfg.nesterov)
+        # centered clipping's centre: last step's aggregate, +0 at the start (PS state, checkpointed as opt_state["cc_center"])
+        self.cc_center = layout.new_arena(device) if self.plan.base == "centered_clip" else None
         if self.plan.base == "cyclic":
             g = torch.Generator().manual_seed(cfg.seed + 4242)
             f = (torch.randn(layout.total, generator=g) + 1.0) * torch.from_numpy(layout.valid_mask()).float()
@@ -305,12 +333,19 @@ class TorchPS:
 
     @property
     def opt_state(self) -> Dict[str, Optional[torch.Tensor]]:
-        if self.cfg.optimizer != "adam":
-            return {}
-        return {"exp_avg_sq": self._gather("exp_avg_sq"), "max_exp_avg_sq": self._gather("max_exp_avg_sq")}
+        state = {} if self.cfg.optimizer != "adam" else {"exp_avg_sq": self._gather("exp_avg_sq"),
+                                                          "max_exp_avg_sq": self._gather("max_exp_avg_sq")}
+        if self.cc_center is not None:
+            state["cc_center"] = self.cc_center.clone()
+        return state
 
     def load_opt_state(self, arenas: Dict[str, torch.Tensor], step: int) -> None:
-        """Adam: second moment (+ AMSGrad maximum) and the per-tensor step count (= updates applied so far)."""
+        """Adam: second moment (+ AMSGrad maximum) and the per-tensor step count (= updates applied so far).  Centered
+        clipping: the centre."""
+        arenas = dict(arenas)
+        center = arenas.pop("cc_center", None)
+        if self.cc_center is not None and center is not None:
+            self.cc_center.copy_(center)
         if self.cfg.optimizer != "adam":
             return
         for v, spec in zip(self._views, self.layout.specs):
@@ -422,6 +457,21 @@ class TorchPS:
             Y[i] = y * scale
         return Y
 
+    def _centered_clip_tensor(self, X: torch.Tensor, v: torch.Tensor) -> torch.Tensor:
+        """Centered clipping (``oracle.centered_clip``) around the centre ``v``, which it replaces: fp64 distances, fp32 weights
+        from ``centered_clip_weight``, then per coordinate acc = fma_rn(w_i, rn(x_i - v), acc) over the rows with w_i != 0 in
+        ascending order, and g = rn(v + acc) -- the fused kernel's fp32 order."""
+        n = X.shape[0]
+        d = (X.double() - v.double()).pow(2).sum(1).tolist()
+        acc = torch.zeros_like(v)
+        for i, di in enumerate(d):
+            w = centered_clip_weight(di, self.cfg.clip_tau, n)
+            if w != 0.0:
+                acc = _fma_f32(w, X[i] - v, acc)
+        g = v + acc
+        v.copy_(g)
+        return g
+
     def _cyclic_tensor(self, R: torch.Tensor, f: torch.Tensor) -> torch.Tensor:
         """R: [n, d] complex64 -> Re(v^T R) / n with v from the C++ locator (N1 replacement)."""
         n, s = self.P, self.cfg.worker_fail
@@ -468,6 +518,8 @@ class TorchPS:
                 g = self._geomedian_tensor(X)
             elif plan.base == "bulyan":
                 g = self._bulyan_tensor(X, plan.f)
+            elif plan.base == "centered_clip":
+                g = self._centered_clip_tensor(X, self.cc_center[spec.offset: spec.offset + spec.numel])
             else:
                 g = self._cyclic_tensor(X, self.f[spec.offset: spec.offset + spec.numel])
             out.append(g)
@@ -478,6 +530,19 @@ class TorchPS:
 
     def apply(self, grads: List[torch.Tensor]) -> None:
         self.optimizer.step(grads=grads, mode=self.plan.opt_mode)
+
+
+def _fma_f32(w: float, b: torch.Tensor, c: torch.Tensor) -> torch.Tensor:
+    """fp32 rn(w * b + c) with one rounding, element-wise (``oracle.fma_f32``): the fp64 product is exact, the sum is rounded to
+    odd in fp64 (TwoSum), then once to fp32."""
+    p = b.double() * float(w)
+    c64 = c.double()
+    s = p + c64
+    bb = s - p
+    err = (p - (s - bb)) + (c64 - bb)
+    odd = torch.isfinite(s) & (err != 0) & ((s.view(torch.int64) & 1) == 0)
+    s = torch.where(odd, torch.nextafter(s, torch.where(err > 0, torch.full_like(s, math.inf), torch.full_like(s, -math.inf))), s)
+    return s.float()
 
 
 def build_codes(cfg: JobConfig):

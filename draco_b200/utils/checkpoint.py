@@ -9,7 +9,9 @@ Here one file per checkpoint, same naming (``<train_dir>model_step_<N>``), conta
 the momentum buffers, the step, the BatchNorm statistics of the evaluating worker (the PS never runs a forward pass, so
 its own BN statistics would be meaningless -- the reason the reference refuses to save ResNets on the PS) and the job
 config.  Resume works for every approach and restores optimizer state.  With ``--worker-momentum`` the blob also holds
-every logical worker's momentum (``"worker_momentum": {w: {tensor name: fp32 tensor}}``); the key is absent otherwise.
+every logical worker's momentum (``"worker_momentum": {w: {tensor name: fp32 tensor}}``); the key is absent otherwise.  Under
+``--mode centered_clip`` the PS's centre travels with the optimizer arenas as ``opt_state["cc_center"]``; other jobs have no
+such entry.
 """
 from __future__ import annotations
 
@@ -68,6 +70,17 @@ def check_worker_momentum(blob: dict, beta: float) -> None:
     if beta == 0 and has:
         raise ValueError("the checkpoint holds worker momentum (it was written with --worker-momentum): resume it with the same "
                          "--worker-momentum, or the workers' state would be dropped")
+
+
+def check_cc_center(blob: dict, centered_clip: bool) -> None:
+    """A job resumes only from a checkpoint of the same kind: with centered clipping's centre iff the job clips."""
+    has = "cc_center" in (blob.get("opt_state") or {})
+    if centered_clip and not has:
+        raise ValueError("--mode centered_clip: the checkpoint holds no centre (it was written by a job with another rule), so "
+                         "the clipping would restart around zero")
+    if not centered_clip and has:
+        raise ValueError("the checkpoint holds centered clipping's centre (it was written with --mode centered_clip): resume it "
+                         "with the same --mode, or the centre would be dropped")
 
 
 def restore_worker_momentum(blob: dict, layout: ArenaLayout, arenas: Dict[int, torch.Tensor]) -> None:

@@ -25,8 +25,15 @@ the mixed rows as raw-slot weights) alone; the update kernel's mode 3 (coordinat
 stage) with mixing against the same modes without it, over the same rows; and the whole chains the PS runs after the last
 bucket -- NNM + multi-Krum and NNM + Bulyan against plain multi-Krum and plain Bulyan.
 
+With --cc-workers it times centered clipping over P rows on the same arena: ``centered_clip_dist`` (the fp64 per-tile partials
+of the P row-to-centre distances, csrc/cuda/clip.cu), ``centered_clip_weights`` (the per-tensor fold and the weights), the update
+kernel's mode 5 and the whole chain, against mode 0 (the mean) over the same rows.  ``bytes`` counts the HBM traffic the algorithm
+needs: the distances read the P rows and the centre, (P + 1) * D * 4, and write the partials, ntiles * P * 8; the weights read the
+partials and write T * P * 4; mode 5 reads the rows and the centre and writes the centre, (P + 2) * D * 4, and mode 0 reads the
+rows, P * D * 4, both plus the 16 * D bytes of parameter / momentum traffic.
+
     python tools/bench_aggregate.py [--workers 7 16] [--groups 3 5 8] [--attack-workers 7 15] [--bulyan-workers 7 15]
-                                    [--nnm-workers 7 15] [--iters 200] [--rounds 3] [--out FILE]
+                                    [--nnm-workers 7 15] [--cc-workers 7 15] [--iters 200] [--rounds 3] [--out FILE]
 """
 from __future__ import annotations
 
@@ -208,6 +215,51 @@ def nnm_arm(K, L, P, iters, rounds, dev, update) -> list:
              "us_rounds": [round(t, 2) for t in ts]} for name, ts in times.items()]
 
 
+def cc_arm(K, L, P, iters, rounds, dev, update) -> list:
+    """Centered clipping's launches alone and chained, against mode 0 over the same rows (see the module docstring)."""
+    import torch
+    T, D, nt = L.ntensors, L.total, L.ntiles
+    slab = torch.randn(P, D, device=dev) * 1e-3
+    center = torch.zeros(D, device=dev)
+    partials = torch.zeros(nt, P, dtype=torch.float64, device=dev)
+    weights = torch.zeros(T, P, dtype=torch.float32, device=dev)
+    tau = 1e-2                                                          # every row is read: no weight is zero
+    K.centered_clip_dist(L, slab, D, P, center, partials)
+    K.centered_clip_weights(L, P, tau, partials, weights)
+
+    def mode5():
+        update(slab, dict(K=P, center=center, weights=weights), cc=True)
+    arms = {
+        "cc_dist": (lambda: K.centered_clip_dist(L, slab, D, P, center, partials), (P + 1) * D * 4 + nt * P * 8),
+        "cc_weights": (lambda: K.centered_clip_weights(L, P, tau, partials, weights), nt * P * 8 + T * P * 4),
+        "mode5_centered_clip": (mode5, (P + 2) * D * 4 + 16 * D),
+        "cc_chain": (lambda: (K.centered_clip_dist(L, slab, D, P, center, partials),
+                              K.centered_clip_weights(L, P, tau, partials, weights), mode5()),
+                     (2 * P + 3) * D * 4 + 2 * nt * P * 8 + T * P * 4 + 16 * D),
+        "mode0_mean": (lambda: update(slab, dict(K=P, scale=1.0 / P)), P * D * 4 + 16 * D),
+    }
+    for fn, _ in arms.values():
+        for _ in range(20):
+            fn()
+    torch.cuda.synchronize()
+    times = {name: [] for name in arms}
+    for _ in range(rounds):
+        for name, (fn, _) in arms.items():
+            s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            s.record()
+            for _ in range(iters):
+                fn()
+            e.record()
+            e.synchronize()
+            times[name].append(s.elapsed_time(e) * 1e3 / iters)
+    out = []
+    for name, ts in times.items():
+        us, nbytes = sorted(ts)[len(ts) // 2], arms[name][1]
+        out.append({"P": P, "arm": name, "us_per_call": round(us, 2), "us_rounds": [round(t, 2) for t in ts], "bytes": nbytes,
+                    "bytes_per_us": round(nbytes / us), "share_of_3.35TBps": round(nbytes / us / HBM_BYTES_PER_US, 3)})
+    return out
+
+
 def main() -> int:
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--workers", type=int, nargs="*", default=[7, 16])
@@ -218,6 +270,7 @@ def main() -> int:
     ap.add_argument("--attack-fail", type=int, default=3, help="liar slots of the attack arm")
     ap.add_argument("--bulyan-workers", type=int, nargs="*", default=[], help="P of the Bulyan / multi-Krum arm (none: skipped)")
     ap.add_argument("--nnm-workers", type=int, nargs="*", default=[], help="P of the NNM arm (none: skipped)")
+    ap.add_argument("--cc-workers", type=int, nargs="*", default=[], help="P of the centered-clipping arm (none: skipped)")
     ap.add_argument("--iters", type=int, default=200)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--out", type=str, default=None, help="also append the JSON lines to this file")
@@ -288,12 +341,15 @@ def main() -> int:
     for P in a.attack_workers:
         lines += attack_arm(K, L, P, a.attack_fail, a.iters, a.rounds, dev)
 
-    def update(slab, kw):
-        K.aggregate_update(L, slab, D, params=params, momentum=mom, hp=hp, step_ptr=step, done_counter=cnt[0:1], **kw)
+    def update(slab, kw, cc=False):
+        launcher = K.centered_clip_update if cc else K.aggregate_update
+        launcher(L, slab, D, params=params, momentum=mom, hp=hp, step_ptr=step, done_counter=cnt[0:1], **kw)
     for P in a.bulyan_workers:
         lines += bulyan_arm(K, L, P, a.iters, a.rounds, dev, update)
     for P in a.nnm_workers:
         lines += nnm_arm(K, L, P, a.iters, a.rounds, dev, update)
+    for P in a.cc_workers:
+        lines += cc_arm(K, L, P, a.iters, a.rounds, dev, update)
     for ln in lines:
         print(json.dumps(ln), flush=True)
     if a.out:
