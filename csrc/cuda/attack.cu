@@ -35,6 +35,7 @@ struct AttackArgs {
   double* gamma;                          // min-max: [ntensors]
   int tile_begin, tile_end;               // stats / write: tiles (tile_end == 0: to the end of the arena)
   int t_begin, t_end;                     // solve: tensors (t_end == 0: every tensor); buckets hold whole tensors
+  double* fold;                           // model scope: [ntensors][ATTACK_NQ(P)] the partials folded per tensor
 };
 
 __device__ __forceinline__ unsigned int liar_mask(const AttackArgs& a) {
@@ -174,10 +175,37 @@ __global__ void __launch_bounds__(DRC_THREADS) attack_stats_kernel(const __grid_
 __device__ __forceinline__ double max_nan(double x, double y) { return (x != x || x > y) ? x : y; }
 __device__ __forceinline__ double min_nan(double x, double y) { return (x != x || x < y) ? x : y; }
 
-// One CTA per tensor: fold the tensor's per-tile partials in tile order, then
+// gamma from the folded sums s_sum[ATTACK_NQ(P)] (a_i, b_i, c, pair distances) of the honest rows:
 //   Dmax^2 = max_{i<j in H} ||g_i - g_j||^2,  c = ||p||^2,
 //   gamma  = min_{i in H} largest root of  c g^2 + 2 b_i g + (a_i - Dmax^2) = 0   (||mu + g p - g_i||^2 = Dmax^2)
 // Both roots' forms are the same number; the one without cancellation is used (b_i > 0: (Dmax^2 - a_i) / (b_i + sqrt(disc))).
+__device__ __forceinline__ double minmax_solve(const double* s_sum, int P, unsigned int honest) {
+  double D2 = 0.0;
+  for (int j = 1; j < P; ++j)
+    for (int i = 0; i < j; ++i)
+      if (((honest >> i) & 1u) && ((honest >> j) & 1u)) D2 = max_nan(s_sum[2 * P + 1 + j * (j - 1) / 2 + i], D2);
+  const double c = s_sum[2 * P];
+  double gamma;
+  if (c == 0.0) {
+    gamma = 0.0;                                               // every honest row equal: the liars send them too
+  } else {
+    gamma = INFINITY;
+    for (int i = 0; i < P; ++i) {
+      if (!((honest >> i) & 1u)) continue;
+      const double ai = s_sum[i], bi = s_sum[P + i];
+      double disc = bi * bi + c * (D2 - ai);
+      if (disc < 0.0) disc = 0.0;                              // a_i <= Dmax^2 up to rounding
+      const double r = sqrt(disc);
+      double g = bi <= 0.0 ? (r - bi) / c : (D2 - ai) / (bi + r);
+      if (g < 0.0) g = 0.0;
+      gamma = min_nan(g, gamma);                               // a NaN in Dmax^2, a_i or b_i reaches gamma through disc
+    }
+  }
+  return gamma;
+}
+
+// One CTA per tensor: fold the tensor's per-tile partials in tile order, then solve as minmax_solve does (the kernel keeps its
+// own copy of the solve so that its machine code stays what it was)
 __global__ void __launch_bounds__(DRC_THREADS) attack_solve_kernel(const __grid_constant__ AttackArgs a) {
   __shared__ double s_sum[ATTACK_MAXQ];
   const unsigned int liars = liar_mask(a);
@@ -216,6 +244,42 @@ __global__ void __launch_bounds__(DRC_THREADS) attack_solve_kernel(const __grid_
     }
   }
   a.gamma[tensor] = gamma;
+}
+
+// Model scope (--attack-scope model): one gamma and one Dmax over the whole model.  attack_fold_kernel folds each tensor's
+// partials in tile order as attack_solve_kernel does (one CTA per tensor) into fold[T][Q]; attack_solve_model_kernel (one CTA)
+// sums every entry over the tensors in ascending order, solves once and writes gamma into every tensor.
+__global__ void __launch_bounds__(DRC_THREADS) attack_fold_kernel(const __grid_constant__ AttackArgs a) {
+  const unsigned int liars = liar_mask(a);
+  const unsigned int honest = ~liars & ((1u << a.P) - 1u);
+  if (liars == 0u || honest == 0u) return;
+  const int tensor = blockIdx.x;
+  const TensorMeta m = a.tv.meta[tensor];
+  const int t0 = (int)(m.offset / DRC_TILE), t1 = t0 + (int)((m.numel + DRC_TILE - 1) / DRC_TILE);
+  const int Q = ATTACK_NQ(a.P);
+  for (int q = threadIdx.x; q < Q; q += DRC_THREADS) {
+    double s = 0.0;
+    for (int t = t0; t < t1; ++t) s += a.partials[(long long)t * Q + q];
+    a.fold[(long long)tensor * Q + q] = s;
+  }
+}
+
+__global__ void __launch_bounds__(DRC_THREADS) attack_solve_model_kernel(const __grid_constant__ AttackArgs a) {
+  __shared__ double s_sum[ATTACK_MAXQ];
+  __shared__ double s_gamma;
+  const unsigned int liars = liar_mask(a);
+  const unsigned int honest = ~liars & ((1u << a.P) - 1u);
+  if (liars == 0u || honest == 0u) return;
+  const int T = a.tv.ntensors, Q = ATTACK_NQ(a.P);
+  for (int q = threadIdx.x; q < Q; q += DRC_THREADS) {
+    double s = 0.0;
+    for (int t = 0; t < T; ++t) s += a.fold[(long long)t * Q + q];
+    s_sum[q] = s;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) s_gamma = minmax_solve(s_sum, a.P, honest);
+  __syncthreads();
+  for (int t = threadIdx.x; t < T; t += DRC_THREADS) a.gamma[t] = s_gamma;
 }
 
 __global__ void __launch_bounds__(DRC_THREADS) attack_write_kernel(const __grid_constant__ AttackArgs a) {
@@ -257,6 +321,13 @@ extern "C" int drc_attack_solve(const AttackArgs* args, cudaStream_t stream) {
   const int t_end = args->t_end > 0 ? args->t_end : args->tv.ntensors;
   if (t_end <= args->t_begin) return (int)cudaErrorInvalidValue;
   attack_solve_kernel<<<t_end - args->t_begin, DRC_THREADS, 0, stream>>>(*args);
+  return (int)cudaGetLastError();
+}
+extern "C" int drc_attack_solve_model(const AttackArgs* args, cudaStream_t stream) {
+  if (!attack_args_ok(args) || args->mode != ATTACK_MINMAX || !args->fold || args->tv.ntensors < 1)
+    return (int)cudaErrorInvalidValue;
+  attack_fold_kernel<<<args->tv.ntensors, DRC_THREADS, 0, stream>>>(*args);
+  attack_solve_model_kernel<<<1, DRC_THREADS, 0, stream>>>(*args);
   return (int)cudaGetLastError();
 }
 extern "C" int drc_attack_write(const AttackArgs* args, int grid, cudaStream_t stream) {

@@ -6,6 +6,8 @@
 //                      or +Inf d_i
 //   aggregate_update   mode 5: g = v + sum_i w_i (x_i - v), v <- g, then the optimizer (aggregate_update.cu)
 //
+// With --rule-scope model the norm is the whole model's: cc_fold_kernel + cc_model_weights_kernel replace cc_weights_kernel.
+//
 // The centre is last step's aggregate, known before the step starts, so only the n row-to-centre distances are needed: the
 // rule runs bucket by bucket on the pipelined PS.  Rows come through an optional [n][T] row table (DETOX's winner_slot).
 // Determinism: per-thread sums, warp shuffles in a fixed pattern, then the 8 warps in order into one partial per (tile, row),
@@ -27,6 +29,7 @@ struct CcArgs {
   double tau;
   int tile_begin, tile_end;               // dist: tiles (tile_end == 0: to the end of the arena)
   int t_begin, t_end;                     // weights: tensors (t_end == 0: every tensor); buckets hold whole tensors
+  double* dist;                           // model scope: [T][n] the per-tensor d_i, folded in tile order
 };
 
 __global__ void __launch_bounds__(DRC_THREADS) cc_dist_kernel(const __grid_constant__ CcArgs a) {
@@ -80,6 +83,32 @@ __global__ void __launch_bounds__(DRC_THREADS) cc_dist_kernel(const __grid_const
 // loads of a batch of CC_FOLD tiles are issued together and the sum stays in order: the fold of a 2304-tile tensor is bound by
 // the load latency of its batches
 #define CC_FOLD 32
+// cc_fold_tensor / cc_weight restate cc_weights_kernel's fold and weight for the model-scope kernels below; the per-tensor
+// kernel keeps its own copy so that its machine code stays what it was
+__device__ __forceinline__ double cc_fold_tensor(const CcArgs& a, int tensor, int i) {
+  const int n = a.n;
+  const TensorMeta m = a.tv.meta[tensor];
+  const int t0 = (int)(m.offset / DRC_TILE), t1 = t0 + (int)((m.numel + DRC_TILE - 1) / DRC_TILE);
+  const double* p = a.partials + i;
+  double d = 0.0;
+  int t = t0;
+  for (; t + CC_FOLD <= t1; t += CC_FOLD) {
+    double b[CC_FOLD];
+#pragma unroll
+    for (int k = 0; k < CC_FOLD; ++k) b[k] = p[(long long)(t + k) * n];
+#pragma unroll
+    for (int k = 0; k < CC_FOLD; ++k) d = __dadd_rn(d, b[k]);
+  }
+  for (; t < t1; ++t) d = __dadd_rn(d, p[(long long)t * n]);
+  return d;
+}
+
+__device__ __forceinline__ float cc_weight(double d, double tau, int n) {
+  if (!(d < INFINITY)) return 0.f;                               // NaN or +Inf: the row is never read
+  if (d == 0.0) return (float)__ddiv_rn(1.0, (double)n);
+  return (float)__ddiv_rn(fmin(1.0, __ddiv_rn(tau, __dsqrt_rn(d))), (double)n);
+}
+
 __global__ void __launch_bounds__(DRC_THREADS) cc_weights_kernel(const __grid_constant__ CcArgs a) {
   const int t_end = a.t_end > 0 ? a.t_end : a.tv.ntensors;
   const int tensor = a.t_begin + (int)(blockIdx.x * (DRC_THREADS / 32) + (threadIdx.x >> 5));
@@ -105,6 +134,38 @@ __global__ void __launch_bounds__(DRC_THREADS) cc_weights_kernel(const __grid_co
   a.weights[tensor * n + i] = w;
 }
 
+// Model scope (--rule-scope model), two kernels.  cc_fold_kernel: the per-tensor fold of cc_weights_kernel, in parallel over
+// the tensors, into dist[T][n].  cc_model_weights_kernel: one CTA; lane i of warp 0 sums dist[t][i] over t in ascending order
+// (a NaN or Inf in one tensor reaches the sum), forms w_i with cc_weight, and the CTA writes w into all T rows of weights, so
+// mode 5 clips every tensor with the one whole-model norm.
+__global__ void __launch_bounds__(DRC_THREADS) cc_fold_kernel(const __grid_constant__ CcArgs a) {
+  const int tensor = (int)(blockIdx.x * (DRC_THREADS / 32) + (threadIdx.x >> 5));
+  const int i = threadIdx.x & 31, n = a.n;
+  if (tensor >= a.tv.ntensors || i >= n) return;
+  a.dist[tensor * n + i] = cc_fold_tensor(a, tensor, i);
+}
+
+__global__ void __launch_bounds__(DRC_THREADS) cc_model_weights_kernel(const __grid_constant__ CcArgs a) {
+  __shared__ float s_w[CC_MAXP];
+  const int n = a.n, T = a.tv.ntensors;
+  if ((int)threadIdx.x < n) {
+    const int i = threadIdx.x;
+    double d = 0.0;
+    int t = 0;
+    for (; t + CC_FOLD <= T; t += CC_FOLD) {
+      double b[CC_FOLD];
+#pragma unroll
+      for (int k = 0; k < CC_FOLD; ++k) b[k] = a.dist[(t + k) * n + i];
+#pragma unroll
+      for (int k = 0; k < CC_FOLD; ++k) d = __dadd_rn(d, b[k]);
+    }
+    for (; t < T; ++t) d = __dadd_rn(d, a.dist[t * n + i]);
+    s_w[i] = cc_weight(d, a.tau, n);
+  }
+  __syncthreads();
+  for (int k = threadIdx.x; k < T * n; k += DRC_THREADS) a.weights[k] = s_w[k % n];
+}
+
 extern "C" int drc_cc_dist(const CcArgs* args, int grid, cudaStream_t stream) {
   if (args->n < 1 || args->n > CC_MAXP || !args->center || !args->partials || grid < 1) return (int)cudaErrorInvalidValue;
   cc_dist_kernel<<<grid, DRC_THREADS, 0, stream>>>(*args);
@@ -117,6 +178,15 @@ extern "C" int drc_cc_weights(const CcArgs* args, cudaStream_t stream) {
   if (args->t_begin < 0 || t_end <= args->t_begin || t_end > args->tv.ntensors) return (int)cudaErrorInvalidValue;
   const int warps = DRC_THREADS / 32;
   cc_weights_kernel<<<(t_end - args->t_begin + warps - 1) / warps, DRC_THREADS, 0, stream>>>(*args);
+  return (int)cudaGetLastError();
+}
+extern "C" int drc_cc_model_weights(const CcArgs* args, cudaStream_t stream) {
+  if (args->n < 1 || args->n > CC_MAXP || !args->partials || !args->weights || !args->dist ||
+      !(args->tau > 0.0 && args->tau < INFINITY) || args->tv.ntensors < 1)
+    return (int)cudaErrorInvalidValue;
+  const int warps = DRC_THREADS / 32;
+  cc_fold_kernel<<<(args->tv.ntensors + warps - 1) / warps, DRC_THREADS, 0, stream>>>(*args);
+  cc_model_weights_kernel<<<1, DRC_THREADS, 0, stream>>>(*args);
   return (int)cudaGetLastError();
 }
 extern "C" int drc_sizeof_CcArgs() { return (int)sizeof(CcArgs); }

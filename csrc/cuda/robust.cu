@@ -491,6 +491,36 @@ extern "C" int drc_nnm_fold(const NnmFoldArgs* args, cudaStream_t stream) {
   return (int)cudaGetLastError();
 }
 
+// ---------------------------------------------------------------------------------------------
+// Model scope (--rule-scope model): a squared distance over the whole model is the sum of the per-tensor squared distances.
+// pair_scope_fold_kernel sums every pair's T entries in ascending tensor order (fp64; a NaN or Inf in one tensor reaches the
+// sum) and writes the sum back into every tensor's table, so krum_select / bulyan_select / geomed_weights / nnm_mix run
+// unchanged and make the same choice in every tensor.  One thread per pair, one CTA: P(P-1)/2 <= 120 pairs.  The loads of a
+// batch of SCOPE_FOLD tensors are issued together and the sum stays in order.
+// ---------------------------------------------------------------------------------------------
+#define SCOPE_FOLD 16
+__global__ void __launch_bounds__(KRUM_MAXPAIRS) pair_scope_fold_kernel(double* pair_d2, int T, int npairs) {
+  const int q = threadIdx.x;
+  if (q >= npairs) return;
+  double s = 0.0;
+  int t = 0;
+  for (; t + SCOPE_FOLD <= T; t += SCOPE_FOLD) {
+    double b[SCOPE_FOLD];
+#pragma unroll
+    for (int k = 0; k < SCOPE_FOLD; ++k) b[k] = pair_d2[(long long)(t + k) * npairs + q];
+#pragma unroll
+    for (int k = 0; k < SCOPE_FOLD; ++k) s = __dadd_rn(s, b[k]);
+  }
+  for (; t < T; ++t) s = __dadd_rn(s, pair_d2[(long long)t * npairs + q]);
+  for (t = 0; t < T; ++t) pair_d2[(long long)t * npairs + q] = s;
+}
+
+extern "C" int drc_pair_scope_fold(double* pair_d2, int T, int P, cudaStream_t stream) {
+  if (!pair_d2 || T < 1 || P < 2 || P > KRUM_MAXP) return (int)cudaErrorInvalidValue;
+  pair_scope_fold_kernel<<<1, KRUM_MAXPAIRS, 0, stream>>>(pair_d2, T, P * (P - 1) / 2);
+  return (int)cudaGetLastError();
+}
+
 extern "C" int drc_pair_dist(const PairDistArgs* args, int grid, cudaStream_t stream) {
   // with or without a row table: at most KRUM_MAXP rows (the pair table of one tensor lives in shared memory)
   if (args->P > KRUM_MAXP) return (int)cudaErrorInvalidValue;

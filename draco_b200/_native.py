@@ -148,13 +148,13 @@ class AttackArgs(C.Structure):
     _fields_ = [("grad_in", ptr), ("slot_stride", i64), ("P", C.c_int), ("mode", C.c_int), ("tv", TileView),
                 ("adv_bitmap", ptr), ("adv_len", C.c_int), ("step_ptr", ptr), ("z", C.c_double), ("stats", ptr),
                 ("partials", ptr), ("gamma", ptr), ("tile_begin", C.c_int), ("tile_end", C.c_int), ("t_begin", C.c_int),
-                ("t_end", C.c_int)]
+                ("t_end", C.c_int), ("fold", ptr)]
 
 
 class CcArgs(C.Structure):
     _fields_ = [("grad_in", ptr), ("slot_stride", i64), ("n", C.c_int), ("rows", ptr), ("tv", TileView), ("center", ptr),
                 ("partials", ptr), ("weights", ptr), ("tau", C.c_double), ("tile_begin", C.c_int), ("tile_end", C.c_int),
-                ("t_begin", C.c_int), ("t_end", C.c_int)]
+                ("t_begin", C.c_int), ("t_end", C.c_int), ("dist", ptr)]
 
 
 def _maybe_build() -> None:
@@ -227,15 +227,18 @@ def cuda() -> C.CDLL:
             "drc_geomed_prep": [C.POINTER(GeoMedPrepArgs), st],
             "drc_geomed_weights": [C.POINTER(GeoMedWeightsArgs), st],
             "drc_pair_dist": [C.POINTER(PairDistArgs), C.c_int, st],
+            "drc_pair_scope_fold": [ptr, C.c_int, C.c_int, st],
             "drc_krum_select": [C.POINTER(KrumSelectArgs), st],
             "drc_bulyan_select": [C.POINTER(BulyanSelectArgs), st],
             "drc_nnm_mix": [C.POINTER(NnmMixArgs), st],
             "drc_nnm_fold": [C.POINTER(NnmFoldArgs), st],
             "drc_attack_stats": [C.POINTER(AttackArgs), C.c_int, st],
             "drc_attack_solve": [C.POINTER(AttackArgs), st],
+            "drc_attack_solve_model": [C.POINTER(AttackArgs), st],
             "drc_attack_write": [C.POINTER(AttackArgs), C.c_int, st],
             "drc_cc_dist": [C.POINTER(CcArgs), C.c_int, st],
             "drc_cc_weights": [C.POINTER(CcArgs), st],
+            "drc_cc_model_weights": [C.POINTER(CcArgs), st],
             "drc_gemm_bf16": [ptr, i64, C.c_int, ptr, i64, C.c_int, ptr, i64, C.c_int, C.c_int, C.c_int, C.c_int, ptr, ptr,
                               C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, st],
             "drc_rt_init": [C.c_int],

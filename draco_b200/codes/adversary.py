@@ -15,7 +15,8 @@ Attack parity (src/model_ops/utils.py:3-23), ``mag = -100``:
   alie     : "A Little Is Enough" (Baruch, Baruch and Goldberg, NeurIPS 2019): mu - z * sigma
   minmax   : min-max (Shejwalkar and Houmansadr, NDSS 2021): mu - gamma * sigma with the largest gamma that keeps the row
              within the largest honest pairwise distance of every honest row
-             (both per tensor, over the honest workers' pushed slots; applied by the PS, see ``alie_row`` / ``minmax_row``)
+             (both per tensor, over the honest workers' pushed slots; applied by the PS, see ``alie_row`` / ``minmax_row``;
+             ``--attack-scope model`` gives min-max one gamma and one Dmax over the whole model, ``minmax_gamma_model``)
 
 The device implementation of the same hook lives in csrc/cuda/push_encode.cu; the integer codes
 below are shared with it.
@@ -155,6 +156,12 @@ def minmax_gamma(H: np.ndarray) -> float:
     largest root is (-b_i + sqrt(b_i^2 - c (a_i - Dmax^2))) / c, written as (Dmax^2 - a_i) / (b_i + sqrt(.)) when b_i > 0
     (the same number without cancellation).  a_i <= Dmax^2 because mu lies in the honest hull, so every root is real and
     >= 0; the clamps only absorb rounding.  c == 0 (all honest rows equal): gamma = 0.  NaN in, NaN out."""
+    return minmax_solve(minmax_terms(H))
+
+
+def minmax_terms(H: np.ndarray) -> np.ndarray:
+    """The fp64 sums gamma depends on, in the device's order: a_i (i < n), b_i, c, then the squared distance of every honest
+    pair (i < j) at 2n + 1 + j(j-1)/2 + i.  Over the whole model each is the sum of the per-tensor ones (``minmax_gamma_model``)."""
     H = np.asarray(H, dtype=np.float64)
     n = H.shape[0]
     mu, sd = honest_stats(H)
@@ -165,6 +172,15 @@ def minmax_gamma(H: np.ndarray) -> float:
         b = (E * p[None, :]).sum(1)
         c = float((p * p).sum())
         d2 = [float(((H[i] - H[j]) ** 2).sum()) for j in range(1, n) for i in range(j)]
+    return np.concatenate([a, b, [c], d2])
+
+
+def minmax_solve(terms: np.ndarray) -> float:
+    """gamma from ``minmax_terms`` (see ``minmax_gamma``)."""
+    terms = np.asarray(terms, dtype=np.float64)
+    n = int(round((-3 + math.sqrt(9 + 8 * (len(terms) - 1))) / 2))        # len = 2n + 1 + n(n-1)/2
+    a, b, c, d2 = terms[:n], terms[n:2 * n], float(terms[2 * n]), [float(x) for x in terms[2 * n + 1:]]
+    with np.errstate(invalid="ignore", over="ignore"):
         D2 = max(d2, key=lambda x: (math.isnan(x), x)) if d2 else 0.0
         if c == 0.0:
             return 0.0
@@ -178,6 +194,15 @@ def minmax_gamma(H: np.ndarray) -> float:
     return math.nan if any(math.isnan(g) for g in roots) else min(roots)
 
 
+def minmax_gamma_model(parts) -> float:
+    """Min-max over the whole model (``--attack-scope model``, as in Shejwalkar and Houmansadr's paper): one gamma and one Dmax
+    for the concatenation of the honest rows' tensors ``parts`` (a list of [n_h, numel_t]).  Every term of ``minmax_terms`` is
+    the fp64 sum, in ascending tensor order, of the per-tensor terms (``oracle.model_d2``), as the fused solve forms it; up to
+    rounding this is ``minmax_gamma`` of the concatenated rows."""
+    from .oracle import model_d2
+    return minmax_solve(model_d2([minmax_terms(H) for H in parts]))
+
+
 def minmax_row(H: np.ndarray) -> np.ndarray:
     """The row every min-max liar sends for one tensor: mu + gamma * p = mu - gamma * sigma (fp64)."""
     mu, sd = honest_stats(H)
@@ -185,18 +210,24 @@ def minmax_row(H: np.ndarray) -> np.ndarray:
         return mu - minmax_gamma(H) * sd
 
 
-def ps_attack(slots: np.ndarray, liars, mode: str, spans, z: Optional[float] = None) -> np.ndarray:
+def ps_attack(slots: np.ndarray, liars, mode: str, spans, z: Optional[float] = None, scope: str = "tensor") -> np.ndarray:
     """Oracle of the whole PS-side step: ``slots`` [P, D] with the liar slots (0-based) replaced, per tensor span
     ``(offset, numel)``, by the attack row built from the honest slots (fp64, rounded to the slots' dtype).  Padding outside
-    the spans is left alone."""
+    the spans is left alone.  ``scope="model"`` (min-max only): one gamma over every span (``minmax_gamma_model``)."""
     out = np.array(slots, copy=True)
     liars = sorted(set(int(w) for w in liars))
     honest = [w for w in range(out.shape[0]) if w not in liars]
     if not liars or not honest:
         return out
-    for off, numel in spans:
-        H = np.asarray(slots[honest, off:off + numel], dtype=np.float64)
-        row = alie_row(H, z) if mode == "alie" else minmax_row(H)
+    parts = [np.asarray(slots[honest, off:off + numel], dtype=np.float64) for off, numel in spans]
+    gamma = minmax_gamma_model(parts) if scope == "model" and mode == "minmax" else None
+    for (off, numel), H in zip(spans, parts):
+        if gamma is not None:
+            mu, sd = honest_stats(H)
+            with np.errstate(invalid="ignore"):
+                row = mu - gamma * sd
+        else:
+            row = alie_row(H, z) if mode == "alie" else minmax_row(H)
         with np.errstate(over="ignore", invalid="ignore"):
             out[liars, off:off + numel] = row.astype(out.dtype)
     return out

@@ -5,6 +5,10 @@ They define the semantics the CUDA kernels (csrc/cuda/*.cu) and the C++ host twi
 *per parameter tensor*, never on the concatenated model (src/master/rep_master.py:154-168,
 src/master/baseline_master.py:271-296).
 
+Every rule that measures distances also has a model scope (``--rule-scope model``, ``model_scope``): the same oracle on the
+rows formed by concatenating every tensor, as the papers define it.  ``model_d2`` restates how the kernels form those
+distances.
+
 ``worker_momentum`` is the one worker-side rule here, and it is fp32 on purpose: every path must produce its exact bits.
 ``centered_clip`` is fp64 where it measures (the distances, the weights) and fp32 where it combines rows, for the same reason.
 """
@@ -354,6 +358,41 @@ def detox(slots: np.ndarray, groups: Sequence[Sequence[int]], mode: str, b: int)
     raise ValueError(f"DETOX has no rule {mode!r}")
 
 
+def model_rows(slots: np.ndarray, spans: Sequence[Tuple[int, int]]) -> np.ndarray:
+    """The whole-model rows of an arena-laid ``slots`` [..., D]: every tensor's real elements ``(offset, numel)`` in tensor
+    order, padding excluded, concatenated along the last axis."""
+    X = np.asarray(slots)
+    return np.concatenate([X[..., off:off + n] for off, n in spans], axis=-1)
+
+
+def split_model(vec: np.ndarray, spans: Sequence[Tuple[int, int]]) -> List[np.ndarray]:
+    """``model_rows`` undone for one result vector: its per-tensor pieces, in tensor order."""
+    out, k = [], 0
+    for _, n in spans:
+        out.append(np.asarray(vec)[..., k:k + n])
+        k += n
+    return out
+
+
+def model_scope(rule, slots: np.ndarray, spans: Sequence[Tuple[int, int]], *args) -> List[np.ndarray]:
+    """Model scope of a per-tensor oracle: ``rule`` applied to ``model_rows(slots, spans)`` (with ``args``), its result split
+    back per tensor.  Under DETOX the rows are the concatenations of each group's per-tensor vote winners (the vote itself
+    stays per tensor); pass those as ``slots``."""
+    return split_model(rule(model_rows(slots, spans), *args), spans)
+
+
+def model_d2(per_tensor) -> np.ndarray:
+    """A model-level distance as the fused kernels form it: the fp64 sum, in ascending tensor id, of the per-tensor fp64
+    distances ``per_tensor`` [T, ...] (pair tables, centered clipping's d_i, or min-max's a_i, b_i, c and pair sums).  A NaN or
+    Inf in any tensor reaches the sum, and the NaN-last and lower-row tie rules of every selection then apply unchanged."""
+    D = np.asarray(per_tensor, dtype=np.float64)
+    acc = np.zeros(D.shape[1:], dtype=np.float64)
+    with np.errstate(invalid="ignore", over="ignore"):
+        for d in D:
+            acc = acc + d
+    return acc
+
+
 def sgd_momentum_step(p: np.ndarray, buf: np.ndarray, g: np.ndarray, lr: float, momentum: float,
                       weight_decay: float = 0.0, dampening: float = 0.0, nesterov: bool = False,
                       first_step: bool = False) -> Tuple[np.ndarray, np.ndarray]:
@@ -425,8 +464,8 @@ def centered_clip(rows: np.ndarray, center: np.ndarray, tau: float, weights=None
     g = v + (1/n) sum_i (x_i - v) min(1, tau / ||x_i - v||), with the n fp32 rows x_i and the fp32 centre v (the previous
     aggregate of this tensor, +0 at the start).  The weights come from ``centered_clip_weights`` (or ``weights``); then per
     coordinate acc = +0, acc = fma_rn(w_i, rn(x_i - v), acc) for i ascending with w_i != 0, and g = rn(v + acc), all fp32 with
-    no other contraction.  g is both the aggregated gradient and the next centre.  The norm and tau are per tensor, where the
-    paper clips the whole model's vector."""
+    no other contraction.  g is both the aggregated gradient and the next centre.  The norm and tau are those of the rows given:
+    per tensor by default, the paper's whole-model vector under ``model_scope`` (``--rule-scope model``)."""
     X = np.asarray(rows, dtype=np.float32)
     v = np.asarray(center, dtype=np.float32)
     w = centered_clip_weights(X, v, tau) if weights is None else np.asarray(weights, dtype=np.float32)

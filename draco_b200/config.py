@@ -19,6 +19,9 @@ NNM_MODES = ("coordinate_median", "trimmed_mean", "krum", "multi_krum", "geometr
 ROBUST_MAXP = 16                    # workers the fused coordinate-wise / Krum / Bulyan kernels take (TRIM_MAXP, KRUM_MAXP)
 ERR_MODES = ("rev_grad", "constant", "random", "omniscient", "alie", "minmax", "none")
 TRANSPORTS = ("nvl", "nccl", "nccl_flat", "gloo")
+SCOPES = ("tensor", "model")        # --rule-scope / --attack-scope: distances per parameter tensor, or over the whole model
+# the --mode values whose rule measures distances between rows (every --approach nnm mode does, through its neighbourhoods)
+DISTANCE_MODES = ("krum", "multi_krum", "geometric_median", "bulyan", "centered_clip")
 
 
 @dataclass
@@ -83,7 +86,9 @@ class JobConfig:
     zero_copy_grads: bool = True    # push reads gradients where autograd left them (pointer table), no flat gather
     attack_z: Optional[float] = None  # --err-mode alie: z of mu - z * sigma (None: Baruch et al.'s z_max for P and f)
     worker_momentum: float = 0.0    # beta of worker-side momentum: every worker pushes m <- beta m + (1 - beta) g (0: off)
-    clip_tau: Optional[float] = None  # --mode centered_clip: the clipping radius tau, per tensor, in the gradient's units
+    clip_tau: Optional[float] = None  # --mode centered_clip: the clipping radius tau in the gradient's units (per rule_scope)
+    rule_scope: str = "tensor"      # distance-based rules: one choice per parameter tensor, or one over the whole model
+    attack_scope: str = "tensor"    # --err-mode minmax: one gamma per parameter tensor, or one over the whole model
 
     # ---- derived --------------------------------------------------------------------------
     def resolve(self, world_size: int) -> "JobConfig":
@@ -127,6 +132,7 @@ class JobConfig:
         self._check_ps_attack()
         self._check_worker_momentum()
         self._check_centered_clip()
+        self._check_scope()
         if self.transport == "gloo":
             self.dtype = "fp32"
             self.cuda_graphs = False
@@ -200,6 +206,30 @@ class JobConfig:
         if self.transport == "nccl_flat":
             raise ValueError("--transport nccl_flat runs the plain mean and the vote only; use --transport nccl for "
                              "--mode centered_clip")
+
+    def _check_scope(self) -> None:
+        """--rule-scope / --attack-scope model: the rule's distances, or min-max's gamma and Dmax, over the whole model."""
+        for flag, v in (("--rule-scope", self.rule_scope), ("--attack-scope", self.attack_scope)):
+            if v not in SCOPES:
+                raise ValueError(f"{flag} must be one of {SCOPES}, got {v!r}")
+        if self.attack_scope == "model" and self.err_mode != "minmax":
+            raise ValueError(f"--attack-scope model sets one gamma for the whole model: it needs --err-mode minmax (got --err-mode "
+                             f"{self.err_mode}; alie is coordinate-wise, so the scope would change nothing)")
+        if self.rule_scope == "tensor" and self.attack_scope == "tensor":
+            return
+        if self.transport == "nccl_flat":
+            raise ValueError("--transport nccl_flat runs the plain mean and the vote only; use --transport nccl for "
+                             "--rule-scope model / --attack-scope model")
+        if self.rule_scope == "tensor":
+            return
+        if not (self.approach == "nnm" or (self.approach in ("baseline", "detox") and self.mode in DISTANCE_MODES)):
+            raise ValueError(f"--rule-scope model applies to the rules that measure distances between rows (--mode "
+                             f"{' | '.join(DISTANCE_MODES)} under baseline or detox, and every --approach nnm mode); --approach "
+                             f"{self.approach} --mode {self.mode} is coordinate-wise, so the scope would change nothing")
+        rows = self.num_groups if self.approach == "detox" else self.num_workers
+        if self.transport == "nvl" and self.mode == "geometric_median" and rows > ROBUST_MAXP:
+            raise ValueError(f"--rule-scope model: the geometric median of more than {ROBUST_MAXP} rows on the nvl transport "
+                             f"streams over the slab per tensor (got {rows} rows); use --transport nccl or fewer rows")
 
     @property
     def alie_z(self) -> float:
@@ -337,8 +367,15 @@ def add_fit_args(parser: argparse.ArgumentParser) -> argparse.ArgumentParser:
            "Mhamdi et al. 2021).  --momentum still applies at the PS on top; the papers' recipe is --worker-momentum 0.9 "
            "--momentum 0")
     a("--clip-tau", type=float, default=None,
-      help="--mode centered_clip: the clipping radius tau, per tensor, in the gradient's own units (required; the papers' "
-           "recipe pairs it with --worker-momentum 0.9 --momentum 0)")
+      help="--mode centered_clip: the clipping radius tau, per tensor (--rule-scope model: of the whole model's norm), in the "
+           "gradient's own units (required; the papers' recipe pairs it with --worker-momentum 0.9 --momentum 0)")
+    a("--rule-scope", type=str, default=d.rule_scope, choices=SCOPES,
+      help="tensor (default): the distance-based rules (krum, multi_krum, geometric_median, bulyan's selection, centered_clip's "
+           "norm, every --approach nnm neighbourhood) measure distances per parameter tensor and may choose differently in each; "
+           "model: over the flattened model, one choice for every tensor, as in the papers")
+    a("--attack-scope", type=str, default=d.attack_scope, choices=SCOPES,
+      help="--err-mode minmax: tensor (default) solves gamma and Dmax per parameter tensor; model: one gamma and one Dmax over "
+           "the flattened model, as in the NDSS paper")
     a("--approach", type=str, default=d.approach,
       help="baseline | maj_vote | cyclic | detox (majority vote inside each repetition group, then --mode across the G group "
            "winners) | nnm (nearest-neighbour mixing: every worker's row is replaced, per tensor, by the mean of its "

@@ -142,6 +142,20 @@ def ps_attack(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, mode
     """Overwrite the liar slots of the step (``adv_bitmap[*step_ptr % adv_len]``) of ``grad_in`` [P, slot_stride] with the ALIE
     (``mode`` 5, ``z``) or min-max (``mode`` 6, workspace ``ws``) row of every tensor, built from the honest slots
     (csrc/cuda/attack.cu).  ``tile_range`` / ``tensor_range``: one bucket (whole tensors).  Returns the kernels launched."""
+    a, g = _attack_args(layout, grad_in, slot_stride, P, mode, adv_bitmap, adv_len, step_ptr, z, ws, tile_range, grid)
+    if tensor_range is not None:
+        a.t_begin, a.t_end = int(tensor_range[0]), int(tensor_range[1])
+    lib = N.cuda()
+    N.check(lib.drc_attack_stats(C.byref(a), g, _stream()), "attack_stats")
+    if mode == 5:
+        return 1
+    N.check(lib.drc_attack_solve(C.byref(a), _stream()), "attack_solve")
+    N.check(lib.drc_attack_write(C.byref(a), g, _stream()), "attack_write")
+    return 3
+
+
+def _attack_args(layout, grad_in, slot_stride, P, mode, adv_bitmap, adv_len, step_ptr, z, ws, tile_range, grid):
+    """The ``AttackArgs`` both attack launchers share, and the grid of the tile kernels."""
     if not 1 <= P <= ATTACK_MAXP:
         raise ValueError(f"the PS-side attacks take 1..{ATTACK_MAXP} worker slots, got {P}")
     if mode not in (5, 6):
@@ -159,16 +173,29 @@ def ps_attack(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, mode
     if tile_range is not None:
         a.tile_begin, a.tile_end = int(tile_range[0]), int(tile_range[1])
         ntiles = a.tile_end - a.tile_begin
-    if tensor_range is not None:
-        a.t_begin, a.t_end = int(tensor_range[0]), int(tensor_range[1])
-    g = grid or max(1, min(ntiles, sm_count() * 8))
+    return a, grid or max(1, min(ntiles, sm_count() * 8))
+
+
+def attack_fold_buffer(layout: ArenaLayout, P: int, device) -> torch.Tensor:
+    """The fp64 [T, Q] scratch of ``ps_attack_model``: each tensor's min-max partials folded in tile order."""
+    return torch.zeros(layout.ntensors, 2 * P + 1 + P * (P - 1) // 2, dtype=torch.float64, device=device)
+
+
+def ps_attack_model(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, *, adv_bitmap: Addr, adv_len: int,
+                    step_ptr: Addr, ws: AttackWorkspace, fold: torch.Tensor, grid: Optional[int] = None) -> int:
+    """The min-max attack with one gamma and one Dmax over the whole model (``--attack-scope model``; codes/adversary.py
+    ``minmax_gamma_model``): the stats pass over the arena, the per-tensor fold of its partials into ``fold``
+    (``attack_fold_buffer``), one solve over their sum in ascending tensor order, which writes gamma into every tensor, then
+    the write pass.  Returns the kernels launched."""
+    Q = 2 * P + 1 + P * (P - 1) // 2
+    _check_buffer("ps_attack_model: fold", fold, torch.float64, (layout.ntensors, Q))
+    a, g = _attack_args(layout, grad_in, slot_stride, P, 6, adv_bitmap, adv_len, step_ptr, 0.0, ws, None, grid)
+    a.fold = fold.data_ptr()
     lib = N.cuda()
     N.check(lib.drc_attack_stats(C.byref(a), g, _stream()), "attack_stats")
-    if mode == 5:
-        return 1
-    N.check(lib.drc_attack_solve(C.byref(a), _stream()), "attack_solve")
+    N.check(lib.drc_attack_solve_model(C.byref(a), _stream()), "attack_solve_model")
     N.check(lib.drc_attack_write(C.byref(a), g, _stream()), "attack_write")
-    return 3
+    return 4
 
 
 # ------------------------------------------------------------------------------------------------ vote (K3)
@@ -354,6 +381,23 @@ def centered_clip_weights(layout: ArenaLayout, n: int, tau: float, partials: tor
     N.check(N.cuda().drc_cc_weights(C.byref(a), _stream()), "cc_weights")
 
 
+def centered_clip_model_weights(layout: ArenaLayout, n: int, tau: float, partials: torch.Tensor, dist: torch.Tensor,
+                                weights: torch.Tensor) -> None:
+    """Model scope (``--rule-scope model``): fold ``centered_clip_dist``'s partials per tensor in tile order into ``dist``
+    [T, n] fp64, sum them over the tensors in ascending order into the whole-model d_i, and write the one set of weights
+    w_i = ``centered_clip_weight(d_i, tau, n)`` into every row of ``weights`` [T, n] (two kernels, csrc/cuda/clip.cu)."""
+    _check_cc_rows("centered_clip_model_weights", n)
+    if not (math.isfinite(tau) and tau > 0):
+        raise ValueError(f"centered_clip_model_weights: tau must be finite and > 0, got {tau}")
+    _check_buffer("centered_clip_model_weights: partials", partials, torch.float64, (layout.ntiles, n))
+    _check_buffer("centered_clip_model_weights: dist", dist, torch.float64, (layout.ntensors, n))
+    _check_buffer("centered_clip_model_weights: weights", weights, torch.float32, (layout.ntensors, n))
+    a = N.CcArgs()
+    a.n, a.tv = n, layout.tile_view(weights.device)
+    a.partials, a.dist, a.weights, a.tau = partials.data_ptr(), dist.data_ptr(), weights.data_ptr(), float(tau)
+    N.check(N.cuda().drc_cc_model_weights(C.byref(a), _stream()), "cc_model_weights")
+
+
 def centered_clip_update(layout: ArenaLayout, grad_in: Addr, slot_stride: int, *, center: torch.Tensor, weights: torch.Tensor,
                          K: int, params: Addr, momentum: Addr, hp: Addr, step_ptr: Addr, done_counter: Addr,
                          select: Optional[torch.Tensor] = None, first_step: int = 1, grad_out: Addr = None,
@@ -489,6 +533,31 @@ def _pair_dist(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, pai
     N.check(N.cuda().drc_pair_dist(C.byref(pa), stream_grid(layout, 4), _stream()), "pair_dist")
 
 
+def _check_pair_table(what: str, layout: ArenaLayout, P: int, pair_d2) -> None:
+    if not 2 <= P <= GEOMED_FAST_MAXP:
+        raise ValueError(f"{what}: takes 2..{GEOMED_FAST_MAXP} rows, got {P}")
+    _check_buffer(f"{what}: pair_d2", pair_d2, torch.float64, (layout.ntensors, P * (P - 1) // 2))
+
+
+def pair_dist(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, pair_d2: torch.Tensor,
+              rows: Optional[torch.Tensor] = None) -> None:
+    """The pair-distance pass alone (the one ``krum_select`` / ``bulyan_select`` / ``geometric_median_weights`` / ``nnm_mix``
+    launch unless ``filled``): the squared distances between the P rows of every tensor, added into the zeroed fp64 ``pair_d2``
+    [T, P(P-1)/2].  ``rows``: optional int32 [P, T] table, row i of tensor t is worker slot ``rows[i, t]``."""
+    _check_pair_table("pair_dist", layout, P, pair_d2)
+    if rows is not None:
+        _check_row_table(layout, rows, P)
+    _pair_dist(layout, grad_in, slot_stride, P, pair_d2, rows)
+
+
+def pair_scope_fold(layout: ArenaLayout, P: int, pair_d2: torch.Tensor) -> None:
+    """Model scope (``--rule-scope model``): replace every tensor's pair table by the model-level one, each pair's entries summed
+    over the tensors in ascending order in fp64 (codes/oracle.py ``model_d2``; csrc/cuda/robust.cu).  The selection kernels
+    then run with ``filled=True`` and make the same choice in every tensor; they zero the table as usual."""
+    _check_pair_table("pair_scope_fold", layout, P, pair_d2)
+    N.check(N.cuda().drc_pair_scope_fold(pair_d2.data_ptr(), layout.ntensors, P, _stream()), "pair_scope_fold")
+
+
 def geometric_median_weights(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, pair_d2: torch.Tensor,
                              weights: torch.Tensor, max_iter: int = 256, eps: float = 1e-10,
                              iters_out: Optional[torch.Tensor] = None, rows: Optional[torch.Tensor] = None,
@@ -553,6 +622,20 @@ def nnm_mix(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, f: int
         raise ValueError(f"nnm_mix: needs 0 <= f < P <= {ROW_TABLE_MAXROWS} (got P = {P}, f = {f})")
     _check_row_table(layout, mix, P)
     _pair_dist(layout, grad_in, slot_stride, P, pair_d2, None)
+    _nnm_mix_kernel(layout, P, f, pair_d2, mix, mixed_out)
+
+
+def nnm_mix_table(layout: ArenaLayout, P: int, f: int, pair_d2: torch.Tensor, mix: torch.Tensor, mixed_out: bool) -> None:
+    """``nnm_mix`` without its pair-distance pass: ``pair_d2`` already holds the raw rows' distances (``pair_dist``, then
+    ``pair_scope_fold`` for one neighbourhood per worker over the whole model)."""
+    if not (0 <= f < P <= ROW_TABLE_MAXROWS):
+        raise ValueError(f"nnm_mix_table: needs 0 <= f < P <= {ROW_TABLE_MAXROWS} (got P = {P}, f = {f})")
+    _check_row_table(layout, mix, P)
+    _check_pair_table("nnm_mix_table", layout, P, pair_d2)
+    _nnm_mix_kernel(layout, P, f, pair_d2, mix, mixed_out)
+
+
+def _nnm_mix_kernel(layout, P, f, pair_d2, mix, mixed_out) -> None:
     na = N.NnmMixArgs(pair_d2.data_ptr(), layout.ntensors, P, f, mix.data_ptr(), int(bool(mixed_out)))
     N.check(N.cuda().drc_nnm_mix(C.byref(na), _stream()), "nnm_mix")
 

@@ -158,7 +158,17 @@ class CollectiveEngine:
         if not liars or not honest:
             return
         z = self.cfg.alie_z if self.cfg.err_mode == "alie" else 0.0
-        for s in self.layout.specs:
+        specs = self.layout.specs
+        if self.cfg.attack_scope == "model":            # --attack-scope model: one gamma over the whole model
+            Hs = [self.slots[honest, s.offset: s.offset + s.numel].double() for s in specs]
+            gamma = minmax_gamma_model(Hs)
+            for s, H in zip(specs, Hs):
+                n = H.shape[0]
+                mu = H.sum(0) / n
+                sd = (((H - mu) ** 2).sum(0) / n).sqrt()
+                self.slots[liars, s.offset: s.offset + s.numel] = (mu - gamma * sd).to(self.slots.dtype)
+            return
+        for s in specs:
             H = self.slots[honest, s.offset: s.offset + s.numel].double()
             row = attack_row(H, self.cfg.err_mode, z).to(self.slots.dtype)
             self.slots[liars, s.offset: s.offset + s.numel] = row
@@ -317,3 +327,21 @@ def attack_row(H: torch.Tensor, mode: str, z: float = 0.0) -> torch.Tensor:
     r = (b * b + c * (D2 - a)).clamp_min(0).sqrt()
     g = torch.where(b <= 0, (r - b) / c, (D2 - a) / (b + r)).clamp_min(0)
     return mu - g.min() * sd
+
+
+def minmax_gamma_model(Hs) -> float:
+    """Min-max's one gamma over the whole model from the honest rows of every tensor (fp64): the sums a_i, b_i, c and the pair
+    distances of each tensor (codes/adversary.py ``minmax_terms``, same layout), added over the tensors in ascending order,
+    then the oracle's closed form (``minmax_solve``)."""
+    from ..codes.adversary import minmax_solve
+    acc = None
+    for H in Hs:
+        n = H.shape[0]
+        mu = H.sum(0) / n
+        sd = (((H - mu) ** 2).sum(0) / n).sqrt()
+        p = -sd
+        E = mu - H
+        d2 = [((H[i] - H[j]) ** 2).sum() for j in range(1, n) for i in range(j)]
+        t = torch.cat([(E * E).sum(1), (E * p).sum(1), (p * p).sum()[None]] + ([torch.stack(d2)] if d2 else []))
+        acc = t if acc is None else acc + t
+    return minmax_solve(acc.cpu().numpy())

@@ -41,13 +41,20 @@ from ..ops import kernels as K
 from ..utils.metrics import PhaseTimer, limit_host_threads, wait_event
 from .arena import ArenaLayout
 from .placement import Placement
-from .ps import PIPELINED_RULES, FusedPS, build_codes, select_rule
+from .ps import FusedPS, build_codes, rule_plan
 from .symm import SymmContext
 from .worker import WorkerCompute, make_model
 
 FLAG_STRIDE = 128            # bytes between flag words (one per 128-B line)
 FLAG_BYTES = 65536
 MAX_BUCKETS = 8              # per-worker gradient-bucket flags
+
+
+def pipelines_ps(cfg: JobConfig, overlap_push: bool) -> bool:
+    """Whether the PS applies the step bucket by bucket.  The rule's part is the PS's own decision (``RulePlan.pipelined``, the
+    scopes included): ``FusedPS.enqueue_step`` waits for a bucket only when it pipelines itself, so an engine that pipelined
+    while the PS took the whole-arena path would let the PS read slots before they land."""
+    return overlap_push and cfg.pipeline_ps and rule_plan(cfg).pipelined and cfg.err_mode != "omniscient"
 
 
 class FusedEngine:
@@ -81,8 +88,7 @@ class FusedEngine:
         self.compress = bool(cfg.compress)
         self.overlap_push = cfg.overlap_push and not self.cyclic and not self.compress
         # PS pipelining: decode + apply + broadcast each gradient bucket as soon as all workers pushed it
-        self.pipeline_ps = (self.overlap_push and cfg.pipeline_ps and select_rule(cfg) in PIPELINED_RULES
-                            and cfg.err_mode != "omniscient")
+        self.pipeline_ps = pipelines_ps(cfg, self.overlap_push)
         self.push_stream = torch.cuda.Stream(device=device) if self.overlap_push else None
         ns = min(max(int(cfg.worker_streams), 1), len(self.local_workers))
         # weight gradients on a side stream (auto = on: +5.6 % for a worker that owns its GPU, +2.4 % with seven workers sharing

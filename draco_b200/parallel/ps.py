@@ -21,7 +21,8 @@ import torch
 from .. import _native as N
 from ..codes.adversary import ATTACK_ALIE, ATTACK_MINMAX, PS_ATTACKS, attack_code
 from ..codes.cyclic import CyclicCode, search_w
-from ..codes.oracle import centered_clip_weight
+from ..codes.oracle import (_bulyan_rounds, _krum_scores_d2, _weiszfeld_weights, centered_clip_weight, model_d2,
+                            nnm_neighbours_d2, nnm_pair_d2)
 from ..codes.repetition import GroupPlan
 from ..config import JobConfig
 from .arena import ArenaLayout
@@ -57,7 +58,8 @@ NNM_RULES = {"coordinate_median": "nnm_median", "trimmed_mean": "nnm_trimmed_mea
 
 
 # rules the fused PS applies bucket by bucket while the workers still push (nothing in them reaches beyond the bucket's
-# tensors: buckets hold whole tensors, and centered clipping's centre is known before the step starts)
+# tensors: buckets hold whole tensors, and centered clipping's centre is known before the step starts).  Only at the default
+# scopes: a whole-model distance, or min-max's whole-model gamma, needs every bucket first (RulePlan.pipelined)
 PIPELINED_RULES = ("mean", "vote", "median", "trimmed_mean", "detox_median", "detox_trimmed_mean", "centered_clip",
                    "detox_centered_clip")
 
@@ -79,7 +81,9 @@ class RulePlan:
     m: int              # Krum / multi-Krum: rows averaged
     theta: int          # Bulyan: rows selected
     opt_mode: str       # the optimizer's mode string
-    pipelined: bool     # the fused PS may apply it bucket by bucket (PIPELINED_RULES)
+    pipelined: bool     # the fused PS may apply it bucket by bucket: a PIPELINED_RULES rule with both scopes "tensor"
+    scope: str          # --rule-scope: tensor | model (one choice over the whole model for every tensor)
+    attack_scope: str   # --attack-scope: tensor | model (min-max: one gamma over the whole model)
 
 
 def rule_plan(cfg: JobConfig) -> RulePlan:
@@ -95,8 +99,9 @@ def rule_plan(cfg: JobConfig) -> RulePlan:
     f = cfg.captured_group_bound if source == "detox" else cfg.worker_fail
     trim = {"median": (rows - 1) // 2, "trimmed_mean": f}.get(base, 0)
     m = {"krum": 1, "multi_krum": rows - f}.get(base, 0)
+    scope, attack_scope = cfg.rule_scope, cfg.attack_scope
     return RulePlan(rule, source, base, rows, f, trim, m, rows - 2 * f if base == "bulyan" else 0, _OPT_MODE[base],
-                    rule in PIPELINED_RULES)
+                    rule in PIPELINED_RULES and scope == "tensor" and attack_scope == "tensor", scope, attack_scope)
 
 
 def hyperparams_tensor(cfg: JobConfig, device) -> torch.Tensor:
@@ -135,6 +140,9 @@ class FusedPS:
         self.adv_bitmap, self.adv_len = adv_bitmap, adv_len
         self.attack_z = cfg.alie_z if self.attack == ATTACK_ALIE else 0.0
         self.attack_ws = K.AttackWorkspace(layout, self.P, device) if self.attack == ATTACK_MINMAX else None
+        # --attack-scope model: min-max's per-tensor sums, folded, then one solve over the whole arena
+        self.attack_fold = (K.attack_fold_buffer(layout, self.P, device)
+                            if self.attack == ATTACK_MINMAX and plan.attack_scope == "model" else None)
         # row source.  DETOX: the rule runs on the G rows the vote's winner_slot table names, inside the kernels that read the
         # slab anyway.  NNM: the mixing masks; the rule then runs on the mixed rows.
         if plan.source == "detox":
@@ -161,6 +169,8 @@ class FusedPS:
             self.cc_center = layout.new_arena(device)
             self.cc_partials = torch.zeros(layout.ntiles, rows, dtype=torch.float64, device=device)
             self.cc_weights = torch.zeros(T, rows, dtype=torch.float32, device=device)
+            if plan.scope == "model":                     # the per-tensor d_i the whole-model norm is summed from
+                self.cc_dist = torch.zeros(T, rows, dtype=torch.float64, device=device)
         if plan.source == "nnm" and plan.base in ("krum", "multi_krum", "geomedian"):
             self.w_raw = torch.zeros(T, self.P, dtype=torch.float32, device=device)   # the choice, folded into raw-slot weights
         if plan.base == "cyclic":
@@ -199,12 +209,16 @@ class FusedPS:
         # (tile range, tensor range) of every bucket; None: the whole arena
         ranges = [((t0, t1), (min(idxs), max(idxs) + 1)) for t0, t1, idxs in buckets] if pipelined else [(None, None)]
         nnm = plan.source == "nnm"
+        model = plan.scope == "model"                     # one choice for every tensor, from the whole-model distances
         n = 0
         for bi, (tiles, tensors) in enumerate(ranges):
             last = bi == len(ranges) - 1
             if pipelined:
                 n += wait_bucket(bi)
-            if self.attack:
+            if self.attack_fold is not None:
+                n += K.ps_attack_model(L, self.grad_in, self.slot_stride, self.P, adv_bitmap=self.adv_bitmap, adv_len=self.adv_len,
+                                       step_ptr=step_ptr, ws=self.attack_ws, fold=self.attack_fold)
+            elif self.attack:
                 n += K.ps_attack(L, self.grad_in, self.slot_stride, self.P, self.attack, adv_bitmap=self.adv_bitmap,
                                  adv_len=self.adv_len, step_ptr=step_ptr, z=self.attack_z, ws=self.attack_ws,
                                  tile_range=tiles, tensor_range=tensors)
@@ -214,9 +228,20 @@ class FusedPS:
                 K.vote(L, self.grad_in, self.slot_stride, self.group_table, self.neq_mask, self.winner_slot, self.winner_member,
                        tile_range=tiles, tensor_range=tensors); n += 2
                 rows = self.winner_slot
+            elif nnm and model:                            # one neighbourhood per worker over the whole model
+                K.pair_dist(L, self.grad_in, self.slot_stride, self.P, self.pair_d2)
+                K.pair_scope_fold(L, self.P, self.pair_d2)
+                K.nnm_mix_table(L, self.P, plan.f, self.pair_d2, self.mix, mixed_out=plan.base not in ("median", "trimmed_mean"))
+                n += 3
             elif nnm:                                      # the choices below read the mixed rows' distances (filled=True)
                 K.nnm_mix(L, self.grad_in, self.slot_stride, self.P, plan.f, self.pair_d2, self.mix,
                           mixed_out=plan.base not in ("median", "trimmed_mean")); n += 2
+            # model scope: the pair table summed over the tensors and written back into each, then filled=True below
+            filled = nnm
+            if model and not nnm and plan.base in ("krum", "multi_krum", "geomedian", "bulyan"):
+                K.pair_dist(L, self.grad_in, self.slot_stride, plan.rows, self.pair_d2, rows=rows)
+                K.pair_scope_fold(L, plan.rows, self.pair_d2); n += 2
+                filled = True
             # selection, then the arguments of the one fused update
             src, agg = self.grad_in, dict(K=plan.rows, select=rows)
             if plan.base in ("mean", "vote"):
@@ -227,6 +252,10 @@ class FusedPS:
                 agg.update(scale=1.0 / self.P, recomb=self.recomb)
             elif plan.base in ("median", "trimmed_mean"):   # coordinate-wise: element by element, nothing per tensor
                 agg.update(scale=1.0 / (plan.rows - 2 * plan.trim), trim=plan.trim)
+            elif plan.base == "centered_clip" and model:   # one norm over the whole model, after the last bucket
+                K.centered_clip_dist(L, self.grad_in, self.slot_stride, plan.rows, self.cc_center, self.cc_partials, rows=rows)
+                K.centered_clip_model_weights(L, plan.rows, self.cfg.clip_tau, self.cc_partials, self.cc_dist, self.cc_weights)
+                n += 3
             elif plan.base == "centered_clip":             # per tensor, from the n distances to the centre: bucket by bucket
                 K.centered_clip_dist(L, self.grad_in, self.slot_stride, plan.rows, self.cc_center, self.cc_partials, rows=rows,
                                      tile_range=tiles)
@@ -234,7 +263,7 @@ class FusedPS:
                                         tensor_range=tensors); n += 2
             elif plan.base == "bulyan":                    # select holds the rows Bulyan keeps
                 K.bulyan_select(L, self.grad_in, self.slot_stride, plan.rows, plan.f, self.pair_d2, self.select, rows=rows,
-                                filled=nnm); n += 1 if nnm else 2
+                                filled=filled); n += 1 if filled else 2
                 agg.update(K=plan.theta, scale=1.0 / (plan.theta - 2 * plan.f), near_median=plan.f, select=self.select)
             elif self.gm is not None:
                 iters = 48
@@ -244,15 +273,15 @@ class FusedPS:
             else:                                          # geometric median weights, or the m best Krum rows
                 if plan.base == "geomedian":
                     K.geometric_median_weights(L, self.grad_in, self.slot_stride, plan.rows, self.pair_d2, self.gm_weights,
-                                               rows=rows, filled=nnm)
+                                               rows=rows, filled=filled)
                     choice = dict(w_mix=self.gm_weights)
                     agg.update(scale=1.0, weights=self.gm_weights)
                 else:
                     K.krum_select(L, self.grad_in, self.slot_stride, plan.rows, plan.f, self.pair_d2, self.select, m=plan.m,
-                                  rows=rows, filled=nnm)
+                                  rows=rows, filled=filled)
                     choice = dict(select=self.select, m=plan.m)
                     agg.update(K=plan.m, scale=1.0 / plan.m, select=self.select)
-                n += 1 if nnm else 2
+                n += 1 if filled else 2
                 if nnm:                                    # a choice over the mixed rows, as weights over the raw slots
                     K.nnm_fold(L, self.P, plan.f, self.mix, self.w_raw, **choice); n += 1
                     agg = dict(K=self.P, scale=1.0, weights=self.w_raw)
@@ -422,7 +451,11 @@ class TorchPS:
             sub.fill_diagonal_(float("nan"))               # sorts last; keep <= |R| - 2 never reaches it unless a real NaN does
             scores = sub.sort(1).values[:, :keep].sum(1)
             chosen.append(R.pop(int(torch.argsort(scores, stable=True)[0])))
-        S = X[chosen].sort(0).values
+        return self._nearest_to_median_mean(X[chosen], f)
+
+    def _nearest_to_median_mean(self, X: torch.Tensor, f: int) -> torch.Tensor:
+        """Bulyan's coordinate stage over the theta chosen rows ``X`` (``oracle.nearest_to_median_mean``, fp32)."""
+        S = X.sort(0).values
         theta = S.shape[0]
         beta = theta - 2 * f
         lo, hi = S[(theta - 1) // 2], S[theta // 2]
@@ -447,7 +480,11 @@ class TorchPS:
         P = X.shape[0]
         d2 = torch.cdist(X.double(), X.double()).pow(2)
         d2.fill_diagonal_(-1.0)                            # row i is its own first neighbour
-        nbrs = d2.argsort(dim=1, stable=True)[:, :P - f].sort(dim=1).values.tolist()
+        return self._mix_rows(X, d2.argsort(dim=1, stable=True)[:, :P - f].sort(dim=1).values.tolist(), f)
+
+    def _mix_rows(self, X: torch.Tensor, nbrs: List[List[int]], f: int) -> torch.Tensor:
+        """Mixed row i: the fp32 sum of the rows ``nbrs[i]`` (ascending) from +0, times fp32(1 / (P - f))."""
+        P = X.shape[0]
         scale = torch.tensor(1.0 / (P - f), dtype=torch.float32, device=X.device)
         Y = torch.empty_like(X)
         for i in range(P):
@@ -457,15 +494,15 @@ class TorchPS:
             Y[i] = y * scale
         return Y
 
-    def _centered_clip_tensor(self, X: torch.Tensor, v: torch.Tensor) -> torch.Tensor:
+    def _centered_clip_tensor(self, X: torch.Tensor, v: torch.Tensor, weights: Optional[List[float]] = None) -> torch.Tensor:
         """Centered clipping (``oracle.centered_clip``) around the centre ``v``, which it replaces: fp64 distances, fp32 weights
-        from ``centered_clip_weight``, then per coordinate acc = fma_rn(w_i, rn(x_i - v), acc) over the rows with w_i != 0 in
-        ascending order, and g = rn(v + acc) -- the fused kernel's fp32 order."""
+        from ``centered_clip_weight`` (or ``weights``, the whole-model ones), then per coordinate acc = fma_rn(w_i, rn(x_i - v),
+        acc) over the rows with w_i != 0 in ascending order, and g = rn(v + acc) -- the fused kernel's fp32 order."""
         n = X.shape[0]
-        d = (X.double() - v.double()).pow(2).sum(1).tolist()
+        if weights is None:
+            weights = [centered_clip_weight(di, self.cfg.clip_tau, n) for di in (X.double() - v.double()).pow(2).sum(1).tolist()]
         acc = torch.zeros_like(v)
-        for i, di in enumerate(d):
-            w = centered_clip_weight(di, self.cfg.clip_tau, n)
+        for i, w in enumerate(weights):
             if w != 0.0:
                 acc = _fma_f32(w, X[i] - v, acc)
         g = v + acc
@@ -490,15 +527,13 @@ class TorchPS:
         on them."""
         plan = self.plan
         self.last_info = {}
+        if plan.scope == "model":
+            return self._aggregate_model(slots)
         out = []
         for spec in self.layout.specs:
             X = slots[:, spec.offset: spec.offset + spec.numel]
             if plan.source == "detox":                   # the vote inside every group
-                winners = []
-                for grp in self.groups.groups:
-                    rows = [X[w - 1] for w in grp]
-                    winners.append(rows[self._vote_tensor(rows)])
-                X = torch.stack(winners)
+                X = self._detox_rows(X)
             elif plan.source == "nnm":
                 X = self._nnm_mix_tensor(X, plan.f)
             if plan.base == "mean":
@@ -525,11 +560,59 @@ class TorchPS:
             out.append(g)
         return out
 
+    def _detox_rows(self, X: torch.Tensor) -> torch.Tensor:
+        """The G group winners of one tensor's vote, in group order."""
+        winners = []
+        for grp in self.groups.groups:
+            rows = [X[w - 1] for w in grp]
+            winners.append(rows[self._vote_tensor(rows)])
+        return torch.stack(winners)
+
+    def _aggregate_model(self, slots: torch.Tensor) -> List[torch.Tensor]:
+        """``--rule-scope model``: the rows of every tensor (worker slots, or the per-tensor vote winners), one choice from the
+        whole-model distances -- the per-tensor fp64 distances summed in ascending tensor order (``oracle.model_d2``) -- and
+        that choice applied to every tensor: Krum / multi-Krum rows, Bulyan's theta rows (then its per-tensor coordinate
+        stage), NNM neighbourhoods (then the rule on the mixed rows), the Weiszfeld weights, centered clipping's weights."""
+        plan, specs = self.plan, self.layout.specs
+        Xs = [slots[:, s.offset: s.offset + s.numel] for s in specs]
+        if plan.source == "detox":
+            Xs = [self._detox_rows(X) for X in Xs]
+        if plan.base == "centered_clip":
+            vs = [self.cc_center[s.offset: s.offset + s.numel] for s in specs]
+            d = model_d2([(X.double() - v.double()).pow(2).sum(1).cpu().numpy() for X, v in zip(Xs, vs)])
+            w = [centered_clip_weight(float(di), self.cfg.clip_tau, plan.rows) for di in d]
+            return [self._centered_clip_tensor(X, v, w) for X, v in zip(Xs, vs)]
+        D = model_d2([_pair_d2(X) for X in Xs])
+        if plan.source == "nnm":
+            A = nnm_neighbours_d2(D, plan.f)
+            nbrs = [[int(j) for j in np.flatnonzero(a)] for a in A]
+            Xs = [self._mix_rows(X, nbrs, plan.f) for X in Xs]
+            if plan.base in ("median", "trimmed_mean"):
+                return [self._trimmed_mean_tensor(X) for X in Xs]
+            D = nnm_pair_d2(D, A, plan.f)
+        if plan.base in ("krum", "multi_krum"):
+            best = np.argsort(_krum_scores_d2(D, plan.f), kind="stable")[:plan.m].tolist()
+            return [X[best[0]] if plan.base == "krum" else X[best].sum(0) / plan.m for X in Xs]
+        if plan.base == "bulyan":
+            chosen = _bulyan_rounds(D, plan.f)
+            return [self._nearest_to_median_mean(X[chosen], plan.f) for X in Xs]
+        # geometric median: the Weiszfeld weights of the concatenated rows, fp32 as the fused update applies them
+        w = torch.from_numpy(_weiszfeld_weights(D, 1e-10, 256)).float().to(slots.device)
+        return [(w[:, None] * X).sum(0) for X in Xs]
+
     def step(self, slots: torch.Tensor) -> None:
         self.apply(self.aggregate(slots))
 
     def apply(self, grads: List[torch.Tensor]) -> None:
         self.optimizer.step(grads=grads, mode=self.plan.opt_mode)
+
+
+def _pair_d2(X: torch.Tensor) -> np.ndarray:
+    """[P, P] fp64 squared distances between the rows of one tensor, from the fp32 values (diagonal 0)."""
+    X64 = X.double()
+    D = torch.stack([((X64 - X64[i]) ** 2).sum(1) for i in range(X.shape[0])]).cpu().numpy()
+    np.fill_diagonal(D, 0.0)                           # a row holding NaN or Inf is NaN off the diagonal only
+    return D
 
 
 def _fma_f32(w: float, b: torch.Tensor, c: torch.Tensor) -> torch.Tensor:
