@@ -16,9 +16,11 @@ struct UpdateArgs {
   int mode;                       // 0: select-sum over `select` table; 1: cyclic recombination; 2: real per-tensor weights;
                                   // 3: coordinate-wise trimmed mean over K rows (see `trim`);
                                   // 4: Bulyan's average of the K - 2 trim values nearest the coordinate median of K rows;
-                                  // 5: centered clipping, v + sum_k w[tensor][k] (g_k - v) around the centre `center`
-  const float* grad_in;           // mode 0: [P][slot_stride] fp32 ; mode 1: [n][2*slot_stride] complex64
-  long long slot_stride;          // elements (fp32 words for mode 0, complex elements for mode 1)
+                                  // 5: centered clipping, v + sum_k w[tensor][k] (g_k - v) around the centre `center`;
+                                  // 6: signSGD majority vote over the K = P sign rows (slots 0..K-1, K <= 32)
+  const float* grad_in;           // mode 0: [P][slot_stride] fp32 ; mode 1: [n][2*slot_stride] complex64 ;
+                                  // mode 6: [K][slot_stride] uint32 sign words (bit b of word w = element 32w + b is < 0)
+  long long slot_stride;          // elements (fp32 words for mode 0, complex elements for mode 1, uint32 sign words for mode 6)
   const int* select;              // modes 0, 2, 3: [K][T] worker slot to read for (k, tensor); null -> rows 0..K-1 for all
                                   // tensors.  DETOX: the vote's winner_slot table, so that the rule runs on the G group winners
   int K;                          // mode 0: rows summed per tensor ; mode 1: n workers
@@ -247,6 +249,35 @@ __device__ __forceinline__ float4 centered_clip_f4(const UpdateArgs& a, long lon
   return g;
 }
 
+// ---------------------------------------------------------------------------------------------
+// Mode 6: signSGD with majority vote (Bernstein et al., ICLR 2019; codes/oracle.py::sign_vote).  The thread's 4 coordinates are
+// bits 4(t % 8) .. 4(t % 8) + 3 of word idx / 32 of each of the K rows.  Per row the nibble is spread into 4 byte counters (bit e
+// to bit 8e: nibble * 0x00204081 & 0x01010101), so one add counts all 4 coordinates (K <= 32 fits a byte).  With n_neg rows
+// saying "-" and K - n_neg saying "+": g = +1 if "+" has the majority, -1 if "-" has it, +0 on a tie and on every padding
+// coordinate, whatever its bits say.
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ unsigned int ld_u32(const unsigned int* p) {   // coherent (data written by peers this step)
+  unsigned int v;
+  asm volatile("ld.global.L1::no_allocate.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+
+__device__ __forceinline__ float4 sign_vote_f4(const UpdateArgs& a, int tile) {
+  int tensor;
+  const int lane_valid = tile_valid(a.tv, tile, tensor) - (int)threadIdx.x * 4;
+  const unsigned int* words = reinterpret_cast<const unsigned int*>(a.grad_in) + (long long)tile * (DRC_TILE / 32) + (threadIdx.x >> 3);
+  const unsigned int shift = 4u * (threadIdx.x & 7u);
+  unsigned int neg = 0u;                                       // byte e: rows whose bit for coordinate e is 1 ("-")
+  for (int k = 0; k < a.K; ++k) neg += (((ld_u32(words + k * a.slot_stride) >> shift) & 0xFu) * 0x00204081u) & 0x01010101u;
+  float out[4];
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    const int n_neg = (int)((neg >> (8 * e)) & 0xFFu), n_pos = a.K - n_neg;
+    out[e] = e >= lane_valid ? 0.f : n_pos > n_neg ? 1.f : n_neg > n_pos ? -1.f : 0.f;
+  }
+  return make_float4(out[0], out[1], out[2], out[3]);
+}
+
 // SORT_N: modes 3 and 4, the sorting-network size (4, 8 or 16 >= K, or >= mixP with MIX).  Each size is its own instantiation so
 // that a launch pays the registers of its own network (4 x SORT_N keys per thread), not those of the largest one.  SEL: rows come
 // through the `select` table (DETOX's winners, Bulyan's choice); mode 3 without a table is its own instantiation, mode 4 always
@@ -289,6 +320,8 @@ __global__ void __launch_bounds__(DRC_THREADS) aggregate_update_kernel(const __g
       g = raw_robust_f4<MODE, SORT_N, SEL>(a, idx, tensor);
     } else if constexpr (MODE == 5) {
       g = centered_clip_f4(a, idx, tensor);
+    } else if constexpr (MODE == 6) {
+      g = sign_vote_f4(a, tile);
     } else {
       for (int k = 0; k < a.K; ++k) {
         const float2 v = a.recomb[tensor * a.K + k];
@@ -301,7 +334,7 @@ __global__ void __launch_bounds__(DRC_THREADS) aggregate_update_kernel(const __g
         g.w += v.x * c1.z - v.y * c1.w;
       }
     }
-    if constexpr (MODE != 5) { g.x *= a.scale; g.y *= a.scale; g.z *= a.scale; g.w *= a.scale; }
+    if constexpr (MODE != 5 && MODE != 6) { g.x *= a.scale; g.y *= a.scale; g.z *= a.scale; g.w *= a.scale; }
     if (a.grad_out) *reinterpret_cast<float4*>(a.grad_out + idx) = g;
 
     float4 p = *reinterpret_cast<const float4*>(a.params + idx);
@@ -370,6 +403,12 @@ extern "C" int drc_aggregate_update(const UpdateArgs* args, int grid, cudaStream
   if (mode == 5) {
     if (K < 1 || K > TRIM_MAXP || !args->recomb || !args->center || args->mix) return (int)cudaErrorInvalidValue;
     aggregate_update_kernel<5><<<grid, DRC_THREADS, 0, stream>>>(*args);
+    return (int)cudaGetLastError();
+  }
+  // signSGD majority vote: K = P <= 32 sign rows in slots 0..K-1 (the adversary bitmaps' width), no row table
+  if (mode == 6) {
+    if (K < 1 || K > DRC_MAX_WORKERS || args->select || args->mix) return (int)cudaErrorInvalidValue;
+    aggregate_update_kernel<6><<<grid, DRC_THREADS, 0, stream>>>(*args);
     return (int)cudaGetLastError();
   }
   // nearest-neighbour mixing: modes 3 (K = mixP mixed rows, no row table) and 4 (K = theta mixed rows named by `select`)

@@ -38,6 +38,9 @@ struct PushArgs {
   float* wmom;
   float wm_beta;
   float wm_scale;
+  // signSGD wire (push_encode_sign*_kernel; appended): dst / local_copy are uint32 words, word w = elements 32w..32w+31 of the
+  // slot's element layout, bit b (LSB = 0) = 1 iff element 32w + b is < 0 after momentum and the adversary hook; padding bits 0
+  int sign;
 };
 
 // counter-based normal generator (Philox-lite: 2 rounds of a 64-bit mix, Box-Muller) keyed by (seed, step, worker, idx)
@@ -77,8 +80,45 @@ __device__ __forceinline__ float4 load_grad4(const PushArgs& a, int k, int tenso
   return ld_stream_f4(reinterpret_cast<const float4*>(a.g32[k] + idx));
 }
 
-// The tile loop of the push; returns the step it pushed.  WMOM: the worker-momentum build.
+// The value a non-cyclic push sends for the thread's 4 elements: the gradient, advanced into the worker's momentum with WMOM,
+// then through the adversary hook
 template <bool WMOM>
+__device__ __forceinline__ float4 push_value(const PushArgs& a, bool lie, unsigned long long key, int tensor, int is_bf16,
+                                             long long idx, int lane_valid) {
+  float4 g = load_grad4(a, 0, tensor, is_bf16, idx, lane_valid);
+  if constexpr (WMOM) {
+    // no FMA: the library-op PS and the oracle (codes/oracle.py worker_momentum) round the two products separately
+    float4* mp = reinterpret_cast<float4*>(a.wmom + idx);
+    float4 m = *mp;
+    m.x = __fadd_rn(__fmul_rn(a.wm_beta, m.x), __fmul_rn(a.wm_scale, g.x));
+    m.y = __fadd_rn(__fmul_rn(a.wm_beta, m.y), __fmul_rn(a.wm_scale, g.y));
+    m.z = __fadd_rn(__fmul_rn(a.wm_beta, m.z), __fmul_rn(a.wm_scale, g.z));
+    m.w = __fadd_rn(__fmul_rn(a.wm_beta, m.w), __fmul_rn(a.wm_scale, g.w));
+    *mp = m;
+    g = m;
+  }
+  if (lie) {
+    if (a.attack == 1) { g.x *= a.magnitude; g.y *= a.magnitude; g.z *= a.magnitude; g.w *= a.magnitude; }
+    else if (a.attack == 2) { g = make_float4(a.magnitude, a.magnitude, a.magnitude, a.magnitude); }
+    else if (a.attack == 3) {
+      float2 n0 = normal_pair(key, (unsigned long long)idx), n1 = normal_pair(key, (unsigned long long)idx + 2);
+      float m = fabsf(a.magnitude);
+      g = make_float4(m * n0.x, m * n0.y, m * n1.x, m * n1.y);
+    }
+    // padding must stay zero so that per-tensor rules never see it
+    if (lane_valid < 4) {
+      if (lane_valid < 1) g.x = 0.f;
+      if (lane_valid < 2) g.y = 0.f;
+      if (lane_valid < 3) g.z = 0.f;
+      g.w = 0.f;
+    }
+  }
+  return g;
+}
+
+// The tile loop of the push; returns the step it pushed.  WMOM: the worker-momentum build.  SIGN: the signSGD build, which
+// sends one bit per element (PushArgs::sign).
+template <bool WMOM, bool SIGN = false>
 __device__ __forceinline__ unsigned long long push_encode_tiles(const PushArgs& a) {
   const unsigned long long step = *a.step_ptr;
   const bool lie = a.attack != 0 && a.adv_len > 0 &&
@@ -95,36 +135,32 @@ __device__ __forceinline__ unsigned long long push_encode_tiles(const PushArgs& 
     const int is_bf16 = a.tv.meta[tensor].is_bf16;
     const long long idx = (long long)tile * DRC_TILE + threadIdx.x * 4;
     const int lane_valid = valid - (int)threadIdx.x * 4;      // elements of this thread that are real
-    if (WMOM || !a.cyclic) {   // the momentum build has no cyclic path
+    if constexpr (SIGN) {
+      // Thread t holds bits 4(t % 8) .. 4(t % 8) + 3 of word t / 8 of the tile, so the 8 lanes of a lane octet fill one word
+      // and a warp's 4 words are 16 contiguous bytes.  Every lane joins the shuffles: padding lanes contribute 0 bits.
+      unsigned int bits = 0u;
+      if (!(a.src_table && lane_valid <= 0)) {
+        const float4 g = push_value<WMOM>(a, lie, key, tensor, is_bf16, idx, lane_valid);
+        bits = (unsigned int)(g.x < 0.f) | ((unsigned int)(g.y < 0.f) << 1) | ((unsigned int)(g.z < 0.f) << 2) |
+               ((unsigned int)(g.w < 0.f) << 3);
+        if (lane_valid < 4) bits &= lane_valid > 0 ? (1u << lane_valid) - 1u : 0u;
+      }
+      const unsigned int lane = threadIdx.x & 31u;
+      unsigned int word = bits << (4u * (lane & 7u));
+      word |= __shfl_xor_sync(0xffffffffu, word, 1);
+      word |= __shfl_xor_sync(0xffffffffu, word, 2);
+      word |= __shfl_xor_sync(0xffffffffu, word, 4);
+      const unsigned int w1 = __shfl_sync(0xffffffffu, word, 8), w2 = __shfl_sync(0xffffffffu, word, 16),
+                         w3 = __shfl_sync(0xffffffffu, word, 24);
+      if (lane == 0) {
+        const uint4 q = make_uint4(word, w1, w2, w3);
+        const long long widx = (long long)tile * (DRC_TILE / 32) + (threadIdx.x >> 5) * 4;   // this warp's 4 words
+        st_f4(reinterpret_cast<float4*>(reinterpret_cast<unsigned int*>(a.dst) + widx), *reinterpret_cast<const float4*>(&q));
+        if (a.local_copy) *reinterpret_cast<uint4*>(reinterpret_cast<unsigned int*>(a.local_copy) + widx) = q;
+      }
+    } else if (WMOM || !a.cyclic) {   // the momentum build has no cyclic path
       if (a.src_table && lane_valid <= 0) continue;             // padding of the slab stays zero, nothing to send
-      float4 g = load_grad4(a, 0, tensor, is_bf16, idx, lane_valid);
-      if constexpr (WMOM) {
-        // no FMA: the library-op PS and the oracle (codes/oracle.py worker_momentum) round the two products separately
-        float4* mp = reinterpret_cast<float4*>(a.wmom + idx);
-        float4 m = *mp;
-        m.x = __fadd_rn(__fmul_rn(a.wm_beta, m.x), __fmul_rn(a.wm_scale, g.x));
-        m.y = __fadd_rn(__fmul_rn(a.wm_beta, m.y), __fmul_rn(a.wm_scale, g.y));
-        m.z = __fadd_rn(__fmul_rn(a.wm_beta, m.z), __fmul_rn(a.wm_scale, g.z));
-        m.w = __fadd_rn(__fmul_rn(a.wm_beta, m.w), __fmul_rn(a.wm_scale, g.w));
-        *mp = m;
-        g = m;
-      }
-      if (lie) {
-        if (a.attack == 1) { g.x *= a.magnitude; g.y *= a.magnitude; g.z *= a.magnitude; g.w *= a.magnitude; }
-        else if (a.attack == 2) { g = make_float4(a.magnitude, a.magnitude, a.magnitude, a.magnitude); }
-        else if (a.attack == 3) {
-          float2 n0 = normal_pair(key, (unsigned long long)idx), n1 = normal_pair(key, (unsigned long long)idx + 2);
-          float m = fabsf(a.magnitude);
-          g = make_float4(m * n0.x, m * n0.y, m * n1.x, m * n1.y);
-        }
-        // padding must stay zero so that per-tensor rules never see it
-        if (lane_valid < 4) {
-          if (lane_valid < 1) g.x = 0.f;
-          if (lane_valid < 2) g.y = 0.f;
-          if (lane_valid < 3) g.z = 0.f;
-          g.w = 0.f;
-        }
-      }
+      const float4 g = push_value<WMOM>(a, lie, key, tensor, is_bf16, idx, lane_valid);
       st_f4(reinterpret_cast<float4*>(a.dst + idx), g);
       if (a.local_copy) *reinterpret_cast<float4*>(a.local_copy + idx) = g;
     } else if constexpr (!WMOM) {
@@ -178,8 +214,21 @@ __global__ void __launch_bounds__(DRC_THREADS) push_encode_wmom_kernel(const __g
   }
 }
 
+// the signSGD builds (--mode sign_vote): one bit per element, plain and with worker momentum (Signum)
+template <bool WMOM>
+__global__ void __launch_bounds__(DRC_THREADS) push_encode_sign_kernel(const __grid_constant__ PushArgs a) {
+  const unsigned long long step = push_encode_tiles<WMOM, true>(a);
+  if (grid_last_cta(a.done_counter)) {
+    if (threadIdx.x == 0 && a.flag) st_release_sys(a.flag, step);
+  }
+}
+
 extern "C" int drc_push_encode(const PushArgs* args, int grid, cudaStream_t stream) {
-  if (args->wmom) {
+  if (args->sign) {
+    if (args->cyclic) return (int)cudaErrorInvalidValue;
+    if (args->wmom) push_encode_sign_kernel<true><<<grid, DRC_THREADS, 0, stream>>>(*args);
+    else push_encode_sign_kernel<false><<<grid, DRC_THREADS, 0, stream>>>(*args);
+  } else if (args->wmom) {
     if (args->cyclic) return (int)cudaErrorInvalidValue;
     push_encode_wmom_kernel<<<grid, DRC_THREADS, 0, stream>>>(*args);
   } else {

@@ -53,7 +53,7 @@ class PushArgs(C.Structure):
                 ("adv_len", C.c_int), ("step_ptr", ptr), ("worker", C.c_int), ("attack", C.c_int),
                 ("magnitude", C.c_float), ("seed", u64), ("done_counter", ptr), ("flag", ptr), ("local_copy", ptr),
                 ("tile_begin", C.c_int), ("tile_end", C.c_int), ("src_table", ptr), ("wmom", ptr), ("wm_beta", C.c_float),
-                ("wm_scale", C.c_float)]
+                ("wm_scale", C.c_float), ("sign", C.c_int)]
 
 
 class OmniArgs(C.Structure):

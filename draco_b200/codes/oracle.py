@@ -11,6 +11,7 @@ distances.
 
 ``worker_momentum`` is the one worker-side rule here, and it is fp32 on purpose: every path must produce its exact bits.
 ``centered_clip`` is fp64 where it measures (the distances, the weights) and fp32 where it combines rows, for the same reason.
+``sign_pack`` / ``sign_vote`` (signSGD with majority vote) are exact integer arithmetic on the signs of fp32 values.
 """
 from __future__ import annotations
 
@@ -475,3 +476,40 @@ def centered_clip(rows: np.ndarray, center: np.ndarray, tau: float, weights=None
             if w[i] != 0:
                 acc = fma_f32(w[i], np.subtract(X[i], v, dtype=np.float32), acc)
         return np.add(v, acc, dtype=np.float32)
+
+
+def sign_pack(x: np.ndarray, valid=None) -> np.ndarray:
+    """The signSGD wire of fp32 values ``x`` [..., n] (n a multiple of 32, in the slot's element layout): uint32 words
+    [..., n / 32] with bit b (LSB = 0) of word w equal to 1 iff x[32 w + b] < 0.  So +0, -0, NaN and +Inf send 0 ("+").
+    ``valid`` (bool [n], the arena's valid mask): padding bits are 0 whatever ``x`` holds there.  Signum is this applied to
+    ``worker_momentum``'s output.  The library transports send the little-endian bytes of these words
+    (``sign_pack(x).view(np.uint8)``): byte i, bit b is element 8 i + b."""
+    x = np.asarray(x, dtype=np.float32)
+    if x.shape[-1] % 32:
+        raise ValueError(f"sign_pack: the last axis must be a multiple of 32, got {x.shape[-1]}")
+    with np.errstate(invalid="ignore"):
+        neg = x < 0
+    if valid is not None:
+        neg = neg & np.asarray(valid, dtype=bool)
+    bits = neg.reshape(*x.shape[:-1], x.shape[-1] // 32, 32).astype(np.uint64)
+    return (bits << np.arange(32, dtype=np.uint64)).sum(axis=-1).astype(np.uint32)
+
+
+def sign_unpack(words: np.ndarray) -> np.ndarray:
+    """uint32 sign words [..., m] -> uint8 bits [..., 32 m] (``sign_pack``'s layout; 1 = "-")."""
+    w = np.asarray(words, dtype=np.uint32)
+    bits = (w[..., None] >> np.arange(32, dtype=np.uint32)) & np.uint32(1)
+    return bits.reshape(*w.shape[:-1], w.shape[-1] * 32).astype(np.uint8)
+
+
+def sign_vote(bits: np.ndarray, P: int, valid) -> np.ndarray:
+    """signSGD with majority vote (Bernstein, Zhao, Azizzadenesheli and Anandkumar, ICLR 2019) over the sign bits [P, n] of
+    the P workers: per coordinate n_neg = rows with bit 1 and n_pos = P - n_neg; g = +1 if n_pos > n_neg, -1 if n_neg > n_pos,
+    +0 on a tie, and +0 on every padding coordinate (``valid`` False) whatever its bits say.  fp32 [n]."""
+    b = np.asarray(bits, dtype=np.int64)
+    if b.ndim != 2 or b.shape[0] != P:
+        raise ValueError(f"sign_vote: expected [{P}, n] bits, got {b.shape}")
+    n_neg = b.sum(axis=0)
+    n_pos = P - n_neg
+    g = np.where(n_pos > n_neg, 1.0, np.where(n_neg > n_pos, -1.0, 0.0)).astype(np.float32)
+    return np.where(np.asarray(valid, dtype=bool), g, np.float32(0.0)).astype(np.float32)

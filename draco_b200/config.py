@@ -13,10 +13,11 @@ from typing import Optional
 
 APPROACHES = ("baseline", "maj_vote", "cyclic", "detox", "nnm")
 MODES = ("normal", "geometric_median", "krum", "maj_vote", "coordinate_median", "trimmed_mean", "multi_krum", "bulyan",
-         "centered_clip")
+         "centered_clip", "sign_vote")
 DETOX_MODES = ("coordinate_median", "trimmed_mean", "multi_krum", "geometric_median", "bulyan", "centered_clip")
 NNM_MODES = ("coordinate_median", "trimmed_mean", "krum", "multi_krum", "geometric_median", "bulyan")
 ROBUST_MAXP = 16                    # workers the fused coordinate-wise / Krum / Bulyan kernels take (TRIM_MAXP, KRUM_MAXP)
+SIGN_VOTE_MAXP = 32                 # workers the fused sign vote takes: the adversary bitmaps are 32-bit (DRC_MAX_WORKERS)
 ERR_MODES = ("rev_grad", "constant", "random", "omniscient", "alie", "minmax", "none")
 TRANSPORTS = ("nvl", "nccl", "nccl_flat", "gloo")
 SCOPES = ("tensor", "model")        # --rule-scope / --attack-scope: distances per parameter tensor, or over the whole model
@@ -114,6 +115,7 @@ class JobConfig:
                                  f"divides num_workers more evenly")
         if self.no_cuda:
             self.transport = "gloo"
+        self._check_sign_vote()
         if self.approach == "baseline" and self.mode in ("coordinate_median", "trimmed_mean", "multi_krum", "bulyan"):
             P = self.num_workers
             self._check_rule_bounds(f"--mode {self.mode}")
@@ -206,6 +208,29 @@ class JobConfig:
         if self.transport == "nccl_flat":
             raise ValueError("--transport nccl_flat runs the plain mean and the vote only; use --transport nccl for "
                              "--mode centered_clip")
+
+    def _check_sign_vote(self) -> None:
+        """--mode sign_vote: every worker sends one bit per coordinate (its sign) and the PS takes the coordinate-wise majority."""
+        if self.mode != "sign_vote":
+            return
+        if self.approach != "baseline":
+            raise ValueError(f"--mode sign_vote votes over the signs of the P workers' rows: use --approach baseline (got "
+                             f"--approach {self.approach})")
+        if self.err_mode in ("omniscient", "alie", "minmax"):
+            raise ValueError(f"--err-mode {self.err_mode} builds a real-valued row from the honest workers' fp32 slots, and the sign "
+                             f"wire has none: use --err-mode rev_grad | constant | random | none with --mode sign_vote")
+        if self.compress:
+            raise ValueError("--mode sign_vote sends 1-bit words of signs, which the lossless codec cannot shrink: pass "
+                             "--compress-grad None")
+        if self.transport == "nccl_flat":
+            raise ValueError("--transport nccl_flat runs the plain mean and the vote only; use --transport nccl for "
+                             "--mode sign_vote")
+        if 2 * self.worker_fail >= self.num_workers:
+            raise ValueError(f"--mode sign_vote needs the honest rows to be a strict majority, num_workers > 2*worker_fail (got "
+                             f"{self.num_workers} workers, worker_fail {self.worker_fail})")
+        if self.transport == "nvl" and self.num_workers > SIGN_VOTE_MAXP:
+            raise ValueError(f"--mode sign_vote on the nvl transport handles at most {SIGN_VOTE_MAXP} workers (got "
+                             f"{self.num_workers}); use --transport nccl for more")
 
     def _check_scope(self) -> None:
         """--rule-scope / --attack-scope model: the rule's distances, or min-max's gamma and Dmax, over the whole model."""
@@ -353,7 +378,10 @@ def add_fit_args(parser: argparse.ArgumentParser) -> argparse.ArgumentParser:
            "4 worker_fail + 3; detox: G and b_G); coordinate_median | trimmed_mean | krum | multi_krum | geometric_median | "
            "bulyan (nnm: the rule applied to the mixed rows, with --worker-fail as f).  centered_clip (baseline, detox; needs "
            "--clip-tau): one step of centered clipping around last step's aggregate v, g = v + (1/n) sum_i (x_i - v) min(1, "
-           "tau / ||x_i - v||) per tensor, and g becomes the next v")
+           "tau / ||x_i - v||) per tensor, and g becomes the next v.  sign_vote (baseline; needs --compress-grad None): signSGD "
+           "with majority vote, every worker sends one bit per coordinate (its sign) and the PS applies the coordinate-wise "
+           "majority sign (+1 / -1, 0 on a tie) through the optimizer, so --lr is the sign step; with --worker-momentum 0.9 "
+           "--momentum 0 it is Signum")
     a("--dataset", type=str, default=d.dataset)
     a("--comm-type", type=str, default=d.comm_type)
     a("--err-mode", type=str, default=d.err_mode,

@@ -58,11 +58,15 @@ def push_encode(layout: ArenaLayout, g32: Sequence[Addr], g16: Sequence[Addr], d
                 worker: int, done_counter: Addr, flag: Addr = None, coef: Optional[Sequence[complex]] = None,
                 adv_bitmap: Addr = None, adv_len: int = 0, attack: int = 0, magnitude: float = -100.0, seed: int = 428,
                 local_copy: Addr = None, grid: Optional[int] = None, tile_range: Optional[tuple] = None,
-                src_table: Addr = None, wmom: Addr = None, wm_beta: float = 0.0) -> None:
+                src_table: Addr = None, wmom: Addr = None, wm_beta: float = 0.0, sign: bool = False) -> None:
     """Fused encode + adversary + store into ``dst`` (a peer pointer) + release flag.  ``coef`` given => cyclic encode
     of ``len(coef)`` gradient streams into an interleaved complex64 slot.  ``tile_range=(t0, t1)`` pushes one bucket.
     ``wmom``: this worker's fp32 momentum arena; the push then advances it, m <- fp32(wm_beta) m + fp32(1 - wm_beta) g
-    (codes/oracle.py ``worker_momentum``), and sends m (through the adversary hook) instead of g."""
+    (codes/oracle.py ``worker_momentum``), and sends m (through the adversary hook) instead of g.
+    ``sign``: the signSGD wire (codes/oracle.py ``sign_pack``).  ``dst`` and ``local_copy`` are then ``layout.total / 32``
+    uint32 words: bit b of word w is 1 iff element 32w + b of what the plain push would store is < 0; padding bits are 0."""
+    if sign and coef is not None:
+        raise ValueError("the sign wire is not defined for the cyclic encode (coef)")
     if wmom is not None:
         if coef is not None:
             raise ValueError("worker momentum is not defined for the cyclic encode (coef)")
@@ -106,6 +110,7 @@ def push_encode(layout: ArenaLayout, g32: Sequence[Addr], g16: Sequence[Addr], d
         from ..codes.oracle import worker_momentum_coefficients
         a.wmom = addr(wmom)
         a.wm_beta, a.wm_scale = worker_momentum_coefficients(wm_beta)
+    a.sign = 1 if sign else 0
     ntiles = layout.ntiles
     if tile_range is not None:
         a.tile_begin, a.tile_end = int(tile_range[0]), int(tile_range[1])
@@ -322,6 +327,29 @@ def _launch_update(a: N.UpdateArgs, layout: ArenaLayout, grad_in: Addr, slot_str
         a.tile_begin, a.tile_end = int(tile_range[0]), int(tile_range[1])
         ntiles = a.tile_end - a.tile_begin
     N.check(N.cuda().drc_aggregate_update(C.byref(a), grid or max(1, min(ntiles, sm_count() * 8)), _stream()), "aggregate_update")
+
+
+SIGN_VOTE_MAXP = N.MAX_WORKERS
+
+
+def sign_vote_update(layout: ArenaLayout, grad_in: Addr, slot_stride: int, *, P: int, params: Addr, momentum: Addr, hp: Addr,
+                     step_ptr: Addr, done_counter: Addr, first_step: int = 1, grad_out: Addr = None, mc_params: Addr = None,
+                     dst: Sequence[Addr] = (), flags: Sequence[Addr] = (), grid: Optional[int] = None,
+                     tile_range: Optional[tuple] = None, exp_avg_sq: Addr = None, max_exp_avg_sq: Addr = None) -> None:
+    """signSGD with majority vote (update-kernel mode 6, codes/oracle.py ``sign_vote``) + the unchanged optimizer step,
+    broadcast and flags.  ``grad_in``: the P <= 32 sign rows of ``push_encode(sign=True)`` in slots 0..P-1, ``slot_stride``
+    uint32 words apart (at least ``layout.total / 32``).  Per coordinate g = +1 if more rows say "+" than "-", -1 if more say
+    "-", +0 on a tie and on padding; g enters the optimizer with scale 1."""
+    if not 1 <= P <= SIGN_VOTE_MAXP:
+        raise ValueError(f"sign vote: takes 1..{SIGN_VOTE_MAXP} rows (the adversary bitmaps' width), got {P}")
+    if slot_stride < layout.total // 32:
+        raise ValueError(f"sign vote: slot_stride is in uint32 words and must hold a slot of {layout.total // 32}, got {slot_stride}")
+    a = N.UpdateArgs()
+    a.mode = 6
+    _launch_update(a, layout, grad_in, slot_stride, select=None, K=P, scale=1.0, recomb=None, params=params,
+                   momentum=momentum, exp_avg_sq=exp_avg_sq, max_exp_avg_sq=max_exp_avg_sq, hp=hp, step_ptr=step_ptr,
+                   first_step=first_step, grad_out=grad_out, mc_params=mc_params, dst=dst, done_counter=done_counter, flags=flags,
+                   tile_range=tile_range, grid=grid)
 
 
 # ------------------------------------------------------------------------------------------------ centered clipping (C13)

@@ -18,7 +18,7 @@ import numpy as np
 import torch
 
 _MODES = ("normal", "geometric_median", "maj_vote", "cyclic", "krum", "coordinate_median", "trimmed_mean", "multi_krum",
-          "bulyan", "centered_clip")
+          "bulyan", "centered_clip", "sign_vote")
 
 
 def _as_tensor(g, like: torch.Tensor) -> torch.Tensor:

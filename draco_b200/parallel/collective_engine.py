@@ -9,7 +9,8 @@ baseline -- the unmodified reference cannot run here (Python 2.7 / torch 0.3 / m
 * encode / adversary / (optional) compression are separate passes over the gradient
 
 Only the communication library differs: NCCL (or Gloo) point-to-point and broadcast instead of mpi4py.  Wire dtype is
-fp32 (complex64 for the cyclic code); ``--compress-grad compress`` runs the C++ lossless codec on the CPU path.
+fp32 (complex64 for the cyclic code, one bit per coordinate for ``--mode sign_vote``); ``--compress-grad compress`` runs the
+C++ lossless codec on the CPU path.
 """
 from __future__ import annotations
 
@@ -65,9 +66,16 @@ class CollectiveEngine:
         self.worker_momentum: Dict[int, torch.Tensor] = (
             {w: self.layout.new_arena(self.device) for w in self.local_workers} if cfg.worker_momentum > 0 else {})
         self._wm_b, self._wm_c = worker_momentum_coefficients(cfg.worker_momentum)
+        # --mode sign_vote: each worker packs its encoded, corrupted buffer into sign bytes (byte i, bit b = element 8 i + b is
+        # < 0; oracle.sign_pack's words read as little-endian bytes) and only those bytes travel
+        self.sign = cfg.mode == "sign_vote"
+        self.signbuf = ({w: torch.zeros(self.layout.total // 8, dtype=torch.uint8, device=self.device) for w in self.local_workers}
+                        if self.sign else {})
+        self._valid = torch.from_numpy(self.layout.valid_mask()).to(self.device) if self.sign else None
         self.ps: Optional[TorchPS] = None
         if self.is_ps:
-            self.slots = torch.zeros(self.P, self.layout.total, dtype=wire, device=self.device)
+            self.slots = (torch.zeros(self.P, self.layout.total // 8, dtype=torch.uint8, device=self.device) if self.sign
+                          else torch.zeros(self.P, self.layout.total, dtype=wire, device=self.device))
             self.ps = TorchPS(cfg, self.layout, self.device, self.params_f32, self.groups, self.code)
         self.compress = cfg.compress and self.device.type == "cpu"
         self.compress_gpu = cfg.compress and self.device.type == "cuda"
@@ -119,6 +127,8 @@ class CollectiveEngine:
             buf.copy_(wc.flat_gradient(0))
         if self.use_adv and self.schedule.is_adversary(w, step):
             self._corrupt(buf, w, step)
+        if self.sign:
+            self.signbuf[w].copy_(sign_bytes(buf, self._valid))
         return buf
 
     def _corrupt(self, buf: torch.Tensor, w: int, step: int) -> None:
@@ -184,17 +194,20 @@ class CollectiveEngine:
         if self.compress_gpu and self.nprocs > 1:
             self._exchange_compressed_gpu(step)
             return
+        send = self.signbuf if self.sign else self.sendbuf
         for w in range(1, self.P + 1):
             src_proc = self.place.proc_of[w]
             if self.is_ps and src_proc == 0:
-                self.slots[w - 1].copy_(self.sendbuf[w])
+                self.slots[w - 1].copy_(send[w])
                 continue
             for s in L.specs:
+                # sign bytes: tensors start on a 1024-element boundary, so each one owns bytes [offset / 8, + ceil(numel / 8))
+                a, b = (s.offset // 8, s.offset // 8 + (s.numel + 7) // 8) if self.sign else (s.offset, s.offset + s.numel)
                 if self.is_ps:
-                    ops.append(dist.P2POp(dist.irecv, self.slots[w - 1, s.offset: s.offset + s.numel], src_proc, group=self.group))
+                    ops.append(dist.P2POp(dist.irecv, self.slots[w - 1, a: b], src_proc, group=self.group))
                 elif src_proc == self.rank:
-                    ops.append(dist.P2POp(dist.isend, self.sendbuf[w][s.offset: s.offset + s.numel], 0, group=self.group))
-                    self.bytes_up += s.numel * self.sendbuf[w].element_size()
+                    ops.append(dist.P2POp(dist.isend, send[w][a: b], 0, group=self.group))
+                    self.bytes_up += (b - a) * send[w].element_size()
         if ops:
             for r in dist.batch_isend_irecv(ops):
                 r.wait()
@@ -306,6 +319,13 @@ class CollectiveEngine:
 
     def close(self) -> None:
         pass
+
+
+def sign_bytes(x: torch.Tensor, valid: torch.Tensor) -> torch.Tensor:
+    """The sign wire of the fp32 arena ``x`` as uint8 [D / 8]: bit b of byte i is 1 iff element 8 i + b is < 0, and 0 wherever
+    ``valid`` (the arena's valid mask) is False -- the little-endian bytes of ``oracle.sign_pack``'s words."""
+    bits = ((x < 0) & valid).view(-1, 8).to(torch.uint8)
+    return (bits << torch.arange(8, dtype=torch.uint8, device=x.device)).sum(1, dtype=torch.uint8)
 
 
 def attack_row(H: torch.Tensor, mode: str, z: float = 0.0) -> torch.Tensor:

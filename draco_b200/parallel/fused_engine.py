@@ -71,6 +71,8 @@ class FusedEngine:
         self.groups, self.code = build_codes(cfg)
         self.cyclic = cfg.approach == "cyclic"
         self.esize = 8 if self.cyclic else 4
+        # --mode sign_vote: one bit per coordinate on the wire (push_encode(sign=True)), so a slot is D / 8 bytes
+        self.sign = cfg.mode == "sign_vote"
         self.step = 1                                   # host mirror of the device step counter
         self.kernels_per_step = 0
         self.graph: Optional[torch.cuda.CUDAGraph] = None
@@ -120,6 +122,7 @@ class FusedEngine:
         bf16 = cfg.dtype == "bf16"
         self.layout = ArenaLayout.from_model(model, bf16, channels_last=True)
         D = self.layout.total
+        self.slot_bytes = D // 8 if self.sign else D * self.esize
 
         # ---------------- symmetric regions -------------------------------------------------------------
         self.symm = SymmContext(device, rank, nprocs, group)
@@ -130,14 +133,14 @@ class FusedEngine:
         self.flagsA = regA.tensor[D * 4: D * 4 + FLAG_BYTES].view(torch.int64)
         self.params_ready_ptr = regA.ptr + D * 4
         if self.is_ps:
-            regB = self.symm.alloc("grad_in", self.P * D * self.esize + FLAG_BYTES)
-            self.grad_in = regB.tensor[: self.P * D * self.esize].view(torch.float32)
-            self.flagsB = regB.tensor[self.P * D * self.esize: self.P * D * self.esize + FLAG_BYTES].view(torch.int64)
+            regB = self.symm.alloc("grad_in", self.P * self.slot_bytes + FLAG_BYTES)
+            self.grad_in = regB.tensor[: self.P * self.slot_bytes].view(torch.float32)
+            self.flagsB = regB.tensor[self.P * self.slot_bytes: self.P * self.slot_bytes + FLAG_BYTES].view(torch.int64)
         all_procs = list(range(nprocs))
         mapA = self.symm.share("params", exporters=all_procs, importers=[0])
         mapB = self.symm.share("grad_in", exporters=[0], importers=all_procs)
         self.ps_grad_base = mapB[0].ptr
-        self.ps_flag_base = mapB[0].ptr + self.P * D * self.esize
+        self.ps_flag_base = mapB[0].ptr + self.P * self.slot_bytes
         self.codec = None
         if self.compress:
             from ..utils.codec import DeviceStreamCodec
@@ -193,7 +196,7 @@ class FusedEngine:
                               adv_bitmap=self.adv_bitmap, adv_len=len(sched.ranks))
             self.dst_ptrs = [mapA[p].ptr for p in self.place.worker_procs() if p != 0]
             self.param_flag_ptrs = [mapA[p].ptr + D * 4 for p in self.place.active_procs()]
-        self._dbg_buf = (torch.zeros(D * self.esize // 4, dtype=torch.float32, device=device)
+        self._dbg_buf = (torch.zeros(self.slot_bytes // 4, dtype=torch.float32, device=device)
                          if self.debug_checksum and self.local_workers else None)
         self._initial_broadcast()
 
@@ -249,7 +252,7 @@ class FusedEngine:
             dist.barrier(group=self.group)
 
     def slot_ptr(self, w: int) -> int:
-        return self.ps_grad_base + (w - 1) * self.layout.total * self.esize
+        return self.ps_grad_base + (w - 1) * self.slot_bytes
 
     def grad_flag_ptr(self, w: int, b: int = 0) -> int:
         return self.ps_flag_base + ((w - 1) * MAX_BUCKETS + b) * FLAG_STRIDE
@@ -406,7 +409,7 @@ class FusedEngine:
                        adv_bitmap=self.adv_bitmap, adv_len=len(self.schedule.ranks),
                        attack=self.attack if self.attack < ATTACK_OMNISCIENT else 0,    # 4..6: not the worker's doing
                        magnitude=cfg.attack_magnitude, seed=cfg.seed,
-                       src_table=wc.ptr_dev[w] if wc.zero_copy else None)
+                       src_table=wc.ptr_dev[w] if wc.zero_copy else None, sign=self.sign)
         if self.worker_momentum:
             push_kw.update(wmom=self.worker_momentum[w], wm_beta=cfg.worker_momentum,
                            local_copy=self._dbg_buf if self.debug_checksum else None)

@@ -36,7 +36,7 @@ def select_rule(cfg: JobConfig) -> str:
     (beyond the reference too) votes inside every group and runs ``--mode`` across the group winners: ``detox_*`` rules.  Bulyan
     (``--mode bulyan``) is beyond the reference as well, and so are centered clipping (``--mode centered_clip``, one step around
     last step's aggregate) and the nnm approach: nearest-neighbour mixing of the worker rows, then ``--mode`` on the mixed rows
-    (``nnm_*`` rules)."""
+    (``nnm_*`` rules), and signSGD with majority vote (``--mode sign_vote``), which works on the workers' sign bits."""
     if cfg.approach == "cyclic":
         return "cyclic"
     if cfg.approach == "maj_vote":
@@ -47,7 +47,7 @@ def select_rule(cfg: JobConfig) -> str:
         return NNM_RULES[cfg.mode]
     return {"normal": "mean", "geometric_median": "geomedian", "krum": "krum", "coordinate_median": "median",
             "trimmed_mean": "trimmed_mean", "multi_krum": "multi_krum", "bulyan": "bulyan",
-            "centered_clip": "centered_clip"}.get(cfg.mode, "mean")
+            "centered_clip": "centered_clip", "sign_vote": "sign_vote"}.get(cfg.mode, "mean")
 
 
 DETOX_RULES = {"coordinate_median": "detox_median", "trimmed_mean": "detox_trimmed_mean", "multi_krum": "detox_multi_krum",
@@ -61,12 +61,12 @@ NNM_RULES = {"coordinate_median": "nnm_median", "trimmed_mean": "nnm_trimmed_mea
 # tensors: buckets hold whole tensors, and centered clipping's centre is known before the step starts).  Only at the default
 # scopes: a whole-model distance, or min-max's whole-model gamma, needs every bucket first (RulePlan.pipelined)
 PIPELINED_RULES = ("mean", "vote", "median", "trimmed_mean", "detox_median", "detox_trimmed_mean", "centered_clip",
-                   "detox_centered_clip")
+                   "detox_centered_clip", "sign_vote")
 
 # the optimizer's mode string for each base rule (SGDModified / AdamModified.step(mode=))
 _OPT_MODE = {"mean": "normal", "vote": "maj_vote", "cyclic": "cyclic", "median": "coordinate_median", "trimmed_mean": "trimmed_mean",
              "krum": "krum", "multi_krum": "multi_krum", "geomedian": "geometric_median", "bulyan": "bulyan",
-             "centered_clip": "centered_clip"}
+             "centered_clip": "centered_clip", "sign_vote": "sign_vote"}
 
 
 @dataclass(frozen=True)
@@ -74,7 +74,8 @@ class RulePlan:
     """A job's aggregation rule as a row source and a base rule, with every parameter worked out once."""
     rule: str           # select_rule's name
     source: str         # raw: the P worker slots | detox: the G group winners of the vote | nnm: the P mixed rows
-    base: str           # mean | vote | cyclic | median | trimmed_mean | krum | multi_krum | geomedian | bulyan | centered_clip
+    base: str           # mean | vote | cyclic | median | trimmed_mean | krum | multi_krum | geomedian | bulyan | centered_clip |
+                        # sign_vote
     rows: int           # rows the base rule runs on: P, or G over the group winners
     f: int              # rows it tolerates: worker_fail, or b_G over the group winners
     trim: int           # median / trimmed mean: values dropped at each end of a coordinate
@@ -123,7 +124,7 @@ class FusedPS:
         self.cfg, self.layout, self.device = cfg, layout, device
         self.P = cfg.num_workers
         self.params = params                       # fp32 [D] master copy (inside the exported region)
-        self.grad_in = grad_in                     # fp32 [P, D] or complex64-as-fp32 [P, 2D]
+        self.grad_in = grad_in                     # fp32 [P, D], complex64-as-fp32 [P, 2D], or sign words [P, D / 32]
         self.momentum = layout.new_arena(device)             # SGD momentum buffer / Adam first moment
         # Adam / AMSGrad state lives in arenas too (checkpointed with the momentum: utils/checkpoint.py)
         self.exp_avg_sq = layout.new_arena(device) if cfg.optimizer == "adam" else None
@@ -132,8 +133,9 @@ class FusedPS:
         self.counters = torch.zeros(16, dtype=torch.int32, device=device)
         T = layout.ntensors
         self.cyclic = cfg.approach == "cyclic"
-        self.slot_stride = layout.total
         self.plan = plan = rule_plan(cfg)
+        # the sign wire packs 32 coordinates into one uint32 word (push_encode(sign=True)); the stride is then in words
+        self.slot_stride = layout.total // 32 if plan.base == "sign_vote" else layout.total
         self.rule = plan.rule
         # --err-mode alie | minmax: the liar slots of each bucket are overwritten after its flags and before its decode
         self.attack = attack_code(cfg.err_mode) if cfg.err_mode in PS_ATTACKS and adv_bitmap is not None else 0
@@ -246,6 +248,8 @@ class FusedPS:
             src, agg = self.grad_in, dict(K=plan.rows, select=rows)
             if plan.base in ("mean", "vote"):
                 agg.update(scale=1.0 / plan.rows)
+            elif plan.base == "sign_vote":                 # nothing to choose: the update kernel counts the signs
+                pass
             elif plan.base == "cyclic":
                 K.cyclic_project(L, self.grad_in, self.slot_stride, self.P, self.f, self.E); n += 1
                 K.cyclic_locate(self.E, self.P, self.cfg.worker_fail, self.recomb, self.healthy, self.flagged); n += 1
@@ -289,7 +293,10 @@ class FusedPS:
                 agg.update(mix=self.mix, mix_f=plan.f)
             if last:
                 n += before_update()
-            if plan.base == "centered_clip":               # the update reads and replaces the centre
+            if plan.base == "sign_vote":                   # the vote over the P sign rows is the update's gradient source
+                K.sign_vote_update(L, self.grad_in, self.slot_stride, P=plan.rows, tile_range=tiles, flags=flags if last else [],
+                                   **common)
+            elif plan.base == "centered_clip":             # the update reads and replaces the centre
                 K.centered_clip_update(L, src, self.slot_stride, center=self.cc_center, weights=self.cc_weights, K=plan.rows,
                                        select=rows, tile_range=tiles, flags=flags if last else [], **common)
             else:
@@ -521,12 +528,29 @@ class TorchPS:
         return (vt @ R).real / n
 
     # --- step -----------------------------------------------------------------------------------
+    def _sign_vote(self, slots: torch.Tensor) -> List[torch.Tensor]:
+        """``--mode sign_vote``: ``slots`` holds the P workers' sign bytes [P, D / 8] (byte i, bit b = element 8 i + b is < 0).
+        Per tensor, the majority sign of every coordinate (``oracle.sign_vote``): +1, -1, or +0 on a tie."""
+        P = self.P
+        shifts = torch.arange(8, dtype=torch.uint8, device=slots.device)
+        one = torch.ones((), dtype=torch.float32, device=slots.device)
+        out = []
+        for s in self.layout.specs:
+            b = slots[:, s.offset // 8: s.offset // 8 + (s.numel + 7) // 8]
+            bits = ((b[:, :, None] >> shifts) & 1).reshape(P, -1)[:, :s.numel]
+            n_neg = bits.sum(0, dtype=torch.int32)
+            n_pos = P - n_neg
+            out.append(torch.where(n_pos > n_neg, one, torch.where(n_neg > n_pos, -one, torch.zeros_like(one))))
+        return out
+
     def aggregate(self, slots: torch.Tensor) -> List[torch.Tensor]:
-        """``slots``: [P, D] fp32 (or [P, D] complex64 for cyclic).  Returns the per-tensor aggregated gradients: per tensor the
-        rows of the row source (the worker slots, the group winners of the vote, or the mixed rows), then the base rule's helper
-        on them."""
+        """``slots``: [P, D] fp32 (or [P, D] complex64 for cyclic, or [P, D / 8] sign bytes for sign_vote).  Returns the
+        per-tensor aggregated gradients: per tensor the rows of the row source (the worker slots, the group winners of the vote,
+        or the mixed rows), then the base rule's helper on them."""
         plan = self.plan
         self.last_info = {}
+        if plan.base == "sign_vote":
+            return self._sign_vote(slots)
         if plan.scope == "model":
             return self._aggregate_model(slots)
         out = []
