@@ -12,7 +12,12 @@
 //     cluster: safe next to any other kernel on any number of concurrent streams, and bit-deterministic (replicas of a batch
 //     on different GPUs must agree exactly for the majority vote, reference: src/master/rep_master.py:162).
 //
-// backward: bn_bwd_reduce_kernel (dy, y, x -> dgamma, dbeta, means)    bn_bwd_apply_kernel (dy, y, x -> dx, dres)
+// backward: bn_bwd_reduce_kernel (dy, mask, x -> dgamma, dbeta, means)    bn_bwd_apply_kernel (dy, mask, x -> dx, dres)
+//
+// ReLU mask: bn_apply_kernel also stores one bit per element (mask[M][C/8], bit = bf16 y > 0), so the backward reads one
+// byte per row and thread instead of the 16-byte y vector.  Downsampling blocks run their two BatchNorms
+// relu(bn2(c2) + bn_sc(s)) as one pass each way (bn_apply_kernel<true>, bn_bwd_reduce_kernel<3, true>,
+// bn_bwd_apply_dual_kernel): no y_sc or dres round trip through memory, and both layers' results equal the two-layer path's.
 //
 // Reference counterpart: nn.BatchNorm2d / F.relu inside src/model_ops/resnet.py:14-64 and vgg.py:46-59 (PyTorch-0.3 CPU).
 #include <cuda_bf16.h>
@@ -44,6 +49,17 @@ struct BnFwdArgs {
   int relu;
 };
 
+// bn_apply_kernel only (a parameter of its own: BnFwdArgs, which bn_stats_kernel takes too, stays as it was)
+struct BnApplyArgs {
+  uint8_t* mask;                  // optional [M][C/8]: bit i of byte (row, cv) = (bf16 y > 0) for channel 8*cv + i
+  // downsampling-block pair (bn_apply_kernel<true>): the residual is a second BatchNorm's output bf16(res * scale_s + shift_s),
+  // formed here from the raw shortcut convolution output in `res` instead of being read back from memory
+  const float* gamma_s;
+  const float* beta_s;
+  const float* mean_s;
+  const float* invstd_s;
+};
+
 struct BnBwdArgs {
   const __nv_bfloat16* dy;        // [M][C]
   const __nv_bfloat16* y;         // forward output (ReLU mask); null when relu == 0 -- or when the mask is recomputed from x
@@ -64,6 +80,16 @@ struct BnBwdArgs {
   int C;
   int rows_per_cta;
   int relu;
+  const uint8_t* mask;            // MASK == 3: the forward's ReLU bits [M][C/8]
+  // downsampling-block pair (dual kernels): the shortcut BatchNorm, whose input xs sees the same masked gradient dz
+  const __nv_bfloat16* xs;        // [M][C]
+  const float* gamma_s;
+  const float* mean_s;
+  const float* invstd_s;
+  __nv_bfloat16* dxs;             // [M][C]
+  float* dgamma_s;
+  float* dbeta_s;
+  float* sums_s;                  // [2][C]
 };
 
 __device__ __forceinline__ void unpack8(const uint4& v, float* f) {
@@ -88,19 +114,38 @@ __device__ __forceinline__ uint4 ldg16(const __nv_bfloat16* p) {
   return v;
 }
 
+// ReLU bits of one row's 8 channels as stored: bit i = (bf16 value i of v) > 0
+__device__ __forceinline__ uint32_t pos_bits8(const uint4& v) {
+  float f[BN_VEC];
+  unpack8(v, f);
+  uint32_t b = 0;
+#pragma unroll
+  for (int i = 0; i < BN_VEC; ++i) b |= (f[i] > 0.f ? 1u : 0u) << i;
+  return b;
+}
+__device__ __forceinline__ uint32_t ldg_u8(const uint8_t* p) {
+  uint16_t v;
+  asm volatile("ld.global.nc.L1::no_allocate.u8 %0, [%1];" : "=h"(v) : "l"(p));
+  return v;
+}
+// the shortcut BatchNorm's output value as the unpaired layer stores it: bf16(fma(x, scale, shift))
+__device__ __forceinline__ float bf16_round(float v) { return __bfloat162float(__float2bfloat16_rn(v)); }
+
 extern __shared__ __align__(16) float bn_smem[];
 
 // CTA-level fold of the per-thread accumulators acc[2][8] over the row groups, then this CTA's partial[2][C] (fixed order).
-__device__ __forceinline__ void cta_fold(const float (&acc)[2][BN_VEC], float* partial_blk, int C, int rgroups, int rg, int cv) {
-  // smem layout: [rgroups][2][C]  (rgroups * 2 * C == BN_THREADS * 16 floats = 32 KB)
+// NA accumulator rows (2, or 3 for the downsampling pair); every index is folded in the same order whatever NA is.
+template <int NA>
+__device__ __forceinline__ void cta_fold(const float (&acc)[NA][BN_VEC], float* partial_blk, int C, int rgroups, int rg, int cv) {
+  // smem layout: [rgroups][NA][C]  (rgroups * NA * C == BN_THREADS * 8 * NA floats = 16 KB * NA)
 #pragma unroll
-  for (int a = 0; a < 2; ++a) {
-    float4* dst = reinterpret_cast<float4*>(&bn_smem[(rg * 2 + a) * C + cv * BN_VEC]);
+  for (int a = 0; a < NA; ++a) {
+    float4* dst = reinterpret_cast<float4*>(&bn_smem[(rg * NA + a) * C + cv * BN_VEC]);
     dst[0] = make_float4(acc[a][0], acc[a][1], acc[a][2], acc[a][3]);
     dst[1] = make_float4(acc[a][4], acc[a][5], acc[a][6], acc[a][7]);
   }
   __syncthreads();
-  const int n_idx = 2 * C;
+  const int n_idx = NA * C;
   for (int idx = threadIdx.x; idx < n_idx; idx += BN_THREADS) {
     float s0 = 0.f, s1 = 0.f;
     int g = 0;
@@ -124,12 +169,15 @@ __device__ __forceinline__ bool last_cta(unsigned int* counter) {
   return s_last != 0;
 }
 
-// Grid-level fold by the last CTA: totals[idx] = sum_b partial[b][idx], idx in [0, 2C): 16-byte loads, the CTAs' partials split
-// into interleaved subsets that are combined in a fixed order.  Result in bn_smem[0 .. 2C).
-__device__ __forceinline__ void grid_fold(const float* partial, int C) {
+// Grid-level fold by the last CTA: totals[idx] = sum_b partial[b][first + idx], idx in [0, 2C), each CTA's partial NA * C floats:
+// 16-byte loads, the CTAs' partials split into interleaved subsets that are combined in a fixed order (which depends on C and
+// the grid only, so a 2C window of a 3-row partial folds exactly as a 2-row partial would).  Result in bn_smem[0 .. 2C).
+template <int NA>
+__device__ __forceinline__ void grid_fold(const float* partial, int C, int first = 0) {
   const int items4 = (2 * C) >> 2;
+  const int stride4 = (NA * C) >> 2;
   const int nblk = (int)gridDim.x;
-  const float4* p4 = reinterpret_cast<const float4*>(partial);
+  const float4* p4 = reinterpret_cast<const float4*>(partial + first);
   float4* s4 = reinterpret_cast<float4*>(bn_smem);
   __syncthreads();
   if (items4 <= BN_THREADS) {
@@ -143,7 +191,7 @@ __device__ __forceinline__ void grid_fold(const float* partial, int C) {
 #pragma unroll
         for (int u = 0; u < FB; ++u) {
           const int g = g0 + u * SUB;
-          v[u] = g < nblk ? __ldcg(p4 + (long long)g * items4 + item) : make_float4(0.f, 0.f, 0.f, 0.f);
+          v[u] = g < nblk ? __ldcg(p4 + (long long)g * stride4 + item) : make_float4(0.f, 0.f, 0.f, 0.f);
         }
 #pragma unroll
         for (int u = 0; u < FB; ++u) { t.x += v[u].x; t.y += v[u].y; t.z += v[u].z; t.w += v[u].w; }    // fixed order
@@ -164,24 +212,25 @@ __device__ __forceinline__ void grid_fold(const float* partial, int C) {
       float4 a0 = make_float4(0.f, 0.f, 0.f, 0.f), a1 = a0;
       int g = 0;
       for (; g + 1 < nblk; g += 2) {
-        const float4 v0 = __ldcg(p4 + (long long)g * items4 + item), v1 = __ldcg(p4 + (long long)(g + 1) * items4 + item);
+        const float4 v0 = __ldcg(p4 + (long long)g * stride4 + item), v1 = __ldcg(p4 + (long long)(g + 1) * stride4 + item);
         a0.x += v0.x; a0.y += v0.y; a0.z += v0.z; a0.w += v0.w;
         a1.x += v1.x; a1.y += v1.y; a1.z += v1.z; a1.w += v1.w;
       }
-      if (g < nblk) { const float4 v0 = __ldcg(p4 + (long long)g * items4 + item); a0.x += v0.x; a0.y += v0.y; a0.z += v0.z; a0.w += v0.w; }
+      if (g < nblk) { const float4 v0 = __ldcg(p4 + (long long)g * stride4 + item); a0.x += v0.x; a0.y += v0.y; a0.z += v0.z; a0.w += v0.w; }
       s4[item] = make_float4(a0.x + a1.x, a0.y + a1.y, a0.z + a1.z, a0.w + a1.w);
     }
   }
   __syncthreads();
 }
 
-// rows [r0, r1) of this CTA, row groups interleaved, BN_UNROLL independent rows in flight per thread
-#define BN_ROW_LOOP(BODY_LOAD, BODY_USE)                                                            \
+// rows [r0, r1) of this CTA, row groups interleaved, UNROLL independent rows in flight per thread
+#define BN_ROW_LOOP(BODY_LOAD, BODY_USE) BN_ROW_LOOP_U(BN_UNROLL, BODY_LOAD, BODY_USE)
+#define BN_ROW_LOOP_U(UNROLL, BODY_LOAD, BODY_USE)                                                  \
   {                                                                                                 \
     long long r = r0 + rg;                                                                          \
-    for (; r + (long long)(BN_UNROLL - 1) * rgroups < r1; r += (long long)BN_UNROLL * rgroups) {    \
-      _Pragma("unroll") for (int u = 0; u < BN_UNROLL; ++u) { const long long off = (r + (long long)u * rgroups) * a.C + cv * BN_VEC; BODY_LOAD }  \
-      _Pragma("unroll") for (int u = 0; u < BN_UNROLL; ++u) { const long long off = (r + (long long)u * rgroups) * a.C + cv * BN_VEC; BODY_USE }   \
+    for (; r + (long long)(UNROLL - 1) * rgroups < r1; r += (long long)UNROLL * rgroups) {          \
+      _Pragma("unroll") for (int u = 0; u < UNROLL; ++u) { const long long off = (r + (long long)u * rgroups) * a.C + cv * BN_VEC; BODY_LOAD }  \
+      _Pragma("unroll") for (int u = 0; u < UNROLL; ++u) { const long long off = (r + (long long)u * rgroups) * a.C + cv * BN_VEC; BODY_USE }   \
     }                                                                                               \
     for (; r < r1; r += rgroups) {                                                                  \
       const int u = 0; const long long off = r * a.C + cv * BN_VEC; BODY_LOAD BODY_USE              \
@@ -202,9 +251,9 @@ __global__ void __launch_bounds__(BN_THREADS, 2) bn_stats_kernel(const BnFwdArgs
       { xv[u] = ldg16(a.x + off); },
       { float f[BN_VEC]; unpack8(xv[u], f);
         _Pragma("unroll") for (int i = 0; i < BN_VEC; ++i) { acc[0][i] += f[i]; acc[1][i] = fmaf(f[i], f[i], acc[1][i]); } (void)off; })
-  cta_fold(acc, a.partial + (long long)blockIdx.x * 2 * a.C, a.C, rgroups, rg, cv);
+  cta_fold<2>(acc, a.partial + (long long)blockIdx.x * 2 * a.C, a.C, rgroups, rg, cv);
   if (last_cta(a.counter)) {
-    grid_fold(a.partial, a.C);
+    grid_fold<2>(a.partial, a.C);
     const float inv_m = 1.0f / (float)a.M;
     for (int c = threadIdx.x; c < a.C; c += BN_THREADS) {
       const float m = bn_smem[c] * inv_m;
@@ -223,48 +272,75 @@ __global__ void __launch_bounds__(BN_THREADS, 2) bn_stats_kernel(const BnFwdArgs
   }
 }
 
-__global__ void __launch_bounds__(BN_THREADS, 2) bn_apply_kernel(const BnFwdArgs a) {
+// Scale / shift per channel sit in shared memory (fwd_smem_bytes: [2][C] floats, [4][C] with DUAL), so the shortcut layer's
+// coefficients add no registers.
+// DUAL: y = relu?(bn(x) + bf16(bn_s(res))) for a downsampling block, the shortcut BatchNorm's output formed from its raw input.
+template <bool DUAL>
+__global__ void __launch_bounds__(BN_THREADS, 2) bn_apply_kernel(const BnFwdArgs a, const BnApplyArgs p) {
   const int tpc = a.C / BN_VEC;
   const int rgroups = BN_THREADS / tpc;
   const int cv = threadIdx.x % tpc, rg = threadIdx.x / tpc;
-  float scale[BN_VEC], shift[BN_VEC];
-#pragma unroll
-  for (int i = 0; i < BN_VEC; ++i) {
-    const int c = cv * BN_VEC + i;
+  for (int c = threadIdx.x; c < a.C; c += BN_THREADS) {
     const float sc = a.gamma[c] * a.invstd[c];
-    scale[i] = sc;
-    shift[i] = fmaf(-a.mean[c], sc, a.beta[c]);
+    bn_smem[c] = sc;
+    bn_smem[a.C + c] = fmaf(-a.mean[c], sc, a.beta[c]);
+    if (DUAL) {
+      const float scs = p.gamma_s[c] * p.invstd_s[c];
+      bn_smem[2 * a.C + c] = scs;
+      bn_smem[3 * a.C + c] = fmaf(-p.mean_s[c], scs, p.beta_s[c]);
+    }
   }
+  __syncthreads();
+  const float* scale = bn_smem + cv * BN_VEC;
+  const float* shift = scale + a.C;
+  const float* sc_s = shift + a.C;
+  const float* sh_s = sc_s + a.C;
   const long long r0 = (long long)blockIdx.x * a.rows_per_cta;
   long long r1 = r0 + a.rows_per_cta; if (r1 > a.M) r1 = a.M;
-  uint4 xv[BN_UNROLL], rv[BN_UNROLL];
+  constexpr int AU = DUAL ? 1 : 2;                                 // rows in flight per thread that fit 64 registers
+  uint4 xv[AU], rv[AU];
   const bool has_res = a.res != nullptr;
-  BN_ROW_LOOP(
+  BN_ROW_LOOP_U(AU,
       { xv[u] = ldg16(a.x + off); if (has_res) rv[u] = ldg16(a.res + off); },
       { float f[BN_VEC]; unpack8(xv[u], f);
         _Pragma("unroll") for (int i = 0; i < BN_VEC; ++i) f[i] = fmaf(f[i], scale[i], shift[i]);
-        if (has_res) { float g[BN_VEC]; unpack8(rv[u], g); _Pragma("unroll") for (int i = 0; i < BN_VEC; ++i) f[i] += g[i]; }
+        if (has_res) { float g[BN_VEC]; unpack8(rv[u], g);
+          if (DUAL) { _Pragma("unroll") for (int i = 0; i < BN_VEC; ++i) g[i] = bf16_round(fmaf(g[i], sc_s[i], sh_s[i])); }
+          _Pragma("unroll") for (int i = 0; i < BN_VEC; ++i) f[i] += g[i]; }
         if (a.relu) { _Pragma("unroll") for (int i = 0; i < BN_VEC; ++i) f[i] = fmaxf(f[i], 0.f); }
-        *reinterpret_cast<uint4*>(a.y + off) = pack8(f); })
+        const uint4 yv = pack8(f);
+        *reinterpret_cast<uint4*>(a.y + off) = yv;
+        if (p.mask) p.mask[off >> 3] = (uint8_t)pos_bits8(yv); })                  // off / 8 == row * C / 8 + cv
 }
 
 // MASK: 0 = no ReLU, 1 = ReLU mask from the saved output y, 2 = mask recomputed from x (specialised: the apply kernel has to fit
-// 64 registers for two CTAs per SM)
-template <int MASK>
+// 64 registers for two CTAs per SM), 3 = the forward's ReLU bits (one byte per row and thread instead of 16).
+// DUAL (MASK == 3): the downsampling pair -- a third accumulator row sum(dz * xhat_s) over the shortcut input xs, with the
+// same rows, order and grid as the unpaired layers, so both layers' dgamma / dbeta equal their separate reductions bit for bit.
+template <int MASK, bool DUAL = false>
 __global__ void __launch_bounds__(BN_THREADS) bn_bwd_reduce_kernel(const BnBwdArgs a) {
+  constexpr int NA = DUAL ? 3 : 2;
   const int tpc = a.C / BN_VEC;
   const int rgroups = BN_THREADS / tpc;
   const int cv = threadIdx.x % tpc, rg = threadIdx.x / tpc;
-  float mean[BN_VEC], istd[BN_VEC];
+  float mean[BN_VEC], istd[BN_VEC], mean_s[BN_VEC], istd_s[BN_VEC];
 #pragma unroll
   for (int i = 0; i < BN_VEC; ++i) { mean[i] = a.mean[cv * BN_VEC + i]; istd[i] = a.invstd[cv * BN_VEC + i]; }
+  if (DUAL) {
+#pragma unroll
+    for (int i = 0; i < BN_VEC; ++i) { mean_s[i] = a.mean_s[cv * BN_VEC + i]; istd_s[i] = a.invstd_s[cv * BN_VEC + i]; }
+  }
   const long long r0 = (long long)blockIdx.x * a.rows_per_cta;
   long long r1 = r0 + a.rows_per_cta; if (r1 > a.M) r1 = a.M;
-  float acc[2][BN_VEC];
+  float acc[NA][BN_VEC];
 #pragma unroll
-  for (int i = 0; i < BN_VEC; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
-  uint4 dv[BN_UNROLL], xv[BN_UNROLL], yv[BN_UNROLL];
-  constexpr bool relu_y = MASK == 1, relu_x = MASK == 2;
+  for (int i = 0; i < BN_VEC; ++i) {
+#pragma unroll
+    for (int k = 0; k < NA; ++k) acc[k][i] = 0.f;
+  }
+  uint4 dv[BN_UNROLL], xv[BN_UNROLL], yv[BN_UNROLL], sv[BN_UNROLL];
+  uint32_t mv[BN_UNROLL];
+  constexpr bool relu_y = MASK == 1, relu_x = MASK == 2, relu_b = MASK == 3;
   float sc[BN_VEC], sh[BN_VEC];
 #pragma unroll
   for (int i = 0; i < BN_VEC; ++i) {
@@ -272,14 +348,19 @@ __global__ void __launch_bounds__(BN_THREADS) bn_bwd_reduce_kernel(const BnBwdAr
     sh[i] = relu_x ? fmaf(-mean[i], sc[i], a.beta[cv * BN_VEC + i]) : 0.f;
   }
   BN_ROW_LOOP(
-      { dv[u] = ldg16(a.dy + off); xv[u] = ldg16(a.x + off); if (relu_y) yv[u] = ldg16(a.y + off); },
+      { dv[u] = ldg16(a.dy + off); xv[u] = ldg16(a.x + off); if (relu_y) yv[u] = ldg16(a.y + off);
+        if (relu_b) mv[u] = ldg_u8(a.mask + (off >> 3)); if (DUAL) sv[u] = ldg16(a.xs + off); },
       { float d[BN_VEC]; float xf[BN_VEC]; unpack8(dv[u], d); unpack8(xv[u], xf);
         if (relu_y) { float yf[BN_VEC]; unpack8(yv[u], yf); _Pragma("unroll") for (int i = 0; i < BN_VEC; ++i) d[i] = yf[i] > 0.f ? d[i] : 0.f; }
         if (relu_x) { _Pragma("unroll") for (int i = 0; i < BN_VEC; ++i) d[i] = relu_mask(xf[i], sc[i], sh[i]) ? d[i] : 0.f; }
-        _Pragma("unroll") for (int i = 0; i < BN_VEC; ++i) { acc[0][i] += d[i]; acc[1][i] = fmaf(d[i], (xf[i] - mean[i]) * istd[i], acc[1][i]); } (void)off; })
-  cta_fold(acc, a.partial + (long long)blockIdx.x * 2 * a.C, a.C, rgroups, rg, cv);
+        if (relu_b) { _Pragma("unroll") for (int i = 0; i < BN_VEC; ++i) d[i] = (mv[u] >> i) & 1u ? d[i] : 0.f; }
+        _Pragma("unroll") for (int i = 0; i < BN_VEC; ++i) { acc[0][i] += d[i]; acc[1][i] = fmaf(d[i], (xf[i] - mean[i]) * istd[i], acc[1][i]); }
+        if (DUAL) { float sf[BN_VEC]; unpack8(sv[u], sf);
+          _Pragma("unroll") for (int i = 0; i < BN_VEC; ++i) acc[NA - 1][i] = fmaf(d[i], (sf[i] - mean_s[i]) * istd_s[i], acc[NA - 1][i]); }
+        (void)off; })
+  cta_fold<NA>(acc, a.partial + (long long)blockIdx.x * NA * a.C, a.C, rgroups, rg, cv);
   if (last_cta(a.counter)) {
-    grid_fold(a.partial, a.C);
+    grid_fold<NA>(a.partial, a.C);
     const float inv_m = 1.0f / (float)a.M;
     for (int c = threadIdx.x; c < a.C; c += BN_THREADS) {
       const float s = bn_smem[c], q = bn_smem[a.C + c];
@@ -287,6 +368,15 @@ __global__ void __launch_bounds__(BN_THREADS) bn_bwd_reduce_kernel(const BnBwdAr
       a.dgamma[c] = q;
       a.sums[c] = s * inv_m;
       a.sums[a.C + c] = q * inv_m;
+      if (DUAL) { a.dbeta_s[c] = s; a.sums_s[c] = s * inv_m; }          // both layers see the same dz
+    }
+    if (DUAL) {
+      grid_fold<NA>(a.partial, a.C, a.C);                              // rows 1, 2: sum(dz * xhat_s) lands in bn_smem[C .. 2C)
+      for (int c = threadIdx.x; c < a.C; c += BN_THREADS) {
+        const float q = bn_smem[a.C + c];
+        a.dgamma_s[c] = q;
+        a.sums_s[a.C + c] = q * inv_m;
+      }
     }
   }
 }
@@ -298,7 +388,7 @@ __global__ void __launch_bounds__(BN_THREADS, 2) bn_bwd_apply_kernel(const BnBwd
   const int cv = threadIdx.x % tpc, rg = threadIdx.x / tpc;
   // dx = gs * (d - m1 - xhat * m2) with xhat = (x - mean) * istd   ==   A * d + B * x + Cc
   float cA[BN_VEC], cB[BN_VEC], cC[BN_VEC];
-  constexpr bool relu_y = MASK == 1, relu_x = MASK == 2;
+  constexpr bool relu_y = MASK == 1, relu_x = MASK == 2, relu_b = MASK == 3;
   __shared__ __align__(16) float s_sh[BN_THREADS * BN_VEC];           // the forward's shift per channel (mask recomputation), read per row: keeps
   if (relu_x) {                                        // the kernel inside 64 registers
     for (int c = threadIdx.x; c < a.C; c += BN_THREADS) s_sh[c] = fmaf(-a.mean[c], a.gamma[c] * a.invstd[c], a.beta[c]);
@@ -315,14 +405,17 @@ __global__ void __launch_bounds__(BN_THREADS, 2) bn_bwd_apply_kernel(const BnBwd
   }
   const long long r0 = (long long)blockIdx.x * a.rows_per_cta;
   long long r1 = r0 + a.rows_per_cta; if (r1 > a.M) r1 = a.M;
-  constexpr int BU = 2;                                            // three streams in flight: keep the register count moderate
+  // three streams in flight: keep the register count moderate (the bit mask's row offset arithmetic tips two rows over 64)
+  constexpr int BU = relu_b ? 1 : 2;
   long long r = r0 + rg;
   for (; r + (long long)(BU - 1) * rgroups < r1; r += (long long)BU * rgroups) {
     uint4 dv[BU], xv[BU], yv[BU];
+    uint32_t mv[BU];
 #pragma unroll
     for (int u = 0; u < BU; ++u) {
       const long long off = (r + (long long)u * rgroups) * a.C + cv * BN_VEC;
       dv[u] = ldg16(a.dy + off); xv[u] = ldg16(a.x + off); if (relu_y) yv[u] = ldg16(a.y + off);
+      if (relu_b) mv[u] = ldg_u8(a.mask + (off >> 3));
     }
 #pragma unroll
     for (int u = 0; u < BU; ++u) {
@@ -335,6 +428,9 @@ __global__ void __launch_bounds__(BN_THREADS, 2) bn_bwd_apply_kernel(const BnBwd
       if (relu_x) {
 #pragma unroll
         for (int i = 0; i < BN_VEC; ++i) d[i] = relu_mask(xf[i], cA[i], sh[i]) ? d[i] : 0.f; }
+      if (relu_b) {
+#pragma unroll
+        for (int i = 0; i < BN_VEC; ++i) d[i] = (mv[u] >> i) & 1u ? d[i] : 0.f; }
       if (a.dres) *reinterpret_cast<uint4*>(a.dres + off) = pack8(d);
       float o[BN_VEC];
 #pragma unroll
@@ -353,11 +449,61 @@ __global__ void __launch_bounds__(BN_THREADS, 2) bn_bwd_apply_kernel(const BnBwd
     if (relu_x) {
 #pragma unroll
       for (int i = 0; i < BN_VEC; ++i) d[i] = relu_mask(xf[i], cA[i], sh[i]) ? d[i] : 0.f; }
+    if (relu_b) { const uint32_t m = ldg_u8(a.mask + (off >> 3));
+#pragma unroll
+      for (int i = 0; i < BN_VEC; ++i) d[i] = (m >> i) & 1u ? d[i] : 0.f; }
     if (a.dres) *reinterpret_cast<uint4*>(a.dres + off) = pack8(d);
     float o[BN_VEC];
 #pragma unroll
     for (int i = 0; i < BN_VEC; ++i) o[i] = fmaf(cA[i], d[i], fmaf(cB[i], xf[i], cC[i]));
     *reinterpret_cast<uint4*>(a.dx + off) = pack8(o);
+  }
+}
+
+// Downsampling pair: dz = mask(dy) -> dx = A * dz + B * x + Cc (bn2) and dxs = As * dz + Bs * xs + Cs (shortcut BatchNorm), the
+// coefficients formed exactly as bn_bwd_apply_kernel forms them.  The shortcut's sit in shared memory (3C floats of dynamic
+// smem, read per row) and one row is in flight per thread: three input streams and two outputs inside 64 registers.
+__global__ void __launch_bounds__(BN_THREADS, 2) bn_bwd_apply_dual_kernel(const BnBwdArgs a) {
+  const int tpc = a.C / BN_VEC;
+  const int rgroups = BN_THREADS / tpc;
+  const int cv = threadIdx.x % tpc, rg = threadIdx.x / tpc;
+  for (int c = threadIdx.x; c < a.C; c += BN_THREADS) {
+    const float istd = a.invstd_s[c], gs = a.gamma_s[c] * istd, m1 = a.sums_s[c], m2 = a.sums_s[a.C + c], mean = a.mean_s[c];
+    bn_smem[c] = gs;
+    bn_smem[a.C + c] = -gs * m2 * istd;
+    bn_smem[2 * a.C + c] = gs * (m2 * istd * mean - m1);
+  }
+  float cA[BN_VEC], cB[BN_VEC], cC[BN_VEC];
+#pragma unroll
+  for (int i = 0; i < BN_VEC; ++i) {
+    const int c = cv * BN_VEC + i;
+    const float istd = a.invstd[c], gs = a.gamma[c] * istd, m1 = a.sums[c], m2 = a.sums[a.C + c], mean = a.mean[c];
+    cA[i] = gs;
+    cB[i] = -gs * m2 * istd;
+    cC[i] = gs * (m2 * istd * mean - m1);
+  }
+  __syncthreads();
+  const float* sA = bn_smem + cv * BN_VEC;
+  const float* sB = sA + a.C;
+  const float* sC = sB + a.C;
+  const long long r0 = (long long)blockIdx.x * a.rows_per_cta;
+  long long r1 = r0 + a.rows_per_cta; if (r1 > a.M) r1 = a.M;
+  for (long long r = r0 + rg; r < r1; r += rgroups) {
+    const long long off = r * a.C + cv * BN_VEC;
+    const uint4 dvv = ldg16(a.dy + off), xvv = ldg16(a.x + off), svv = ldg16(a.xs + off);
+    const uint32_t m = ldg_u8(a.mask + (off >> 3));
+    float d[BN_VEC], f[BN_VEC], o[BN_VEC];
+    unpack8(dvv, d);
+#pragma unroll
+    for (int i = 0; i < BN_VEC; ++i) d[i] = (m >> i) & 1u ? d[i] : 0.f;
+    unpack8(xvv, f);
+#pragma unroll
+    for (int i = 0; i < BN_VEC; ++i) o[i] = fmaf(cA[i], d[i], fmaf(cB[i], f[i], cC[i]));
+    *reinterpret_cast<uint4*>(a.dx + off) = pack8(o);
+    unpack8(svv, f);
+#pragma unroll
+    for (int i = 0; i < BN_VEC; ++i) o[i] = fmaf(sA[i], d[i], fmaf(sB[i], f[i], sC[i]));
+    *reinterpret_cast<uint4*>(a.dxs + off) = pack8(o);
   }
 }
 
@@ -380,18 +526,31 @@ int plan_rows(long long M, int C, int num_sms, bool reduce, int* grid) {
   return (int)rows;
 }
 
-size_t smem_bytes(int C) {
-  // cta_fold: BN_THREADS * 16 floats (32 KB); grid_fold: totals 2C floats + BN_THREADS float4 of scratch
-  size_t a = (size_t)BN_THREADS * 2 * BN_VEC * sizeof(float);
+size_t smem_bytes(int C, int na = 2) {
+  // cta_fold: BN_THREADS * 8 * na floats (32 KB, 48 KB for the pair); grid_fold: totals 2C floats + BN_THREADS float4 of scratch
+  size_t a = (size_t)BN_THREADS * na * BN_VEC * sizeof(float);
   size_t b = ((size_t)2 * C + 4 * BN_THREADS) * sizeof(float);
   return a > b ? a : b;
+}
+
+// bn_apply_kernel's per-channel coefficients; C = 4096 with DUAL needs 64 KB (opted in once per process)
+size_t fwd_smem_bytes(int C, bool dual) {
+  const size_t b = (size_t)(dual ? 4 : 2) * C * sizeof(float);
+  if (dual && b > 48 * 1024) {
+    static const bool once = [] {
+      cudaFuncSetAttribute(bn_apply_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * 4096 * (int)sizeof(float));
+      return true;
+    }();
+    (void)once;
+  }
+  return b;
 }
 
 }  // namespace
 
 extern "C" int drc_bn_supported(int C) { return supported(C) ? 1 : 0; }
 
-// workspace floats needed for `partial`
+// workspace floats needed for `partial` (the downsampling pair's backward needs 3/2 of it)
 extern "C" long long drc_bn_workspace(long long M, int C, int num_sms) {
   if (!supported(C)) return -1;
   int grid; plan_rows(M, C, num_sms, true, &grid);
@@ -399,7 +558,8 @@ extern "C" long long drc_bn_workspace(long long M, int C, int num_sms) {
 }
 
 // Forward.  have_stats != 0: mean / invstd were produced by the convolution epilogue -> only the apply kernel runs.
-extern "C" int drc_bn_fwd(const void* x, const void* res, void* y, const float* gamma, const float* beta, float* running_mean,
+// mask (optional, relu only): the ReLU bits [M][C/8] for the backward's MASK == 3.
+extern "C" int drc_bn_fwd(const void* x, const void* res, void* y, void* mask, const float* gamma, const float* beta, float* running_mean,
                           float* running_var, float* mean, float* invstd, float* partial, unsigned int* counter, long long M, int C,
                           float eps, float momentum, int relu, int num_sms, int have_stats, cudaStream_t stream) {
   if (!supported(C)) return -1;
@@ -407,36 +567,85 @@ extern "C" int drc_bn_fwd(const void* x, const void* res, void* y, const float* 
   a.x = (const __nv_bfloat16*)x; a.res = (const __nv_bfloat16*)res; a.y = (__nv_bfloat16*)y; a.gamma = gamma; a.beta = beta;
   a.running_mean = running_mean; a.running_var = running_var; a.mean = mean; a.invstd = invstd; a.partial = partial;
   a.counter = counter; a.M = M; a.C = C; a.eps = eps; a.momentum = momentum; a.relu = relu;
+  BnApplyArgs p = {};
+  p.mask = relu ? (uint8_t*)mask : nullptr;
   int grid;
   if (!have_stats) {
     a.rows_per_cta = plan_rows(M, C, num_sms, true, &grid);
     bn_stats_kernel<<<grid, BN_THREADS, smem_bytes(C), stream>>>(a);
   }
   a.rows_per_cta = plan_rows(M, C, num_sms, false, &grid);
-  bn_apply_kernel<<<grid, BN_THREADS, 0, stream>>>(a);
+  bn_apply_kernel<false><<<grid, BN_THREADS, fwd_smem_bytes(C, false), stream>>>(a, p);
   return (int)cudaGetLastError();
 }
 
-extern "C" int drc_bn_bwd(const void* dy, const void* y, const void* x, const float* gamma, const float* beta, const float* mean,
-                          const float* invstd,
+// Forward of a downsampling block's pair: y = relu(bn(x) + bn_s(xs)) in one pass, both layers' statistics from their
+// convolutions' epilogues.  Same values as drc_bn_fwd(xs) followed by drc_bn_fwd(x, residual = that output).
+extern "C" int drc_bn_fwd_dual(const void* x, const void* xs, void* y, void* mask, const float* gamma, const float* beta,
+                               const float* mean, const float* invstd, const float* gamma_s, const float* beta_s,
+                               const float* mean_s, const float* invstd_s, long long M, int C, int num_sms, cudaStream_t stream) {
+  if (!supported(C) || !mask) return -1;
+  BnFwdArgs a;
+  a.x = (const __nv_bfloat16*)x; a.res = (const __nv_bfloat16*)xs; a.y = (__nv_bfloat16*)y; a.gamma = gamma; a.beta = beta;
+  a.running_mean = a.running_var = nullptr; a.mean = const_cast<float*>(mean); a.invstd = const_cast<float*>(invstd);
+  a.partial = nullptr; a.counter = nullptr; a.M = M; a.C = C; a.eps = 0.f; a.momentum = 0.f; a.relu = 1;
+  BnApplyArgs p;
+  p.mask = (uint8_t*)mask; p.gamma_s = gamma_s; p.beta_s = beta_s; p.mean_s = mean_s; p.invstd_s = invstd_s;
+  int grid;
+  a.rows_per_cta = plan_rows(M, C, num_sms, false, &grid);
+  bn_apply_kernel<true><<<grid, BN_THREADS, fwd_smem_bytes(C, true), stream>>>(a, p);
+  return (int)cudaGetLastError();
+}
+
+// mask_mode: 0 = no ReLU, 1 = mask from the saved output y, 2 = recomputed from x (needs beta), 3 = the forward's bits `mask`
+extern "C" int drc_bn_bwd(const void* dy, const void* y, const void* mask, const void* x, const float* gamma, const float* beta,
+                          const float* mean, const float* invstd,
                           void* dx, void* dres, float* dgamma, float* dbeta, float* partial, float* sums, unsigned int* counter,
-                          long long M, int C, int relu, int num_sms, cudaStream_t stream) {
+                          long long M, int C, int mask_mode, int num_sms, cudaStream_t stream) {
   if (!supported(C)) return -1;
-  BnBwdArgs a;
+  if ((mask_mode == 1 && !y) || (mask_mode == 2 && !beta) || (mask_mode == 3 && !mask) || mask_mode < 0 || mask_mode > 3) return -2;
+  BnBwdArgs a = {};
   a.dy = (const __nv_bfloat16*)dy; a.y = (const __nv_bfloat16*)y; a.x = (const __nv_bfloat16*)x; a.gamma = gamma; a.beta = beta;
-  a.mean = mean; a.invstd = invstd;
-  if (relu && !y && !beta) return -2; a.dx = (__nv_bfloat16*)dx; a.dres = (__nv_bfloat16*)dres; a.dgamma = dgamma; a.dbeta = dbeta;
-  a.partial = partial; a.sums = sums; a.counter = counter; a.M = M; a.C = C; a.relu = relu;
+  a.mean = mean; a.invstd = invstd; a.mask = (const uint8_t*)mask;
+  a.dx = (__nv_bfloat16*)dx; a.dres = (__nv_bfloat16*)dres; a.dgamma = dgamma; a.dbeta = dbeta;
+  a.partial = partial; a.sums = sums; a.counter = counter; a.M = M; a.C = C; a.relu = mask_mode != 0;
   int grid;
   a.rows_per_cta = plan_rows(M, C, num_sms, true, &grid);
-  const int mask = !relu ? 0 : (y ? 1 : 2);
-  if (mask == 0) bn_bwd_reduce_kernel<0><<<grid, BN_THREADS, smem_bytes(C), stream>>>(a);
-  else if (mask == 1) bn_bwd_reduce_kernel<1><<<grid, BN_THREADS, smem_bytes(C), stream>>>(a);
-  else bn_bwd_reduce_kernel<2><<<grid, BN_THREADS, smem_bytes(C), stream>>>(a);
+  if (mask_mode == 0) bn_bwd_reduce_kernel<0><<<grid, BN_THREADS, smem_bytes(C), stream>>>(a);
+  else if (mask_mode == 1) bn_bwd_reduce_kernel<1><<<grid, BN_THREADS, smem_bytes(C), stream>>>(a);
+  else if (mask_mode == 2) bn_bwd_reduce_kernel<2><<<grid, BN_THREADS, smem_bytes(C), stream>>>(a);
+  else bn_bwd_reduce_kernel<3><<<grid, BN_THREADS, smem_bytes(C), stream>>>(a);
   a.rows_per_cta = plan_rows(M, C, num_sms, false, &grid);
-  if (mask == 0) bn_bwd_apply_kernel<0><<<grid, BN_THREADS, 0, stream>>>(a);
-  else if (mask == 1) bn_bwd_apply_kernel<1><<<grid, BN_THREADS, 0, stream>>>(a);
-  else bn_bwd_apply_kernel<2><<<grid, BN_THREADS, 0, stream>>>(a);
+  if (mask_mode == 0) bn_bwd_apply_kernel<0><<<grid, BN_THREADS, 0, stream>>>(a);
+  else if (mask_mode == 1) bn_bwd_apply_kernel<1><<<grid, BN_THREADS, 0, stream>>>(a);
+  else if (mask_mode == 2) bn_bwd_apply_kernel<2><<<grid, BN_THREADS, 0, stream>>>(a);
+  else bn_bwd_apply_kernel<3><<<grid, BN_THREADS, 0, stream>>>(a);
+  return (int)cudaGetLastError();
+}
+
+// Backward of the downsampling pair (the forward's bits `mask`): one reduce for both layers' sums (partial: 3/2 of
+// drc_bn_workspace, sums and sums_s [2][C] each), one apply writing dx and dxs.  Bit-identical to drc_bn_bwd(mode 3, dres)
+// for the main layer followed by drc_bn_bwd(dres, mode 0) for the shortcut layer.
+extern "C" int drc_bn_bwd_dual(const void* dy, const void* mask, const void* x, const void* xs, const float* gamma,
+                               const float* mean, const float* invstd, const float* gamma_s, const float* mean_s,
+                               const float* invstd_s, void* dx, void* dxs, float* dgamma, float* dbeta, float* dgamma_s,
+                               float* dbeta_s, float* partial, float* sums, float* sums_s, unsigned int* counter, long long M,
+                               int C, int num_sms, cudaStream_t stream) {
+  if (!supported(C) || !mask) return -1;
+  BnBwdArgs a = {};
+  a.dy = (const __nv_bfloat16*)dy; a.mask = (const uint8_t*)mask; a.x = (const __nv_bfloat16*)x; a.xs = (const __nv_bfloat16*)xs;
+  a.gamma = gamma; a.mean = mean; a.invstd = invstd; a.gamma_s = gamma_s; a.mean_s = mean_s; a.invstd_s = invstd_s;
+  a.dx = (__nv_bfloat16*)dx; a.dxs = (__nv_bfloat16*)dxs; a.dgamma = dgamma; a.dbeta = dbeta; a.dgamma_s = dgamma_s;
+  a.dbeta_s = dbeta_s; a.partial = partial; a.sums = sums; a.sums_s = sums_s; a.counter = counter; a.M = M; a.C = C; a.relu = 1;
+  int grid;
+  a.rows_per_cta = plan_rows(M, C, num_sms, true, &grid);
+  // 48 KB of dynamic shared memory next to the static ticket flag: over the default limit, opted in once per process
+  static const int smem_ok = (int)cudaFuncSetAttribute(bn_bwd_reduce_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                       (int)smem_bytes(4096, 3));
+  if (smem_ok != 0) return smem_ok;
+  bn_bwd_reduce_kernel<3, true><<<grid, BN_THREADS, smem_bytes(C, 3), stream>>>(a);
+  a.rows_per_cta = plan_rows(M, C, num_sms, false, &grid);
+  bn_bwd_apply_dual_kernel<<<grid, BN_THREADS, 3 * C * sizeof(float), stream>>>(a);
   return (int)cudaGetLastError();
 }
 
@@ -445,7 +654,7 @@ extern "C" int drc_bn_bwd(const void* dy, const void* y, const void* x, const fl
 extern "C" int drc_bn_bwd_apply(const void* dz, const void* x, const float* gamma, const float* mean, const float* invstd,
                                 const float* sums, void* dx, long long M, int C, int num_sms, cudaStream_t stream) {
   if (!supported(C)) return -1;
-  BnBwdArgs a;
+  BnBwdArgs a = {};
   a.dy = (const __nv_bfloat16*)dz; a.y = nullptr; a.x = (const __nv_bfloat16*)x; a.gamma = gamma; a.beta = nullptr;
   a.mean = mean; a.invstd = invstd; a.dx = (__nv_bfloat16*)dx; a.dres = nullptr; a.dgamma = nullptr; a.dbeta = nullptr;
   a.partial = nullptr; a.sums = const_cast<float*>(sums); a.counter = nullptr; a.M = M; a.C = C; a.relu = 0;

@@ -30,12 +30,13 @@ def _conv(cin: int, cout: int, k: int, stride: int = 1) -> nn.Conv2d:
     return Conv2d(cin, cout, kernel_size=k, stride=stride, padding=k // 2, bias=False)
 
 
-def _shortcut(seq: nn.Sequential, x: torch.Tensor) -> torch.Tensor:
-    """Identity or projection (conv1x1 + BN) shortcut; the projection's BatchNorm statistics come from its convolution too."""
+def _bn_residual_relu(bn: FusedBatchNorm2d, c: torch.Tensor, seq: nn.Sequential, x: torch.Tensor) -> torch.Tensor:
+    """relu(bn(c) + shortcut(x)) for an identity or projection (conv1x1 + BN) shortcut.  The projection's BatchNorm statistics
+    come from its convolution too, and ``residual_bn`` lets both BatchNorms run as one pass each way (ops/norm.py)."""
     if len(seq) == 0:
-        return x
-    conv, bn = seq[0], seq[1]
-    return bn(conv(x, bn=bn))
+        return bn(c, residual=x, relu=True)
+    conv, bn_s = seq[0], seq[1]
+    return bn(c, residual_bn=(bn_s, conv(x, bn=bn_s)), relu=True)
 
 
 class BasicBlock(nn.Module):
@@ -58,7 +59,7 @@ class BasicBlock(nn.Module):
         c1, xs = self.conv1(x, bn=self.bn1, fork=True)
         out = self.bn1(c1, relu=True)
         # bn2 + shortcut add + relu in one pass (ops/norm.py)
-        return self.bn2(self.conv2(out, bn=self.bn2), residual=_shortcut(self.shortcut, xs), relu=True)
+        return _bn_residual_relu(self.bn2, self.conv2(out, bn=self.bn2), self.shortcut, xs)
 
 
 class Bottleneck(nn.Module):
@@ -80,7 +81,7 @@ class Bottleneck(nn.Module):
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         out = self.bn1(self.conv1(x, bn=self.bn1), relu=True)
         out = self.bn2(self.conv2(out, bn=self.bn2), relu=True)
-        return self.bn3(self.conv3(out, bn=self.bn3), residual=_shortcut(self.shortcut, x), relu=True)
+        return _bn_residual_relu(self.bn3, self.conv3(out, bn=self.bn3), self.shortcut, x)
 
 
 class ResNet(nn.Module):
