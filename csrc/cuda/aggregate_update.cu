@@ -17,7 +17,9 @@ struct UpdateArgs {
                                   // 3: coordinate-wise trimmed mean over K rows (see `trim`);
                                   // 4: Bulyan's average of the K - 2 trim values nearest the coordinate median of K rows;
                                   // 5: centered clipping, v + sum_k w[tensor][k] (g_k - v) around the centre `center`;
-                                  // 6: signSGD majority vote over the K = P sign rows (slots 0..K-1, K <= 32)
+                                  // 6: signSGD majority vote over the K = P sign rows (slots 0..K-1, K <= 32);
+                                  // 7: mode 3 over the K = nb worker-bucket rows of `wb_mask` / `wb_scale`;
+                                  // 8: mode 5 over those rows
   const float* grad_in;           // mode 0: [P][slot_stride] fp32 ; mode 1: [n][2*slot_stride] complex64 ;
                                   // mode 6: [K][slot_stride] uint32 sign words (bit b of word w = element 32w + b is < 0)
   long long slot_stride;          // elements (fp32 words for mode 0, complex elements for mode 1, uint32 sign words for mode 6)
@@ -52,6 +54,9 @@ struct UpdateArgs {
   float mix_scale;                // fp32(1 / n_mix), n_mix = P - f
   // centered clipping (mode 5; appended) ------------------------------------------------------------------------------------
   float* center;                  // [D] the centre v, replaced by the aggregate g; weights in `recomb` as float [T][K]
+  // worker buckets (mode 7; appended) ---------------------------------------------------------------------------------------
+  const unsigned int* wb_mask;    // [K] member masks of the step's K = nb bucket rows (bit j = slot j), from wbucket_plan_kernel
+  const float* wb_scale;          // [K] fp32(1 / |b|) of each bucket row
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -227,6 +232,46 @@ __device__ __forceinline__ float4 mixed_robust_f4(const UpdateArgs& a, long long
 }
 
 // ---------------------------------------------------------------------------------------------
+// Mode 7: mode 3 over worker-bucket rows (--bucketing; bucketing.cu wbucket_plan_kernel; codes/oracle.py::wbucket_rows).
+// Bucket row r holds the raw slots of wb_mask[r].  Per coordinate it is formed in fp32 as
+//     y = -0.0f;  for the member slots j in ascending order: y = y + x_j  (round to nearest);  y = y * wb_scale[r]  (rounded),
+// where -0.0f + x_j is x_j for every x_j, so y starts from the lowest member; a one-member row is that member (times 1.0f,
+// which changes at most a NaN's payload, and every NaN maps to the same key).  The buckets are disjoint, so each raw value is
+// loaded once and summed into its own row only; the K = nb row values are then reduced by trimmed_sum as in raw_robust_f4,
+// with the network chosen from nb (SORT_N >= K), not from P.
+// ---------------------------------------------------------------------------------------------
+template <int N>
+__device__ __forceinline__ float4 wbucket_robust_f4(const UpdateArgs& a, long long idx) {
+  float4 y[N];
+#pragma unroll
+  for (int r = 0; r < N; ++r) {
+    y[r] = make_float4(-0.f, -0.f, -0.f, -0.f);
+    if (r < a.K) {
+      for (unsigned int m = a.wb_mask[r]; m; m &= m - 1u) {
+        const float4 v = ld_f4(reinterpret_cast<const float4*>(a.grad_in + (__ffs(m) - 1) * a.slot_stride + idx));
+        y[r].x = __fadd_rn(y[r].x, v.x); y[r].y = __fadd_rn(y[r].y, v.y);
+        y[r].z = __fadd_rn(y[r].z, v.z); y[r].w = __fadd_rn(y[r].w, v.w);
+      }
+      const float sc = a.wb_scale[r];
+      y[r].x = __fmul_rn(y[r].x, sc); y[r].y = __fmul_rn(y[r].y, sc);
+      y[r].z = __fmul_rn(y[r].z, sc); y[r].w = __fmul_rn(y[r].w, sc);
+    }
+  }
+  float out[4];
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    unsigned int k[N];
+#pragma unroll
+    for (int r = 0; r < N; ++r) {
+      const float v = e == 0 ? y[r].x : e == 1 ? y[r].y : e == 2 ? y[r].z : y[r].w;
+      k[r] = r < a.K ? float_key(v) : 0xFFFFFFFFu;
+    }
+    out[e] = trimmed_sum<N>(k, a.K, a.trim);
+  }
+  return make_float4(out[0], out[1], out[2], out[3]);
+}
+
+// ---------------------------------------------------------------------------------------------
 // Mode 5: centered clipping (clip.cu; codes/oracle.py::centered_clip).  Per coordinate, from acc = +0 and for the rows k in
 // ascending order whose weight w_k = w[tensor][k] (cc_weights_kernel) is not zero: acc = fma_rn(w_k, rn(x_k - v), acc); then
 // g = rn(v + acc), stored back as the next step's centre.  A zero weight (a NaN or +Inf distance) skips the row's load, so
@@ -241,6 +286,30 @@ __device__ __forceinline__ float4 centered_clip_f4(const UpdateArgs& a, long lon
     if (w == 0.f) continue;
     const int slot = a.select ? a.select[k * a.tv.ntensors + tensor] : k;
     const float4 x = ld_f4(reinterpret_cast<const float4*>(a.grad_in + slot * a.slot_stride + idx));
+    acc.x = __fmaf_rn(w, __fsub_rn(x.x, v.x), acc.x); acc.y = __fmaf_rn(w, __fsub_rn(x.y, v.y), acc.y);
+    acc.z = __fmaf_rn(w, __fsub_rn(x.z, v.z), acc.z); acc.w = __fmaf_rn(w, __fsub_rn(x.w, v.w), acc.w);
+  }
+  const float4 g = make_float4(__fadd_rn(v.x, acc.x), __fadd_rn(v.y, acc.y), __fadd_rn(v.z, acc.z), __fadd_rn(v.w, acc.w));
+  *reinterpret_cast<float4*>(a.center + idx) = g;
+  return g;
+}
+
+// Mode 8: mode 5 over the K = nb worker-bucket rows (--bucketing).  Row k, for a non-zero weight only, is formed per coordinate
+// as in mode 7 (members ascending from -0.0f, then times wb_scale[k]); a bucket of zero weight is never read.
+__device__ __forceinline__ float4 centered_clip_wbucket_f4(const UpdateArgs& a, long long idx, int tensor) {
+  const float* wts = reinterpret_cast<const float*>(a.recomb);
+  const float4 v = *reinterpret_cast<const float4*>(a.center + idx);
+  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int k = 0; k < a.K; ++k) {
+    const float w = wts[tensor * a.K + k];
+    if (w == 0.f) continue;
+    float4 x = make_float4(-0.f, -0.f, -0.f, -0.f);
+    for (unsigned int m = a.wb_mask[k]; m; m &= m - 1u) {
+      const float4 y = ld_f4(reinterpret_cast<const float4*>(a.grad_in + (__ffs(m) - 1) * a.slot_stride + idx));
+      x.x = __fadd_rn(x.x, y.x); x.y = __fadd_rn(x.y, y.y); x.z = __fadd_rn(x.z, y.z); x.w = __fadd_rn(x.w, y.w);
+    }
+    const float sc = a.wb_scale[k];
+    x.x = __fmul_rn(x.x, sc); x.y = __fmul_rn(x.y, sc); x.z = __fmul_rn(x.z, sc); x.w = __fmul_rn(x.w, sc);
     acc.x = __fmaf_rn(w, __fsub_rn(x.x, v.x), acc.x); acc.y = __fmaf_rn(w, __fsub_rn(x.y, v.y), acc.y);
     acc.z = __fmaf_rn(w, __fsub_rn(x.z, v.z), acc.z); acc.w = __fmaf_rn(w, __fsub_rn(x.w, v.w), acc.w);
   }
@@ -318,6 +387,10 @@ __global__ void __launch_bounds__(DRC_THREADS) aggregate_update_kernel(const __g
       g = mixed_robust_f4<MODE, SORT_N>(a, idx, tensor);
     } else if constexpr (MODE == 3 || MODE == 4) {
       g = raw_robust_f4<MODE, SORT_N, SEL>(a, idx, tensor);
+    } else if constexpr (MODE == 7) {
+      g = wbucket_robust_f4<SORT_N>(a, idx);
+    } else if constexpr (MODE == 8) {
+      g = centered_clip_wbucket_f4(a, idx, tensor);
     } else if constexpr (MODE == 5) {
       g = centered_clip_f4(a, idx, tensor);
     } else if constexpr (MODE == 6) {
@@ -334,7 +407,7 @@ __global__ void __launch_bounds__(DRC_THREADS) aggregate_update_kernel(const __g
         g.w += v.x * c1.z - v.y * c1.w;
       }
     }
-    if constexpr (MODE != 5 && MODE != 6) { g.x *= a.scale; g.y *= a.scale; g.z *= a.scale; g.w *= a.scale; }
+    if constexpr (MODE != 5 && MODE != 6 && MODE != 8) { g.x *= a.scale; g.y *= a.scale; g.z *= a.scale; g.w *= a.scale; }
     if (a.grad_out) *reinterpret_cast<float4*>(a.grad_out + idx) = g;
 
     float4 p = *reinterpret_cast<const float4*>(a.params + idx);
@@ -396,13 +469,27 @@ extern "C" int drc_aggregate_update(const UpdateArgs* args, int grid, cudaStream
   if (args->ndst > DRC_MAX_DST || args->flags.n > DRC_MAX_DST) return (int)cudaErrorInvalidValue;
   // modes 3 and 4 sort K <= TRIM_MAXP rows per coordinate and keep K - 2 trim of them; mode 4 reads its K = theta rows
   // through the table bulyan_select filled
-  if ((mode == 3 || mode == 4) && (K < 1 || K > TRIM_MAXP || args->trim < 0 || 2 * args->trim >= K))
+  if ((mode == 3 || mode == 4 || mode == 7) && (K < 1 || K > TRIM_MAXP || args->trim < 0 || 2 * args->trim >= K))
     return (int)cudaErrorInvalidValue;
   if (mode == 4 && !args->select) return (int)cudaErrorInvalidValue;
   // centered clipping: K <= TRIM_MAXP rows (through `select` or slots 0..K-1), their weights and the centre
   if (mode == 5) {
     if (K < 1 || K > TRIM_MAXP || !args->recomb || !args->center || args->mix) return (int)cudaErrorInvalidValue;
     aggregate_update_kernel<5><<<grid, DRC_THREADS, 0, stream>>>(*args);
+    return (int)cudaGetLastError();
+  }
+  // worker buckets: the trimmed mean / median of K = nb <= TRIM_MAXP bucket rows, formed from the masks and scales of
+  // wbucket_plan_kernel (no row table, no mixing)
+  if (mode == 7) {
+    if (!args->wb_mask || !args->wb_scale || args->select || args->mix) return (int)cudaErrorInvalidValue;
+    launch_sorted<7, false, false>(args, K, grid, stream);
+    return (int)cudaGetLastError();
+  }
+  // centered clipping over the K = nb worker-bucket rows
+  if (mode == 8) {
+    if (K < 1 || K > TRIM_MAXP || !args->recomb || !args->center || !args->wb_mask || !args->wb_scale || args->select || args->mix)
+      return (int)cudaErrorInvalidValue;
+    aggregate_update_kernel<8><<<grid, DRC_THREADS, 0, stream>>>(*args);
     return (int)cudaGetLastError();
   }
   // signSGD majority vote: K = P <= 32 sign rows in slots 0..K-1 (the adversary bitmaps' width), no row table

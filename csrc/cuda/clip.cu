@@ -30,6 +30,9 @@ struct CcArgs {
   int tile_begin, tile_end;               // dist: tiles (tile_end == 0: to the end of the arena)
   int t_begin, t_end;                     // weights: tensors (t_end == 0: every tensor); buckets hold whole tensors
   double* dist;                           // model scope: [T][n] the per-tensor d_i, folded in tile order
+  // worker buckets (appended): row i is the bucket row of wb_mask[i] / wb_scale[i] (bucketing.cu), formed in registers
+  const unsigned int* wb_mask;
+  const float* wb_scale;
 };
 
 __global__ void __launch_bounds__(DRC_THREADS) cc_dist_kernel(const __grid_constant__ CcArgs a) {
@@ -62,6 +65,54 @@ __global__ void __launch_bounds__(DRC_THREADS) cc_dist_kernel(const __grid_const
           if (lane_valid > 1) { const double e = __dsub_rn((double)x[i].y, (double)v.y); d = __dadd_rn(d, __dmul_rn(e, e)); }
           if (lane_valid > 2) { const double e = __dsub_rn((double)x[i].z, (double)v.z); d = __dadd_rn(d, __dmul_rn(e, e)); }
           if (lane_valid > 3) { const double e = __dsub_rn((double)x[i].w, (double)v.w); d = __dadd_rn(d, __dmul_rn(e, e)); }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) d = __dadd_rn(d, __shfl_xor_sync(0xffffffffu, d, o));
+        if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5][i] = d;
+      }
+    }
+    __syncthreads();
+    if ((int)threadIdx.x < n) {
+      double s = 0.0;
+#pragma unroll
+      for (int w = 0; w < DRC_THREADS / 32; ++w) s = __dadd_rn(s, s_part[w][threadIdx.x]);
+      a.partials[(long long)tile * n + threadIdx.x] = s;
+    }
+    __syncthreads();
+  }
+}
+
+// cc_dist_kernel over the n = nb worker-bucket rows (--bucketing): row i is formed per coordinate in fp32 from its member slots
+// in ascending order, starting from -0.0f, then times wb_scale[i] (aggregate_update.cu mode 7's rows, codes/oracle.py::
+// wbucket_rows).  The rest is cc_dist_kernel's fixed-order reduction; a kernel of its own keeps cc_dist_kernel's machine code.
+__global__ void __launch_bounds__(DRC_THREADS) cc_dist_wbucket_kernel(const __grid_constant__ CcArgs a) {
+  __shared__ double s_part[DRC_THREADS / 32][CC_MAXP];
+  const int n = a.n;
+  const int tile_end = a.tile_end > 0 ? a.tile_end : a.tv.ntiles;
+  for (int tile = a.tile_begin + blockIdx.x; tile < tile_end; tile += gridDim.x) {
+    int tensor;
+    const int valid = tile_valid(a.tv, tile, tensor);
+    const long long idx = (long long)tile * DRC_TILE + threadIdx.x * 4;
+    const int lane_valid = valid - (int)threadIdx.x * 4;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (lane_valid > 0) v = *reinterpret_cast<const float4*>(a.center + idx);
+#pragma unroll
+    for (int i = 0; i < CC_MAXP; ++i) {
+      if (i < n) {
+        double d = 0.0;
+        if (lane_valid > 0) {
+          float4 y = make_float4(-0.f, -0.f, -0.f, -0.f);
+          for (unsigned int m = a.wb_mask[i]; m; m &= m - 1u) {
+            const float4 x = ld_f4(reinterpret_cast<const float4*>(a.grad_in + (__ffs(m) - 1) * a.slot_stride + idx));
+            y.x = __fadd_rn(y.x, x.x); y.y = __fadd_rn(y.y, x.y); y.z = __fadd_rn(y.z, x.z); y.w = __fadd_rn(y.w, x.w);
+          }
+          const float sc = a.wb_scale[i];
+          y.x = __fmul_rn(y.x, sc); y.y = __fmul_rn(y.y, sc); y.z = __fmul_rn(y.z, sc); y.w = __fmul_rn(y.w, sc);
+          const double e0 = __dsub_rn((double)y.x, (double)v.x);
+          d = __dmul_rn(e0, e0);
+          if (lane_valid > 1) { const double e = __dsub_rn((double)y.y, (double)v.y); d = __dadd_rn(d, __dmul_rn(e, e)); }
+          if (lane_valid > 2) { const double e = __dsub_rn((double)y.z, (double)v.z); d = __dadd_rn(d, __dmul_rn(e, e)); }
+          if (lane_valid > 3) { const double e = __dsub_rn((double)y.w, (double)v.w); d = __dadd_rn(d, __dmul_rn(e, e)); }
         }
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) d = __dadd_rn(d, __shfl_xor_sync(0xffffffffu, d, o));
@@ -168,6 +219,11 @@ __global__ void __launch_bounds__(DRC_THREADS) cc_model_weights_kernel(const __g
 
 extern "C" int drc_cc_dist(const CcArgs* args, int grid, cudaStream_t stream) {
   if (args->n < 1 || args->n > CC_MAXP || !args->center || !args->partials || grid < 1) return (int)cudaErrorInvalidValue;
+  if (args->wb_mask) {                                           // worker-bucket rows: no row table
+    if (!args->wb_scale || args->rows) return (int)cudaErrorInvalidValue;
+    cc_dist_wbucket_kernel<<<grid, DRC_THREADS, 0, stream>>>(*args);
+    return (int)cudaGetLastError();
+  }
   cc_dist_kernel<<<grid, DRC_THREADS, 0, stream>>>(*args);
   return (int)cudaGetLastError();
 }

@@ -77,7 +77,17 @@ class UpdateArgs(C.Structure):
                 ("exp_avg_sq", ptr), ("max_exp_avg_sq", ptr), ("hp", ptr), ("step_ptr", ptr), ("first_step", u64), ("grad_out", ptr), ("mc_params", ptr),
                 ("dst", ptr * MAX_DST), ("ndst", C.c_int), ("done_counter", ptr), ("flags", FlagList),
                 ("tile_begin", C.c_int), ("tile_end", C.c_int), ("trim", C.c_int),
-                ("mix", ptr), ("mixP", C.c_int), ("mix_scale", C.c_float), ("center", ptr)]
+                ("mix", ptr), ("mixP", C.c_int), ("mix_scale", C.c_float), ("center", ptr), ("wb_mask", ptr), ("wb_scale", ptr)]
+
+
+class WbucketArgs(C.Structure):
+    _fields_ = [("masks", ptr), ("nb", C.c_int), ("P", C.c_int), ("T", C.c_int), ("raw_d2", ptr), ("wb_d2", ptr), ("select", ptr),
+                ("m", C.c_int), ("w_rows", ptr), ("wsel", ptr), ("wts", ptr), ("K", C.c_int)]
+
+
+class WbucketPlanArgs(C.Structure):
+    _fields_ = [("schedule", ptr), ("len", C.c_int), ("P", C.c_int), ("s", C.c_int), ("step_ptr", ptr), ("masks", ptr),
+                ("scales", ptr)]
 
 
 class StreamPushArgs(C.Structure):
@@ -154,7 +164,7 @@ class AttackArgs(C.Structure):
 class CcArgs(C.Structure):
     _fields_ = [("grad_in", ptr), ("slot_stride", i64), ("n", C.c_int), ("rows", ptr), ("tv", TileView), ("center", ptr),
                 ("partials", ptr), ("weights", ptr), ("tau", C.c_double), ("tile_begin", C.c_int), ("tile_end", C.c_int),
-                ("t_begin", C.c_int), ("t_end", C.c_int), ("dist", ptr)]
+                ("t_begin", C.c_int), ("t_end", C.c_int), ("dist", ptr), ("wb_mask", ptr), ("wb_scale", ptr)]
 
 
 def _maybe_build() -> None:
@@ -239,6 +249,9 @@ def cuda() -> C.CDLL:
             "drc_cc_dist": [C.POINTER(CcArgs), C.c_int, st],
             "drc_cc_weights": [C.POINTER(CcArgs), st],
             "drc_cc_model_weights": [C.POINTER(CcArgs), st],
+            "drc_wbucket_plan": [C.POINTER(WbucketPlanArgs), st],
+            "drc_wbucket_table": [C.POINTER(WbucketArgs), st],
+            "drc_wbucket_fold": [C.POINTER(WbucketArgs), st],
             "drc_gemm_bf16": [ptr, i64, C.c_int, ptr, i64, C.c_int, ptr, i64, C.c_int, C.c_int, C.c_int, C.c_int, ptr, ptr,
                               C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, st],
             "drc_rt_init": [C.c_int],

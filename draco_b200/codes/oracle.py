@@ -321,6 +321,80 @@ def nnm(slots: np.ndarray, f: int, mode: str) -> np.ndarray:
     raise ValueError(f"NNM has no rule {mode!r}")
 
 
+BUCKETING_MODES = ("coordinate_median", "trimmed_mean", "krum", "multi_krum", "geometric_median", "centered_clip")
+
+
+def wbucket_rows(slots: np.ndarray, buckets: Sequence[Sequence[int]]) -> np.ndarray:
+    """The fp32 worker-bucket rows (``--bucketing``; Karimireddy, He and Jaggi, ICLR 2022), one per bucket of
+    ``codes.bucketing.wbuckets`` (members ascending, buckets ordered by their lowest member).  A one-member bucket's row is
+    that member's value, bit for bit; otherwise y = x_lowest, then y = rn(y + x_j) for the other members in ascending slot
+    order, then one rounded multiply by fp32(1 / |b|), with no contraction.  fp32 on purpose: every path forms these bits."""
+    X = np.asarray(slots, dtype=np.float32)
+    out = np.empty((len(buckets),) + X.shape[1:], dtype=np.float32)
+    with np.errstate(invalid="ignore", over="ignore"):
+        for b, members in enumerate(buckets):
+            y = X[members[0]].copy()
+            for j in members[1:]:
+                y = np.add(y, X[j], dtype=np.float32)
+            out[b] = y if len(members) == 1 else np.multiply(y, np.float32(1.0 / len(members)), dtype=np.float32)
+    return out
+
+
+def wbucket_pair_d2(D: np.ndarray, buckets: Sequence[Sequence[int]], P: int) -> np.ndarray:
+    """Squared distances between the bucket rows from the raw table ``D`` [P, P] alone (``nnm_pair_d2``'s identity): with
+    c = a_b / |b| - a_k / |k| (a_b the 0/1 membership of bucket b), ||y_b - y_k||^2 = -1/2 c^T D c in fp64, clamped at 0 (a NaN
+    stays a NaN).  Buckets are disjoint, so c touches the members of b and k only."""
+    A = np.zeros((len(buckets), P))
+    for b, members in enumerate(buckets):
+        A[b, list(members)] = 1.0 / len(members)
+    D = np.array(D, dtype=np.float64)
+    np.fill_diagonal(D, 0.0)
+    nb = len(buckets)
+    out = np.zeros((nb, nb))
+    with np.errstate(invalid="ignore", over="ignore"):
+        for b in range(nb):
+            for k in range(nb):
+                if b == k:
+                    continue
+                u = np.array(sorted(list(buckets[b]) + list(buckets[k])))
+                c = A[b, u] - A[k, u]
+                v = -0.5 * (c @ D[np.ix_(u, u)] @ c)
+                out[b, k] = v if not v < 0.0 else 0.0
+    return out
+
+
+def bucketing(slots: np.ndarray, perm, s: int, f: int, mode: str, center=None, tau=None, D=None):
+    """Bucketing, then the robust rule ``mode`` on the nb = ceil(P / s) bucket rows (``wbucket_rows``) of the permutation
+    ``perm``, per tensor, with f = ``--worker-fail`` (each liar spoils at most one bucket):
+
+    * ``coordinate_median``: trim (nb - 1) // 2;  * ``trimmed_mean``: trim f;  * ``krum``: s = f;  * ``multi_krum``: s = f,
+      averaging nb - f rows;  * ``geometric_median``: Weiszfeld weights over the bucket table, applied to the bucket rows;
+    * ``centered_clip``: around ``center`` with n = nb and radius ``tau`` (returns the aggregate, which is the next centre).
+
+    The distance rules take their table from ``wbucket_pair_d2`` over the raw table ``D`` (``_raw_d2(slots)`` unless given:
+    ``--rule-scope model`` passes the whole-model table).  With s = 1 this is the baseline rule on the raw slots."""
+    from .bucketing import wbuckets
+    X = np.asarray(slots, dtype=np.float32)
+    P = X.shape[0]
+    B = wbuckets(perm, s)
+    nb = len(B)
+    Y = wbucket_rows(X, B)
+    if mode == "coordinate_median":
+        return coordinate_median(Y)
+    if mode == "trimmed_mean":
+        return trimmed_mean(Y, f)
+    if mode == "centered_clip":
+        return centered_clip(Y, center, tau)
+    Db = wbucket_pair_d2(_raw_d2(X) if D is None else D, B, P)
+    if mode == "krum":
+        return Y[int(np.argsort(_krum_scores_d2(Db, f), kind="stable")[0])].astype(np.float64)
+    if mode == "multi_krum":
+        return Y[np.argsort(_krum_scores_d2(Db, f), kind="stable")[:nb - f]].astype(np.float64).mean(axis=0)
+    if mode == "geometric_median":
+        return _weiszfeld_weights(Db, 1e-10, 256) @ Y.astype(np.float64)
+    raise ValueError(f"bucketing has no rule {mode!r}")
+
+
 def captured_group_bound(worker_fail: int, group_size: int) -> int:
     """DETOX's b_G: a group of r >= ``group_size`` members returns a liar's row only when at least (r + 1) // 2 of them lie
     (fewer leave the honest rows a strict majority, which Boyer-Moore always returns; for even r, r / 2 liars can tie and win),

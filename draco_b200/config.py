@@ -23,6 +23,8 @@ TRANSPORTS = ("nvl", "nccl", "nccl_flat", "gloo")
 SCOPES = ("tensor", "model")        # --rule-scope / --attack-scope: distances per parameter tensor, or over the whole model
 # the --mode values whose rule measures distances between rows (every --approach nnm mode does, through its neighbourhoods)
 DISTANCE_MODES = ("krum", "multi_krum", "geometric_median", "bulyan", "centered_clip")
+# --bucketing: the rules that run on the worker-bucket means
+BUCKETING_MODES = ("coordinate_median", "trimmed_mean", "krum", "multi_krum", "geometric_median", "centered_clip")
 
 
 @dataclass
@@ -90,6 +92,8 @@ class JobConfig:
     clip_tau: Optional[float] = None  # --mode centered_clip: the clipping radius tau in the gradient's units (per rule_scope)
     rule_scope: str = "tensor"      # distance-based rules: one choice per parameter tensor, or one over the whole model
     attack_scope: str = "tensor"    # --err-mode minmax: one gamma per parameter tensor, or one over the whole model
+    bucketing: int = 0              # worker buckets of s: the robust rule runs on the means of ceil(P / s) random buckets (0: off)
+    dirichlet_alpha: Optional[float] = None  # heterogeneous data: each holder's shard has Dirichlet(alpha) class shares (None: IID)
 
     # ---- derived --------------------------------------------------------------------------
     def resolve(self, world_size: int) -> "JobConfig":
@@ -135,6 +139,8 @@ class JobConfig:
         self._check_worker_momentum()
         self._check_centered_clip()
         self._check_scope()
+        self._check_bucketing()
+        self._check_dirichlet()
         if self.transport == "gloo":
             self.dtype = "fp32"
             self.cuda_graphs = False
@@ -255,6 +261,48 @@ class JobConfig:
         if self.transport == "nvl" and self.mode == "geometric_median" and rows > ROBUST_MAXP:
             raise ValueError(f"--rule-scope model: the geometric median of more than {ROBUST_MAXP} rows on the nvl transport "
                              f"streams over the slab per tensor (got {rows} rows); use --transport nccl or fewer rows")
+
+    def _check_bucketing(self) -> None:
+        """--bucketing s: each step the PS permutes the P worker slots at random, averages them in worker buckets of s and runs
+        ``--mode`` on the nb = ceil(P / s) bucket means, with the rule's bound over nb rows (one liar spoils one bucket)."""
+        s = self.bucketing
+        if s == 0:
+            return
+        P, f = self.num_workers, self.worker_fail
+        if self.approach != "baseline":
+            raise ValueError(f"--bucketing averages the raw worker rows before the rule: use --approach baseline (got --approach "
+                             f"{self.approach})")
+        if self.mode not in BUCKETING_MODES:
+            raise ValueError(f"--bucketing takes --mode {' | '.join(BUCKETING_MODES)} (the rule applied to the bucket means), got "
+                             f"--mode {self.mode}: the mean of bucket means is the mean, Bulyan would need nb >= 4f + 3, and "
+                             f"sign_vote has no fp32 rows")
+        if not 1 <= s <= P:
+            raise ValueError(f"--bucketing s needs 1 <= s <= num_workers (got {s} with {P} workers; 0 turns it off)")
+        if self.transport == "nccl_flat":
+            raise ValueError("--transport nccl_flat runs the plain mean and the vote only; use --transport nccl for --bucketing")
+        if self.transport == "nvl" and P > ROBUST_MAXP:
+            raise ValueError(f"--bucketing on the nvl transport handles at most {ROBUST_MAXP} workers (got {P}); use --transport "
+                             f"nccl for more")
+        nb = -(-P // s)
+        what = f"{P} workers in buckets of {s} give nb = {nb} bucket rows, worker_fail {f}"
+        if self.mode in ("krum", "multi_krum") and nb <= 2 * f + 2:
+            raise ValueError(f"--bucketing --mode {self.mode} needs nb > 2*worker_fail + 2 (Krum's condition over the bucket rows; "
+                             f"{what})")
+        if self.mode not in ("krum", "multi_krum") and 2 * f >= nb:
+            raise ValueError(f"--bucketing --mode {self.mode} needs nb > 2*worker_fail (the honest bucket rows must be a strict "
+                             f"majority; {what})")
+
+    def _check_dirichlet(self) -> None:
+        """--dirichlet-alpha a: each data holder (a worker, or a repetition group) draws from its own shard, whose class shares
+        follow Dirichlet(a)."""
+        a = self.dirichlet_alpha
+        if a is None:
+            return
+        if not (math.isfinite(a) and a > 0):
+            raise ValueError(f"--dirichlet-alpha must be a finite concentration > 0 (got {a}); leave it unset for IID data")
+        if self.approach == "cyclic":
+            raise ValueError("--dirichlet-alpha gives every data holder its own shard; under --approach cyclic the workers split "
+                             "one global batch, so there is no holder to give it to")
 
     @property
     def alie_z(self) -> float:
@@ -404,6 +452,14 @@ def add_fit_args(parser: argparse.ArgumentParser) -> argparse.ArgumentParser:
     a("--attack-scope", type=str, default=d.attack_scope, choices=SCOPES,
       help="--err-mode minmax: tensor (default) solves gamma and Dmax per parameter tensor; model: one gamma and one Dmax over "
            "the flattened model, as in the NDSS paper")
+    a("--bucketing", type=int, default=d.bucketing,
+      help="s (0 = off; --approach baseline): every step the PS permutes the workers at random, averages them in worker buckets "
+           "of s and runs --mode (coordinate_median | trimmed_mean | krum | multi_krum | geometric_median | centered_clip) on "
+           "the ceil(P / s) bucket means, with --worker-fail as f (Karimireddy, He and Jaggi, ICLR 2022)")
+    a("--dirichlet-alpha", type=float, default=None,
+      help="heterogeneous data: every data holder (a worker; a group under maj_vote / detox) samples from its own shard, whose "
+           "class shares are drawn from Dirichlet(alpha) (small alpha: few classes per holder).  Unset: every worker samples "
+           "the whole dataset")
     a("--approach", type=str, default=d.approach,
       help="baseline | maj_vote | cyclic | detox (majority vote inside each repetition group, then --mode across the G group "
            "winners) | nnm (nearest-neighbour mixing: every worker's row is replaced, per tensor, by the mean of its "

@@ -127,6 +127,38 @@ def augment_cifar(x_u8: torch.Tensor, seed: int) -> torch.Tensor:
     return out.to(torch.uint8)
 
 
+DIRICHLET_MAX_DRAWS = 100
+
+
+def dirichlet_shards(labels, holders: int, alpha: float, batch_size: int, seed: int) -> List[np.ndarray]:
+    """Heterogeneous split of a dataset over ``holders`` (Hsu, Qi and Brown, 2019): for each class c in ascending order, its
+    indices ascending are cut by shares p ~ Dir(alpha 1_H) at ``(cumsum(p)[:-1] * n_c).astype(int)``, and holder h takes chunk
+    h.  When a shard holds fewer than ``batch_size`` samples, every class is drawn again from the same generator, up to
+    ``DIRICHLET_MAX_DRAWS`` draws.  Returns each holder's indices, ascending."""
+    y = np.asarray(labels).reshape(-1)
+    rng = np.random.RandomState((seed * 1000003 + 0xD1C1) & 0x7FFFFFFF)
+    by_class = [np.flatnonzero(y == c) for c in np.unique(y)]
+    for _ in range(DIRICHLET_MAX_DRAWS):
+        parts: List[List[np.ndarray]] = [[] for _ in range(holders)]
+        for idx in by_class:
+            p = rng.dirichlet(np.full(holders, float(alpha)))
+            for h, chunk in enumerate(np.split(idx, (np.cumsum(p)[:-1] * len(idx)).astype(int))):
+                parts[h].append(chunk)
+        shards = [np.sort(np.concatenate(c)) for c in parts]
+        if min(len(s) for s in shards) >= batch_size:
+            return shards
+    raise ValueError(f"--dirichlet-alpha {alpha}: no split of {len(y)} samples over {holders} holders gave every shard at least "
+                     f"B = {batch_size} samples in {DIRICHLET_MAX_DRAWS} draws; raise alpha or the dataset size, or lower the "
+                     f"batch size")
+
+
+def class_histograms(labels, shards: Sequence[np.ndarray]) -> List[List[int]]:
+    """Samples of each class in every shard."""
+    y = np.asarray(labels).reshape(-1)
+    k = int(y.max()) + 1 if len(y) else 0
+    return [np.bincount(y[s], minlength=k).tolist() for s in shards]
+
+
 @dataclass
 class BatchPlan:
     """Maps (step, worker rank) to dataset indices for one approach."""
@@ -139,6 +171,7 @@ class BatchPlan:
     group_seeds: Optional[List[int]] = None
     seed: int = 428
     redundancy: int = 1                       # cyclic: 2s+1
+    shards: Optional[List[np.ndarray]] = None  # --dirichlet-alpha: the dataset indices of every data holder (dirichlet_shards)
 
     def _perm(self, seed: int) -> np.ndarray:
         cache = self.__dict__.setdefault("_perm_cache", {})
@@ -157,8 +190,23 @@ class BatchPlan:
         width = self.batch_size * (self.num_workers if self.approach == "cyclic" else 1)
         return max(self.dataset_size // width, 1)
 
+    def _holder(self, rank: int) -> int:
+        """The data holder of a worker: itself (baseline, nnm), or its repetition group (maj_vote, detox)."""
+        return self.group_of[rank] if self.approach in ("maj_vote", "detox") else rank - 1
+
+    def _shard_indices(self, step: int, rank: int) -> List[np.ndarray]:
+        """Heterogeneous data: the holder's own epochs over its shard, a permutation per epoch seeded as the IID batches are."""
+        shard, B = self.shards[self._holder(rank)], self.batch_size
+        epoch, pos = divmod(max(step - 1, 0), len(shard) // B)
+        seed = (self.group_seeds[self.group_of[rank]] + epoch if self.approach in ("maj_vote", "detox")
+                else self.seed * 1000003 + rank * 7919 + epoch)
+        perm = np.random.RandomState(seed & 0x7FFFFFFF).permutation(len(shard))
+        return [shard[perm[pos * B: (pos + 1) * B]]]
+
     def indices(self, step: int, rank: int) -> List[np.ndarray]:
         """List of index arrays (one per sub-batch this worker computes at ``step``; length 1 unless cyclic)."""
+        if self.shards is not None:
+            return self._shard_indices(step, rank)
         spe = self.steps_per_epoch()
         epoch, pos = divmod(max(step - 1, 0), spe)
         B = self.batch_size

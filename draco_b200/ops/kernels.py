@@ -329,6 +329,136 @@ def _launch_update(a: N.UpdateArgs, layout: ArenaLayout, grad_in: Addr, slot_str
     N.check(N.cuda().drc_aggregate_update(C.byref(a), grid or max(1, min(ntiles, sm_count() * 8)), _stream()), "aggregate_update")
 
 
+WBUCKET_MAXP = 16      # raw slots the fused bucket rules take (the sorting networks' TRIM_MAXP)
+
+
+def wbucket_plan(schedule: torch.Tensor, s: int, *, step_ptr: Addr, masks: torch.Tensor, scales: torch.Tensor) -> None:
+    """--bucketing s: from row ``*step_ptr % len`` of the int32 [len, P] permutation ``schedule`` (codes.bucketing.
+    bucket_schedule), write the step's nb = ceil(P / s) bucket rows into ``masks`` (int32 [nb], bit j = slot j; codes.bucketing.
+    wbucket_masks) and ``scales`` (fp32 [nb], fp32(1 / |b|)), rows ordered by their lowest member.  One single-thread kernel."""
+    if schedule.dim() != 2 or schedule.dtype != torch.int32 or not schedule.is_cuda or not schedule.is_contiguous():
+        raise ValueError("wbucket plan: schedule must be a contiguous int32 CUDA tensor [len, P]")
+    L, P = schedule.shape
+    if not (1 <= P <= WBUCKET_MAXP and 1 <= s <= P and L >= 1):
+        raise ValueError(f"wbucket plan: needs 1 <= s <= P <= {WBUCKET_MAXP} (got P = {P}, s = {s})")
+    nb = -(-P // s)
+    _check_buffer("wbucket plan: masks", masks, torch.int32, (nb,))
+    _check_buffer("wbucket plan: scales", scales, torch.float32, (nb,))
+    a = N.WbucketPlanArgs(schedule.data_ptr(), L, P, s, addr(step_ptr), masks.data_ptr(), scales.data_ptr())
+    N.check(N.cuda().drc_wbucket_plan(C.byref(a), _stream()), "wbucket_plan")
+
+
+def wbucket_update(layout: ArenaLayout, grad_in: Addr, slot_stride: int, *, masks: torch.Tensor, scales: torch.Tensor, trim: int,
+                   params: Addr, momentum: Addr, hp: Addr, step_ptr: Addr, done_counter: Addr, first_step: int = 1,
+                   grad_out: Addr = None, mc_params: Addr = None, dst: Sequence[Addr] = (), flags: Sequence[Addr] = (),
+                   grid: Optional[int] = None, tile_range: Optional[tuple] = None, exp_avg_sq: Addr = None,
+                   max_exp_avg_sq: Addr = None) -> None:
+    """The coordinate-wise trimmed mean / median over the K = nb worker-bucket rows of ``masks`` / ``scales`` (``wbucket_plan``;
+    update-kernel mode 7: each bucket row formed in fp32 from its raw slots, codes/oracle.py ``wbucket_rows``), dropping ``trim``
+    values at each end, scaled by 1 / (nb - 2 trim), + the unchanged optimizer step, broadcast and flags."""
+    nb = masks.shape[0] if masks.dim() == 1 else 0
+    if not (1 <= nb <= WBUCKET_MAXP and 0 <= 2 * trim < nb):
+        raise ValueError(f"wbucket trimmed mean: nb = {nb} rows (at most {WBUCKET_MAXP}) must exceed 2 * trim = {2 * trim}")
+    _check_buffer("wbucket update: masks", masks, torch.int32, (nb,))
+    _check_buffer("wbucket update: scales", scales, torch.float32, (nb,))
+    a = N.UpdateArgs()
+    a.mode, a.trim, a.wb_mask, a.wb_scale = 7, int(trim), masks.data_ptr(), scales.data_ptr()
+    _launch_update(a, layout, grad_in, slot_stride, select=None, K=nb, scale=1.0 / (nb - 2 * trim), recomb=None, params=params,
+                   momentum=momentum, exp_avg_sq=exp_avg_sq, max_exp_avg_sq=max_exp_avg_sq, hp=hp, step_ptr=step_ptr,
+                   first_step=first_step, grad_out=grad_out, mc_params=mc_params, dst=dst, done_counter=done_counter, flags=flags,
+                   tile_range=tile_range, grid=grid)
+
+
+def wbucket_cc_dist(layout: ArenaLayout, grad_in: Addr, slot_stride: int, *, masks: torch.Tensor, scales: torch.Tensor,
+                    center: torch.Tensor, partials: torch.Tensor, tile_range: Optional[tuple] = None,
+                    grid: Optional[int] = None) -> None:
+    """``centered_clip_dist`` over the n = nb worker-bucket rows of ``masks`` / ``scales`` (each row formed in fp32 from its raw
+    slots, codes/oracle.py ``wbucket_rows``; csrc/cuda/clip.cu ``cc_dist_wbucket_kernel``).  ``centered_clip_weights`` /
+    ``centered_clip_model_weights`` then run unchanged with n = nb."""
+    nb = masks.shape[0] if masks.dim() == 1 else 0
+    _check_cc_rows("wbucket_cc_dist", nb)
+    _check_buffer("wbucket_cc_dist: masks", masks, torch.int32, (nb,))
+    _check_buffer("wbucket_cc_dist: scales", scales, torch.float32, (nb,))
+    _check_buffer("wbucket_cc_dist: center", center, torch.float32, (layout.total,))
+    _check_buffer("wbucket_cc_dist: partials", partials, torch.float64, (layout.ntiles, nb))
+    a = N.CcArgs()
+    a.grad_in, a.slot_stride, a.n = addr(grad_in), slot_stride, nb
+    a.tv = layout.tile_view(center.device)
+    a.center, a.partials, a.wb_mask, a.wb_scale = center.data_ptr(), partials.data_ptr(), masks.data_ptr(), scales.data_ptr()
+    ntiles = layout.ntiles
+    if tile_range is not None:
+        a.tile_begin, a.tile_end = int(tile_range[0]), int(tile_range[1])
+        ntiles = a.tile_end - a.tile_begin
+    N.check(N.cuda().drc_cc_dist(C.byref(a), grid or max(1, min(ntiles, sm_count() * 8)), _stream()), "cc_dist")
+
+
+def wbucket_cc_update(layout: ArenaLayout, grad_in: Addr, slot_stride: int, *, masks: torch.Tensor, scales: torch.Tensor,
+                      center: torch.Tensor, weights: torch.Tensor, params: Addr, momentum: Addr, hp: Addr, step_ptr: Addr,
+                      done_counter: Addr, first_step: int = 1, grad_out: Addr = None, mc_params: Addr = None,
+                      dst: Sequence[Addr] = (), flags: Sequence[Addr] = (), grid: Optional[int] = None,
+                      tile_range: Optional[tuple] = None, exp_avg_sq: Addr = None, max_exp_avg_sq: Addr = None) -> None:
+    """``centered_clip_update`` over the K = nb worker-bucket rows (update-kernel mode 8): a bucket of weight 0 is never read,
+    the others are formed in fp32 from their raw slots as in ``wbucket_update``."""
+    nb = masks.shape[0] if masks.dim() == 1 else 0
+    _check_cc_rows("wbucket_cc_update", nb)
+    _check_buffer("wbucket_cc_update: masks", masks, torch.int32, (nb,))
+    _check_buffer("wbucket_cc_update: scales", scales, torch.float32, (nb,))
+    _check_buffer("wbucket_cc_update: center", center, torch.float32, (layout.total,))
+    _check_buffer("wbucket_cc_update: weights", weights, torch.float32, (layout.ntensors, nb))
+    a = N.UpdateArgs()
+    a.mode, a.center, a.wb_mask, a.wb_scale = 8, center.data_ptr(), masks.data_ptr(), scales.data_ptr()
+    _launch_update(a, layout, grad_in, slot_stride, select=None, K=nb, scale=1.0, recomb=weights, params=params,
+                   momentum=momentum, exp_avg_sq=exp_avg_sq, max_exp_avg_sq=max_exp_avg_sq, hp=hp, step_ptr=step_ptr,
+                   first_step=first_step, grad_out=grad_out, mc_params=mc_params, dst=dst, done_counter=done_counter, flags=flags,
+                   tile_range=tile_range, grid=grid)
+
+
+def wbucket_table(layout: ArenaLayout, P: int, *, masks: torch.Tensor, raw_d2: torch.Tensor, wb_d2: torch.Tensor) -> None:
+    """The nb bucket rows' pair table ``wb_d2`` [T, nb(nb-1)/2] fp64 from the raw slots' table ``raw_d2`` [T, P(P-1)/2]
+    (``pair_dist``, then ``pair_scope_fold`` at model scope), which it zeroes: -1/2 c^T D c clamped at 0 (codes/oracle.py
+    ``wbucket_pair_d2``; csrc/cuda/bucketing.cu).  ``krum_select`` / ``geometric_median_weights`` then read ``wb_d2`` with
+    ``filled=True``."""
+    nb = masks.shape[0] if masks.dim() == 1 else 0
+    if not 2 <= nb <= P <= WBUCKET_MAXP:
+        raise ValueError(f"wbucket_table: needs 2 <= nb <= P <= {WBUCKET_MAXP} (got nb = {nb}, P = {P})")
+    _check_buffer("wbucket_table: masks", masks, torch.int32, (nb,))
+    _check_pair_table("wbucket_table: raw", layout, P, raw_d2)
+    _check_pair_table("wbucket_table: bucket", layout, nb, wb_d2)
+    a = N.WbucketArgs(masks.data_ptr(), nb, P, layout.ntensors, raw_d2.data_ptr(), wb_d2.data_ptr())
+    N.check(N.cuda().drc_wbucket_table(C.byref(a), _stream()), "wbucket_table")
+
+
+def wbucket_fold(layout: ArenaLayout, P: int, *, masks: torch.Tensor, weights: torch.Tensor, select: Optional[torch.Tensor] = None,
+                 m: int = 0, wsel: Optional[torch.Tensor] = None, w_rows: Optional[torch.Tensor] = None) -> None:
+    """A choice over the bucket rows as weights over the raw slots (w_b / |b|, formed in fp64, rounded to fp32 once;
+    csrc/cuda/bucketing.cu).  Krum / multi-Krum (``select``: int32 [m, T] bucket rows): the compact ``wsel`` int32 [K, T] slots
+    and ``weights`` fp32 [T, K], K = min(m s, P), padded with weight 0 on a chosen slot, for ``aggregate_update(K=K,
+    weights=weights, select=wsel)``.  Geometric median (``w_rows``: fp32 [T, nb]): ``weights`` fp32 [T, P] over every slot."""
+    nb, T = (masks.shape[0] if masks.dim() == 1 else 0), layout.ntensors
+    if not 1 <= nb <= P <= WBUCKET_MAXP:
+        raise ValueError(f"wbucket_fold: needs 1 <= nb <= P <= {WBUCKET_MAXP} (got nb = {nb}, P = {P})")
+    _check_buffer("wbucket_fold: masks", masks, torch.int32, (nb,))
+    a = N.WbucketArgs()
+    a.masks, a.nb, a.P, a.T = masks.data_ptr(), nb, P, T
+    if (select is None) == (w_rows is None):
+        raise ValueError("wbucket_fold: pass either select (Krum / multi-Krum) or w_rows (geometric median)")
+    if select is not None:
+        if not 1 <= m <= nb:
+            raise ValueError(f"wbucket_fold: needs 1 <= m <= nb = {nb}, got {m}")
+        _check_buffer("wbucket_fold: select", select, torch.int32, (m, T))
+        K = wsel.shape[0] if isinstance(wsel, torch.Tensor) and wsel.dim() == 2 else 0
+        if not 1 <= K <= P:
+            raise ValueError(f"wbucket_fold: wsel must be int32 [K, T] with 1 <= K <= P = {P}")
+        _check_buffer("wbucket_fold: wsel", wsel, torch.int32, (K, T))
+        _check_buffer("wbucket_fold: weights", weights, torch.float32, (T, K))
+        a.select, a.m, a.wsel, a.wts, a.K = select.data_ptr(), m, wsel.data_ptr(), weights.data_ptr(), K
+    else:
+        _check_buffer("wbucket_fold: w_rows", w_rows, torch.float32, (T, nb))
+        _check_buffer("wbucket_fold: weights", weights, torch.float32, (T, P))
+        a.w_rows, a.wts = w_rows.data_ptr(), weights.data_ptr()
+    N.check(N.cuda().drc_wbucket_fold(C.byref(a), _stream()), "wbucket_fold")
+
+
 SIGN_VOTE_MAXP = N.MAX_WORKERS
 
 

@@ -290,7 +290,7 @@ class CollectiveEngine:
             elif self.use_adv and self.cfg.err_mode in PS_ATTACKS:
                 self._ps_attack(step)
             with self._phase("t_decode"):                 # reference: "Method Time Cost"
-                grads = self.ps.aggregate(self.slots)
+                grads = self.ps.aggregate(self.slots, step=step)
             with self._phase("t_update"):                 # reference: "Update Time Cost"
                 self.ps.apply(grads)
         if self.timer:

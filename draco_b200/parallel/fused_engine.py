@@ -35,7 +35,7 @@ import torch.distributed as dist
 
 from ..codes.adversary import ATTACK_OMNISCIENT, PS_ATTACKS, attack_code, generate_schedule
 from ..config import JobConfig
-from ..data import BatchPlan, TensorDataset
+from ..data import BatchPlan, TensorDataset, dirichlet_shards
 from ..ops import conv as _conv_ops
 from ..ops import kernels as K
 from ..utils.metrics import PhaseTimer, limit_host_threads, wait_event
@@ -635,7 +635,11 @@ class FusedEngine:
 
 def make_plan(cfg: JobConfig, dataset: Optional[TensorDataset], groups) -> BatchPlan:
     n = len(dataset) if dataset is not None else cfg.synthetic_size
+    shards = None
+    if cfg.dirichlet_alpha is not None and dataset is not None:   # --dirichlet-alpha: one shard per worker, or per group
+        holders = len(groups.groups) if groups is not None else cfg.num_workers
+        shards = dirichlet_shards(dataset.labels.numpy(), holders, cfg.dirichlet_alpha, cfg.batch_size, cfg.seed)
     return BatchPlan(cfg.approach, n, cfg.batch_size, cfg.num_workers,
                      group_of=groups.rank_to_group if groups is not None else None,
                      group_seeds=groups.seeds if groups is not None else None,
-                     seed=428, redundancy=cfg.redundancy if cfg.approach == "cyclic" else 1)
+                     seed=428, redundancy=cfg.redundancy if cfg.approach == "cyclic" else 1, shards=shards)

@@ -20,9 +20,10 @@ import torch
 
 from .. import _native as N
 from ..codes.adversary import ATTACK_ALIE, ATTACK_MINMAX, PS_ATTACKS, attack_code
+from ..codes.bucketing import bucket_schedule, wbuckets
 from ..codes.cyclic import CyclicCode, search_w
 from ..codes.oracle import (_bulyan_rounds, _krum_scores_d2, _weiszfeld_weights, centered_clip_weight, model_d2,
-                            nnm_neighbours_d2, nnm_pair_d2)
+                            nnm_neighbours_d2, nnm_pair_d2, wbucket_pair_d2)
 from ..codes.repetition import GroupPlan
 from ..config import JobConfig
 from .arena import ArenaLayout
@@ -63,6 +64,9 @@ NNM_RULES = {"coordinate_median": "nnm_median", "trimmed_mean": "nnm_trimmed_mea
 PIPELINED_RULES = ("mean", "vote", "median", "trimmed_mean", "detox_median", "detox_trimmed_mean", "centered_clip",
                    "detox_centered_clip", "sign_vote")
 
+# the base rules FusedPS runs over worker buckets (every --bucketing rule)
+WBUCKET_FUSED_BASES = ("median", "trimmed_mean", "krum", "multi_krum", "geomedian", "centered_clip")
+
 # the optimizer's mode string for each base rule (SGDModified / AdamModified.step(mode=))
 _OPT_MODE = {"mean": "normal", "vote": "maj_vote", "cyclic": "cyclic", "median": "coordinate_median", "trimmed_mean": "trimmed_mean",
              "krum": "krum", "multi_krum": "multi_krum", "geomedian": "geometric_median", "bulyan": "bulyan",
@@ -73,10 +77,11 @@ _OPT_MODE = {"mean": "normal", "vote": "maj_vote", "cyclic": "cyclic", "median":
 class RulePlan:
     """A job's aggregation rule as a row source and a base rule, with every parameter worked out once."""
     rule: str           # select_rule's name
-    source: str         # raw: the P worker slots | detox: the G group winners of the vote | nnm: the P mixed rows
+    source: str         # raw: the P worker slots | detox: the G group winners of the vote | nnm: the P mixed rows |
+                        # wbucket: the nb = ceil(P / s) worker-bucket means of --bucketing s
     base: str           # mean | vote | cyclic | median | trimmed_mean | krum | multi_krum | geomedian | bulyan | centered_clip |
                         # sign_vote
-    rows: int           # rows the base rule runs on: P, or G over the group winners
+    rows: int           # rows the base rule runs on: P, G over the group winners, or nb over the worker buckets
     f: int              # rows it tolerates: worker_fail, or b_G over the group winners
     trim: int           # median / trimmed mean: values dropped at each end of a coordinate
     m: int              # Krum / multi-Krum: rows averaged
@@ -96,13 +101,16 @@ def rule_plan(cfg: JobConfig) -> RulePlan:
         source, base = "detox", rule.removeprefix("detox_")
     elif rule.startswith("nnm_"):
         source, base = "nnm", rule.removeprefix("nnm_")
-    rows = cfg.num_groups if source == "detox" else cfg.num_workers
+    elif cfg.bucketing:                                   # --bucketing s: the rule runs on the nb worker-bucket means
+        source, rule = "wbucket", "wbucket_" + rule
+    rows = {"detox": cfg.num_groups, "wbucket": -(-cfg.num_workers // max(cfg.bucketing, 1))}.get(source, cfg.num_workers)
     f = cfg.captured_group_bound if source == "detox" else cfg.worker_fail
     trim = {"median": (rows - 1) // 2, "trimmed_mean": f}.get(base, 0)
     m = {"krum": 1, "multi_krum": rows - f}.get(base, 0)
     scope, attack_scope = cfg.rule_scope, cfg.attack_scope
     return RulePlan(rule, source, base, rows, f, trim, m, rows - 2 * f if base == "bulyan" else 0, _OPT_MODE[base],
-                    rule in PIPELINED_RULES and scope == "tensor" and attack_scope == "tensor", scope, attack_scope)
+                    rule.removeprefix("wbucket_") in PIPELINED_RULES and scope == "tensor" and attack_scope == "tensor", scope,
+                    attack_scope)
 
 
 def hyperparams_tensor(cfg: JobConfig, device) -> torch.Tensor:
@@ -155,6 +163,10 @@ class FusedPS:
             self.winner_member = torch.zeros(G, T, dtype=torch.int32, device=device)
         elif plan.source == "nnm":
             self.mix = torch.zeros(self.P, T, dtype=torch.int32, device=device)
+        elif plan.source == "wbucket":                    # the permutation table, and the step's bucket rows (wbucket_plan)
+            self.wb_schedule = torch.from_numpy(bucket_schedule(self.P, cfg.max_steps, cfg.seed)).to(device)
+            self.wb_mask = torch.zeros(plan.rows, dtype=torch.int32, device=device)
+            self.wb_scale = torch.zeros(plan.rows, dtype=torch.float32, device=device)
         # base rule.  The geometric median of more than GEOMED_FAST_MAXP rows streams over the slab once per Weiszfeld iteration;
         # every other choice starts from the table of pairwise distances between the rows
         rows = plan.rows
@@ -173,8 +185,19 @@ class FusedPS:
             self.cc_weights = torch.zeros(T, rows, dtype=torch.float32, device=device)
             if plan.scope == "model":                     # the per-tensor d_i the whole-model norm is summed from
                 self.cc_dist = torch.zeros(T, rows, dtype=torch.float64, device=device)
-        if plan.source == "nnm" and plan.base in ("krum", "multi_krum", "geomedian"):
+        if plan.source in ("nnm", "wbucket") and plan.base in ("krum", "multi_krum", "geomedian"):
             self.w_raw = torch.zeros(T, self.P, dtype=torch.float32, device=device)   # the choice, folded into raw-slot weights
+        if plan.source == "wbucket" and plan.base in ("krum", "multi_krum", "geomedian"):
+            # the raw slots' pair table, turned into the bucket rows' table (pair_d2) by wbucket_table
+            self.wb_raw_d2 = torch.zeros(T, self.P * (self.P - 1) // 2, dtype=torch.float64, device=device)
+            if plan.base == "geomedian" and rows == 1:    # one bucket holds every slot: its Weiszfeld weight is 1
+                self.gm_weights.fill_(1.0)
+            if plan.base != "geomedian":                  # Krum / multi-Krum: the compact table of the chosen buckets' slots
+                kc = min(plan.m * cfg.bucketing, self.P)
+                self.wb_wsel = torch.zeros(kc, T, dtype=torch.int32, device=device)
+                self.w_raw = torch.zeros(T, kc, dtype=torch.float32, device=device)
+        if plan.source == "wbucket" and plan.base not in WBUCKET_FUSED_BASES:
+            raise ValueError(f"FusedPS: no fused worker-bucket build of the {plan.base} rule")
         if plan.base == "cyclic":
             self.code = code
             self.E = torch.zeros(T, self.P, 2, dtype=torch.float64, device=device)
@@ -213,6 +236,9 @@ class FusedPS:
         nnm = plan.source == "nnm"
         model = plan.scope == "model"                     # one choice for every tensor, from the whole-model distances
         n = 0
+        if plan.source == "wbucket":                      # the step's worker buckets, before the first gradient bucket arrives
+            K.wbucket_plan(self.wb_schedule, self.cfg.bucketing, step_ptr=step_ptr, masks=self.wb_mask, scales=self.wb_scale)
+            n += 1
         for bi, (tiles, tensors) in enumerate(ranges):
             last = bi == len(ranges) - 1
             if pipelined:
@@ -240,7 +266,15 @@ class FusedPS:
                           mixed_out=plan.base not in ("median", "trimmed_mean")); n += 2
             # model scope: the pair table summed over the tensors and written back into each, then filled=True below
             filled = nnm
-            if model and not nnm and plan.base in ("krum", "multi_krum", "geomedian", "bulyan"):
+            wb_choice = plan.source == "wbucket" and plan.base in ("krum", "multi_krum", "geomedian")
+            if wb_choice and plan.rows > 1:                # the raw table, folded at model scope, then the bucket rows' table
+                K.pair_dist(L, self.grad_in, self.slot_stride, self.P, self.wb_raw_d2)
+                n += 1
+                if model:
+                    K.pair_scope_fold(L, self.P, self.wb_raw_d2); n += 1
+                K.wbucket_table(L, self.P, masks=self.wb_mask, raw_d2=self.wb_raw_d2, wb_d2=self.pair_d2); n += 1
+            filled = filled or wb_choice
+            if model and not nnm and not wb_choice and plan.base in ("krum", "multi_krum", "geomedian", "bulyan"):
                 K.pair_dist(L, self.grad_in, self.slot_stride, plan.rows, self.pair_d2, rows=rows)
                 K.pair_scope_fold(L, plan.rows, self.pair_d2); n += 2
                 filled = True
@@ -257,12 +291,18 @@ class FusedPS:
             elif plan.base in ("median", "trimmed_mean"):   # coordinate-wise: element by element, nothing per tensor
                 agg.update(scale=1.0 / (plan.rows - 2 * plan.trim), trim=plan.trim)
             elif plan.base == "centered_clip" and model:   # one norm over the whole model, after the last bucket
-                K.centered_clip_dist(L, self.grad_in, self.slot_stride, plan.rows, self.cc_center, self.cc_partials, rows=rows)
+                if plan.source == "wbucket":
+                    self._wbucket_cc_dist(None)
+                else:
+                    K.centered_clip_dist(L, self.grad_in, self.slot_stride, plan.rows, self.cc_center, self.cc_partials, rows=rows)
                 K.centered_clip_model_weights(L, plan.rows, self.cfg.clip_tau, self.cc_partials, self.cc_dist, self.cc_weights)
                 n += 3
             elif plan.base == "centered_clip":             # per tensor, from the n distances to the centre: bucket by bucket
-                K.centered_clip_dist(L, self.grad_in, self.slot_stride, plan.rows, self.cc_center, self.cc_partials, rows=rows,
-                                     tile_range=tiles)
+                if plan.source == "wbucket":
+                    self._wbucket_cc_dist(tiles)
+                else:
+                    K.centered_clip_dist(L, self.grad_in, self.slot_stride, plan.rows, self.cc_center, self.cc_partials, rows=rows,
+                                         tile_range=tiles)
                 K.centered_clip_weights(L, plan.rows, self.cfg.clip_tau, self.cc_partials, self.cc_weights,
                                         tensor_range=tensors); n += 2
             elif plan.base == "bulyan":                    # select holds the rows Bulyan keeps
@@ -275,7 +315,9 @@ class FusedPS:
                 src = self.gm.median
                 agg.update(K=1, scale=1.0)
             else:                                          # geometric median weights, or the m best Krum rows
-                if plan.base == "geomedian":
+                if plan.base == "geomedian" and plan.rows == 1:
+                    n -= 1                                 # one bucket: its weight is 1, nothing to choose
+                elif plan.base == "geomedian":
                     K.geometric_median_weights(L, self.grad_in, self.slot_stride, plan.rows, self.pair_d2, self.gm_weights,
                                                rows=rows, filled=filled)
                     choice = dict(w_mix=self.gm_weights)
@@ -289,6 +331,13 @@ class FusedPS:
                 if nnm:                                    # a choice over the mixed rows, as weights over the raw slots
                     K.nnm_fold(L, self.P, plan.f, self.mix, self.w_raw, **choice); n += 1
                     agg = dict(K=self.P, scale=1.0, weights=self.w_raw)
+                elif wb_choice and plan.base == "geomedian":   # the bucket rows' weights over every raw slot
+                    K.wbucket_fold(L, self.P, masks=self.wb_mask, weights=self.w_raw, w_rows=self.gm_weights); n += 1
+                    agg = dict(K=self.P, scale=1.0, weights=self.w_raw)
+                elif wb_choice:                            # the chosen buckets' slots only, so no other slot is read
+                    K.wbucket_fold(L, self.P, masks=self.wb_mask, weights=self.w_raw, select=self.select, m=plan.m,
+                                   wsel=self.wb_wsel); n += 1
+                    agg = dict(K=self.wb_wsel.shape[0], scale=1.0, weights=self.w_raw, select=self.wb_wsel)
             if nnm and plan.base in ("median", "trimmed_mean", "bulyan"):
                 agg.update(mix=self.mix, mix_f=plan.f)
             if last:
@@ -296,13 +345,24 @@ class FusedPS:
             if plan.base == "sign_vote":                   # the vote over the P sign rows is the update's gradient source
                 K.sign_vote_update(L, self.grad_in, self.slot_stride, P=plan.rows, tile_range=tiles, flags=flags if last else [],
                                    **common)
+            elif plan.base == "centered_clip" and plan.source == "wbucket":
+                K.wbucket_cc_update(L, src, self.slot_stride, masks=self.wb_mask, scales=self.wb_scale, center=self.cc_center,
+                                    weights=self.cc_weights, tile_range=tiles, flags=flags if last else [], **common)
             elif plan.base == "centered_clip":             # the update reads and replaces the centre
                 K.centered_clip_update(L, src, self.slot_stride, center=self.cc_center, weights=self.cc_weights, K=plan.rows,
                                        select=rows, tile_range=tiles, flags=flags if last else [], **common)
+            elif plan.source == "wbucket" and plan.base in ("median", "trimmed_mean"):   # bucket rows formed in the kernel
+                K.wbucket_update(L, self.grad_in, self.slot_stride, masks=self.wb_mask, scales=self.wb_scale, trim=plan.trim,
+                                 tile_range=tiles, flags=flags if last else [], **common)
             else:
                 K.aggregate_update(L, src, self.slot_stride, tile_range=tiles, flags=flags if last else [], **agg, **common)
             n += 1
         return n
+
+    def _wbucket_cc_dist(self, tiles) -> None:
+        """Centered clipping's row-to-centre partials of the bucket rows over ``tiles`` (None: the arena)."""
+        self.K.wbucket_cc_dist(self.layout, self.grad_in, self.slot_stride, masks=self.wb_mask, scales=self.wb_scale,
+                               center=self.cc_center, partials=self.cc_partials, tile_range=tiles)
 
 
 # =====================================================================================================
@@ -330,6 +390,8 @@ class TorchPS:
                                          dampening=cfg.dampening, nesterov=cfg.nesterov)
         # centered clipping's centre: last step's aggregate, +0 at the start (PS state, checkpointed as opt_state["cc_center"])
         self.cc_center = layout.new_arena(device) if self.plan.base == "centered_clip" else None
+        # --bucketing: the permutation of every step (row step % len, as the fused PS reads it)
+        self.wb_schedule = bucket_schedule(self.P, cfg.max_steps, cfg.seed) if self.plan.source == "wbucket" else None
         if self.plan.base == "cyclic":
             g = torch.Generator().manual_seed(cfg.seed + 4242)
             f = (torch.randn(layout.total, generator=g) + 1.0) * torch.from_numpy(layout.valid_mask()).float()
@@ -543,16 +605,44 @@ class TorchPS:
             out.append(torch.where(n_pos > n_neg, one, torch.where(n_neg > n_pos, -one, torch.zeros_like(one))))
         return out
 
-    def aggregate(self, slots: torch.Tensor) -> List[torch.Tensor]:
+    def _wbuckets(self, step: Optional[int]) -> List[List[int]]:
+        """The worker buckets of ``step`` (``codes.bucketing.wbuckets`` of the schedule's row step % len)."""
+        if step is None:
+            raise ValueError("--bucketing: aggregate() needs the step, which picks the permutation")
+        return wbuckets(self.wb_schedule[step % len(self.wb_schedule)], self.cfg.bucketing)
+
+    @staticmethod
+    def _wbucket_rows(X: torch.Tensor, buckets: List[List[int]]) -> torch.Tensor:
+        """The fp32 bucket rows (``oracle.wbucket_rows``): the lowest member, plus the others in ascending slot order, each add
+        rounded, then one rounded multiply by fp32(1 / |b|); a one-member bucket's row is its member, bit for bit."""
+        Y = torch.empty((len(buckets),) + tuple(X.shape[1:]), dtype=X.dtype, device=X.device)
+        for b, members in enumerate(buckets):
+            y = X[members[0]].clone()
+            for j in members[1:]:
+                y = y + X[j]
+            Y[b] = y if len(members) == 1 else y * torch.tensor(1.0 / len(members), dtype=torch.float32, device=X.device)
+        return Y
+
+    def _wbucket_choice(self, Y: torch.Tensor, Db: np.ndarray) -> torch.Tensor:
+        """Krum / multi-Krum / the geometric median on the bucket rows ``Y`` from their fp64 table ``Db``."""
+        plan = self.plan
+        if plan.base in ("krum", "multi_krum"):
+            best = np.argsort(_krum_scores_d2(Db, plan.f), kind="stable")[:plan.m].tolist()
+            return Y[best[0]] if plan.base == "krum" else Y[best].sum(0) / plan.m
+        w = torch.from_numpy(_weiszfeld_weights(Db, 1e-10, 256)).float().to(Y.device)
+        return (w[:, None] * Y).sum(0)
+
+    def aggregate(self, slots: torch.Tensor, step: Optional[int] = None) -> List[torch.Tensor]:
         """``slots``: [P, D] fp32 (or [P, D] complex64 for cyclic, or [P, D / 8] sign bytes for sign_vote).  Returns the
         per-tensor aggregated gradients: per tensor the rows of the row source (the worker slots, the group winners of the vote,
-        or the mixed rows), then the base rule's helper on them."""
+        the mixed rows, or the worker-bucket means of ``step``'s permutation), then the base rule's helper on them."""
         plan = self.plan
         self.last_info = {}
         if plan.base == "sign_vote":
             return self._sign_vote(slots)
         if plan.scope == "model":
-            return self._aggregate_model(slots)
+            return self._aggregate_model(slots, step)
+        buckets = self._wbuckets(step) if plan.source == "wbucket" else None
         out = []
         for spec in self.layout.specs:
             X = slots[:, spec.offset: spec.offset + spec.numel]
@@ -560,6 +650,12 @@ class TorchPS:
                 X = self._detox_rows(X)
             elif plan.source == "nnm":
                 X = self._nnm_mix_tensor(X, plan.f)
+            elif buckets is not None:
+                Y = self._wbucket_rows(X, buckets)
+                if plan.base in ("krum", "multi_krum", "geomedian"):   # distances from the raw table (oracle.wbucket_pair_d2)
+                    out.append(self._wbucket_choice(Y, _wbucket_table(_pair_d2(X), buckets, self.P)))
+                    continue
+                X = Y
             if plan.base == "mean":
                 g = X.sum(0) / plan.rows
             elif plan.base == "vote":                    # the winners summed in group order, then divided by G
@@ -592,15 +688,27 @@ class TorchPS:
             winners.append(rows[self._vote_tensor(rows)])
         return torch.stack(winners)
 
-    def _aggregate_model(self, slots: torch.Tensor) -> List[torch.Tensor]:
-        """``--rule-scope model``: the rows of every tensor (worker slots, or the per-tensor vote winners), one choice from the
-        whole-model distances -- the per-tensor fp64 distances summed in ascending tensor order (``oracle.model_d2``) -- and
-        that choice applied to every tensor: Krum / multi-Krum rows, Bulyan's theta rows (then its per-tensor coordinate
-        stage), NNM neighbourhoods (then the rule on the mixed rows), the Weiszfeld weights, centered clipping's weights."""
+    def _aggregate_model(self, slots: torch.Tensor, step: Optional[int] = None) -> List[torch.Tensor]:
+        """``--rule-scope model``: the rows of every tensor (worker slots, the per-tensor vote winners, or the worker-bucket
+        means), one choice from the whole-model distances -- the per-tensor fp64 distances summed in ascending tensor order
+        (``oracle.model_d2``) -- and that choice applied to every tensor: Krum / multi-Krum rows, Bulyan's theta rows (then its
+        per-tensor coordinate stage), NNM neighbourhoods (then the rule on the mixed rows), the Weiszfeld weights, centered
+        clipping's weights.  Worker buckets take their table from the whole-model raw table (``oracle.wbucket_pair_d2``)."""
         plan, specs = self.plan, self.layout.specs
         Xs = [slots[:, s.offset: s.offset + s.numel] for s in specs]
         if plan.source == "detox":
             Xs = [self._detox_rows(X) for X in Xs]
+        if plan.source == "wbucket":
+            buckets = self._wbuckets(step)
+            Ys = [self._wbucket_rows(X, buckets) for X in Xs]
+            if plan.base != "centered_clip":
+                Db = _wbucket_table(model_d2([_pair_d2(X) for X in Xs]), buckets, self.P)
+                if plan.base in ("krum", "multi_krum"):
+                    best = np.argsort(_krum_scores_d2(Db, plan.f), kind="stable")[:plan.m].tolist()
+                    return [Y[best[0]] if plan.base == "krum" else Y[best].sum(0) / plan.m for Y in Ys]
+                w = torch.from_numpy(_weiszfeld_weights(Db, 1e-10, 256)).float().to(slots.device)
+                return [(w[:, None] * Y).sum(0) for Y in Ys]
+            Xs = Ys
         if plan.base == "centered_clip":
             vs = [self.cc_center[s.offset: s.offset + s.numel] for s in specs]
             d = model_d2([(X.double() - v.double()).pow(2).sum(1).cpu().numpy() for X, v in zip(Xs, vs)])
@@ -624,8 +732,8 @@ class TorchPS:
         w = torch.from_numpy(_weiszfeld_weights(D, 1e-10, 256)).float().to(slots.device)
         return [(w[:, None] * X).sum(0) for X in Xs]
 
-    def step(self, slots: torch.Tensor) -> None:
-        self.apply(self.aggregate(slots))
+    def step(self, slots: torch.Tensor, step: Optional[int] = None) -> None:
+        self.apply(self.aggregate(slots, step=step))
 
     def apply(self, grads: List[torch.Tensor]) -> None:
         self.optimizer.step(grads=grads, mode=self.plan.opt_mode)
@@ -637,6 +745,23 @@ def _pair_d2(X: torch.Tensor) -> np.ndarray:
     D = torch.stack([((X64 - X64[i]) ** 2).sum(1) for i in range(X.shape[0])]).cpu().numpy()
     np.fill_diagonal(D, 0.0)                           # a row holding NaN or Inf is NaN off the diagonal only
     return D
+
+
+def _wbucket_table(D: np.ndarray, buckets: List[List[int]], P: int) -> np.ndarray:
+    """[nb, nb] fp64 squared distances between the bucket rows from the raw table ``D`` [P, P]: with M = A D A^T (row b of A
+    is 1 / |b| on b's members), ||y_b - y_k||^2 = M_bk - (M_bb + M_kk) / 2, clamped at 0.  A non-finite entry anywhere in D
+    would reach every entry of the products, so such a table takes the per-pair form of ``oracle.wbucket_pair_d2``, which
+    only reads the members of b and k."""
+    if not np.isfinite(D).all():
+        return wbucket_pair_d2(D, buckets, P)
+    A = np.zeros((len(buckets), P))
+    for b, members in enumerate(buckets):
+        A[b, members] = 1.0 / len(members)
+    M = A @ D @ A.T
+    d = np.diag(M)
+    Db = np.maximum(M - 0.5 * (d[:, None] + d[None, :]), 0.0)
+    np.fill_diagonal(Db, 0.0)
+    return Db
 
 
 def _fma_f32(w: float, b: torch.Tensor, c: torch.Tensor) -> torch.Tensor:

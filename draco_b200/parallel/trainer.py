@@ -20,7 +20,7 @@ import torch
 import torch.distributed as dist
 
 from ..config import JobConfig
-from ..data import TensorDataset, load_dataset
+from ..data import TensorDataset, class_histograms, load_dataset
 from ..utils.checkpoint import (arena_tensors, check_cc_center, check_worker_momentum, checkpoint_path, load_checkpoint,
                                 model_buffers, restore_into, restore_worker_momentum, save_checkpoint)
 from ..utils.metrics import MetricsLogger
@@ -83,6 +83,9 @@ class Trainer:
             from .collective_engine import CollectiveEngine
             self.engine = CollectiveEngine(cfg, rank, world, self.device, dataset)
         self.logger = MetricsLogger(cfg.metrics_file, rank, cfg.log_interval, quiet)
+        plan = getattr(getattr(self.engine, "worker", None), "plan", None)
+        if plan is not None and plan.shards is not None:    # --dirichlet-alpha: every holder's class counts, once
+            self.logger.log(0, "data", class_hist=class_histograms(dataset.labels.numpy(), plan.shards))
         self.is_ps = rank == 0
         self.eval_rank = self.engine.place.proc_of[1]          # the process hosting worker 1 evaluates (reference: rank 1)
         if cfg.checkpoint_step > 0:
