@@ -7,6 +7,8 @@
 //   min-max (Shejwalkar & Houmansadr, NDSS 2021):  mu - gamma * sigma, with the largest gamma such that no honest row is
 //            farther from it than the largest honest pairwise distance Dmax (per tensor; closed form, see attack_solve_kernel)
 //            three kernels: stats (mu, sigma + per-tile fp64 partials) -> solve (one CTA per tensor) -> write
+//   IPM     (Xie, Koyejo and Gupta, UAI 2019):     -eps * mu                            one pass: attack_ipm_kernel
+// (mimic, which copies one honest slot, is in mimic.cu)
 //
 // Determinism: every per-coordinate statistic is a fixed-order fp64 sum over the honest rows in slot order, with the
 // roundings of the oracle (no contracted multiply-adds), so an ALIE row is the oracle's fp64 row rounded to fp32; the per-tensor
@@ -19,17 +21,18 @@
 #define ATTACK_MAXQ ATTACK_NQ(ATTACK_MAXP)
 #define ATTACK_ALIE 5                                             // ATTACK_* codes of codes/adversary.py
 #define ATTACK_MINMAX 6
+#define ATTACK_IPM 7
 
 struct AttackArgs {
   float* grad_in;                         // [P][slot_stride] worker slots (PS memory)
   long long slot_stride;
   int P;
-  int mode;                               // ATTACK_ALIE | ATTACK_MINMAX
+  int mode;                               // ATTACK_ALIE | ATTACK_MINMAX | ATTACK_IPM
   TileView tv;
   const unsigned int* adv_bitmap;         // [adv_len] liar bitmap per step (bit w = slot w lies)
   int adv_len;
   const unsigned long long* step_ptr;
-  double z;                               // ALIE's z
+  double z;                               // ALIE's z; IPM's eps
   float* stats;                           // min-max: [2][slot_stride] mu, sigma (fp32)
   double* partials;                       // min-max: [ntiles][ATTACK_NQ(P)]
   double* gamma;                          // min-max: [ntensors]
@@ -304,15 +307,50 @@ __global__ void __launch_bounds__(DRC_THREADS) attack_write_kernel(const __grid_
   }
 }
 
+// IPM, inner-product manipulation (Xie, Koyejo and Gupta, UAI 2019): every liar sends fp32(-eps * mu), mu the honest mean of
+// ALIE's kernel (the same fp64 sum in slot order, one rounded division); a.z holds eps.  Coordinate-wise, so it runs per
+// gradient bucket like ALIE.  Its own kernel, so that attack_stats_kernel's machine code stays what it was.
+__global__ void __launch_bounds__(DRC_THREADS) attack_ipm_kernel(const __grid_constant__ AttackArgs a) {
+  const unsigned int liars = liar_mask(a);
+  const unsigned int honest = ~liars & ((1u << a.P) - 1u);
+  if (liars == 0u || honest == 0u) return;
+  const double nh = (double)__popc(honest);
+  const int tile_end = a.tile_end > 0 ? a.tile_end : a.tv.ntiles;
+  for (int tile = a.tile_begin + blockIdx.x; tile < tile_end; tile += gridDim.x) {
+    int tensor;
+    const int valid = tile_valid(a.tv, tile, tensor);
+    const long long idx = (long long)tile * DRC_TILE + threadIdx.x * 4;
+    const int lane_valid = valid - (int)threadIdx.x * 4;
+    if (lane_valid <= 0) continue;
+    double mu[4] = {0.0, 0.0, 0.0, 0.0};
+    for (int i = 0; i < a.P; ++i)
+      if ((honest >> i) & 1u) {
+        const float4 v = ld_f4(reinterpret_cast<const float4*>(a.grad_in + i * a.slot_stride + idx));
+#pragma unroll
+        for (int k = 0; k < 4; ++k) mu[k] += (double)lane_of(v, k);       // padding lanes are summed but never stored
+      }
+    float r[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) r[k] = (float)__dmul_rn(-a.z, mu[k] / nh);
+    for (int w = 0; w < a.P; ++w)
+      if ((liars >> w) & 1u) store_row(a.grad_in + w * a.slot_stride + idx, r, lane_valid);
+  }
+}
+
 static bool attack_args_ok(const AttackArgs* a) {
   if (a->P < 1 || a->P > ATTACK_MAXP) return false;
-  if (a->mode != ATTACK_ALIE && a->mode != ATTACK_MINMAX) return false;
+  if (a->mode != ATTACK_ALIE && a->mode != ATTACK_MINMAX && a->mode != ATTACK_IPM) return false;
   if (a->mode == ATTACK_MINMAX && (!a->stats || !a->partials || !a->gamma)) return false;
   return true;
 }
 
+extern "C" int drc_attack_ipm(const AttackArgs* args, int grid, cudaStream_t stream) {
+  if (!attack_args_ok(args) || args->mode != ATTACK_IPM || grid < 1) return (int)cudaErrorInvalidValue;
+  attack_ipm_kernel<<<grid, DRC_THREADS, 0, stream>>>(*args);
+  return (int)cudaGetLastError();
+}
 extern "C" int drc_attack_stats(const AttackArgs* args, int grid, cudaStream_t stream) {
-  if (!attack_args_ok(args) || grid < 1) return (int)cudaErrorInvalidValue;
+  if (!attack_args_ok(args) || args->mode == ATTACK_IPM || grid < 1) return (int)cudaErrorInvalidValue;
   attack_stats_kernel<<<grid, DRC_THREADS, 0, stream>>>(*args);
   return (int)cudaGetLastError();
 }

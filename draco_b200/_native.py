@@ -161,6 +161,12 @@ class AttackArgs(C.Structure):
                 ("t_end", C.c_int), ("fold", ptr)]
 
 
+class MimicArgs(C.Structure):
+    _fields_ = [("grad_in", ptr), ("slot_stride", i64), ("P", C.c_int), ("warmup", C.c_int), ("tv", TileView),
+                ("adv_bitmap", ptr), ("adv_len", C.c_int), ("step_ptr", ptr), ("m", ptr), ("z", ptr), ("u", ptr),
+                ("partials", ptr), ("fold", ptr), ("upart", ptr), ("ufold", ptr), ("w", ptr), ("target", ptr)]
+
+
 class CcArgs(C.Structure):
     _fields_ = [("grad_in", ptr), ("slot_stride", i64), ("n", C.c_int), ("rows", ptr), ("tv", TileView), ("center", ptr),
                 ("partials", ptr), ("weights", ptr), ("tau", C.c_double), ("tile_begin", C.c_int), ("tile_end", C.c_int),
@@ -246,6 +252,8 @@ def cuda() -> C.CDLL:
             "drc_attack_solve": [C.POINTER(AttackArgs), st],
             "drc_attack_solve_model": [C.POINTER(AttackArgs), st],
             "drc_attack_write": [C.POINTER(AttackArgs), C.c_int, st],
+            "drc_attack_ipm": [C.POINTER(AttackArgs), C.c_int, st],
+            "drc_mimic_step": [C.POINTER(MimicArgs), C.c_int, st],
             "drc_cc_dist": [C.POINTER(CcArgs), C.c_int, st],
             "drc_cc_weights": [C.POINTER(CcArgs), st],
             "drc_cc_model_weights": [C.POINTER(CcArgs), st],

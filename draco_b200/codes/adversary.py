@@ -17,6 +17,9 @@ Attack parity (src/model_ops/utils.py:3-23), ``mag = -100``:
              within the largest honest pairwise distance of every honest row
              (both per tensor, over the honest workers' pushed slots; applied by the PS, see ``alie_row`` / ``minmax_row``;
              ``--attack-scope model`` gives min-max one gamma and one Dmax over the whole model, ``minmax_gamma_model``)
+  ipm      : inner-product manipulation (Xie, Koyejo and Gupta, UAI 2019): -eps * mu per coordinate (``ipm_row``)
+  mimic    : (Karimireddy, He and Jaggi, ICLR 2022) every liar copies the honest slot that lies furthest along a direction z
+             the PS learns during the first W steps (``mimic_z0`` / ``mimic_step``; whole model, stateful)
 
 The device implementation of the same hook lives in csrc/cuda/push_encode.cu; the integer codes
 below are shared with it.
@@ -40,7 +43,12 @@ ATTACK_RANDOM = 3
 ATTACK_OMNISCIENT = 4
 ATTACK_ALIE = 5
 ATTACK_MINMAX = 6
-PS_ATTACKS = ("alie", "minmax")     # built by the PS from the honest slots; the liars push their true gradient
+ATTACK_IPM = 7
+ATTACK_MIMIC = 8
+# built by the PS from the honest slots; the liars push their true gradient
+PS_ATTACKS = ("alie", "minmax", "ipm", "mimic")
+IPM_EPS = 0.1             # --attack-eps default: this repository's choice (the paper evaluates several eps)
+MIMIC_WARMUP = 20         # --mimic-warmup default: this repository's choice (steps of the online power iteration)
 
 _ATTACK_CODES = {
     "none": ATTACK_NONE,
@@ -50,6 +58,8 @@ _ATTACK_CODES = {
     "omniscient": ATTACK_OMNISCIENT,
     "alie": ATTACK_ALIE,
     "minmax": ATTACK_MINMAX,
+    "ipm": ATTACK_IPM,
+    "mimic": ATTACK_MIMIC,
 }
 
 
@@ -210,10 +220,104 @@ def minmax_row(H: np.ndarray) -> np.ndarray:
         return mu - minmax_gamma(H) * sd
 
 
+def ipm_row(H: np.ndarray, eps: float) -> np.ndarray:
+    """The row every IPM liar sends for one tensor: -eps * mu, mu the fp64 honest mean summed in slot order and divided once
+    (ALIE's mu), in fp64; the slot gets it rounded to fp32 once."""
+    H = np.asarray(H, dtype=np.float64)
+    acc = np.zeros(H.shape[1:], dtype=np.float64)
+    with np.errstate(invalid="ignore", over="ignore"):
+        for h in H:
+            acc = acc + h
+        return -eps * (acc / H.shape[0])
+
+
+def mimic_z0(spans, total: int, seed: int = SEED) -> np.ndarray:
+    """Mimic's starting direction, fp32 [total]: standard normals on the valid coordinates (one Philox stream keyed by the
+    adversary seed, laid out over the spans in ascending order, 0 on padding), divided by their norm -- per-tensor fp64 sums
+    of squares added in ascending tensor order (``oracle.model_d2``), one sqrt -- and rounded to fp32 once."""
+    from .oracle import model_d2
+    n = sum(int(numel) for _, numel in spans)
+    g = np.random.Generator(np.random.Philox(key=seed)).standard_normal(n)
+    x = np.zeros(total, dtype=np.float64)
+    at = 0
+    for off, numel in spans:
+        x[off:off + numel] = g[at:at + numel]
+        at += numel
+    nrm = math.sqrt(float(model_d2([[float((x[o:o + k] ** 2).sum())] for o, k in spans])[0]))
+    return (x / nrm).astype(np.float32)
+
+
+@dataclass
+class MimicState:
+    """Mimic's PS state: ``m`` the running mean of the honest means (+0 at the start) and ``z`` the unit direction, both fp32
+    [D] and 0 on padding."""
+    m: np.ndarray
+    z: np.ndarray
+
+
+def _model_dot(a: np.ndarray, b: np.ndarray, spans) -> float:
+    """<a, b> over the spans: each tensor's fp64 sum, added in ascending tensor order (``oracle.model_d2``)."""
+    from .oracle import model_d2
+    with np.errstate(invalid="ignore", over="ignore"):
+        per = [[float((a[o:o + k].astype(np.float64) * b[o:o + k].astype(np.float64)).sum())] for o, k in spans]
+    return float(model_d2(per)[0])
+
+
+def mimic_step(slots: np.ndarray, liars, spans, state: MimicState, t: int, W: int):
+    """One PS step of the mimic attack (the definition the fused kernels and the library path share).
+
+    With H the honest slots in ascending order, n = |H|, and every whole-model sum the per-tensor fp64 sums added in ascending
+    tensor order:
+
+    1. s_i = <x_i, z> for i in H;
+    2. k = the first i in H with the largest s_i (``np.argmax``: a NaN counts as the largest, ties go to the lower slot);
+    3. every liar slot becomes a bit copy of x_k on the spans (padding is never written);
+    4. only while t < W (t = step - 1, the warm-up index): c = (sum_{i in H} x_i) / n in fp64; m = fp32((t m + c) / (t + 1));
+       w_i = s_i - <m, z> (the new m; equal to <x_i - m, z> up to rounding, the form the kernels use);
+       u = t z + sum_{i in H} w_i (x_i - m) in fp64 without contraction; z = fp32(u / ||u||), unchanged when ||u|| = 0.
+       Steps 1-3 use the z from before the update.
+
+    Returns (the new slots, k, the new ``MimicState``).  ``slots`` [P, D] fp32; ``liars`` 0-based."""
+    out = np.array(slots, copy=True)
+    liars = sorted(set(int(w) for w in liars))
+    honest = [w for w in range(out.shape[0]) if w not in liars]
+    m, z = state.m.copy(), state.z.copy()
+    if not honest:
+        return out, -1, MimicState(m, z)
+    s = np.array([_model_dot(slots[i], z, spans) for i in honest])
+    k = honest[int(np.argmax(s))]
+    for off, numel in spans:
+        out[liars, off:off + numel] = slots[k, off:off + numel]
+    if t < W:
+        n = len(honest)
+        with np.errstate(invalid="ignore", over="ignore"):
+            for off, numel in spans:
+                sl = slice(off, off + numel)
+                c = np.zeros(numel, dtype=np.float64)
+                for i in honest:
+                    c = c + slots[i, sl].astype(np.float64)
+                m[sl] = ((t * m[sl].astype(np.float64) + c / n) / (t + 1)).astype(np.float32)
+            mz = _model_dot(m, z, spans)
+            w = [float(si) - mz for si in s]
+            u = np.zeros(out.shape[1], dtype=np.float64)
+            for off, numel in spans:
+                sl = slice(off, off + numel)
+                acc = t * z[sl].astype(np.float64)
+                for wi, i in zip(w, honest):
+                    acc = acc + wi * (slots[i, sl].astype(np.float64) - m[sl].astype(np.float64))
+                u[sl] = acc
+            nrm = math.sqrt(_model_dot(u, u, spans))
+            if nrm != 0.0:
+                for off, numel in spans:
+                    z[off:off + numel] = (u[off:off + numel] / nrm).astype(np.float32)
+    return out, k, MimicState(m, z)
+
+
 def ps_attack(slots: np.ndarray, liars, mode: str, spans, z: Optional[float] = None, scope: str = "tensor") -> np.ndarray:
     """Oracle of the whole PS-side step: ``slots`` [P, D] with the liar slots (0-based) replaced, per tensor span
     ``(offset, numel)``, by the attack row built from the honest slots (fp64, rounded to the slots' dtype).  Padding outside
-    the spans is left alone.  ``scope="model"`` (min-max only): one gamma over every span (``minmax_gamma_model``)."""
+    the spans is left alone.  ``scope="model"`` (min-max only): one gamma over every span (``minmax_gamma_model``).  ``z`` is
+    ALIE's z or IPM's eps; mimic has state and its own ``mimic_step``."""
     out = np.array(slots, copy=True)
     liars = sorted(set(int(w) for w in liars))
     honest = [w for w in range(out.shape[0]) if w not in liars]
@@ -226,6 +330,8 @@ def ps_attack(slots: np.ndarray, liars, mode: str, spans, z: Optional[float] = N
             mu, sd = honest_stats(H)
             with np.errstate(invalid="ignore"):
                 row = mu - gamma * sd
+        elif mode == "ipm":
+            row = ipm_row(H, z)
         else:
             row = alie_row(H, z) if mode == "alie" else minmax_row(H)
         with np.errstate(over="ignore", invalid="ignore"):

@@ -18,7 +18,7 @@ DETOX_MODES = ("coordinate_median", "trimmed_mean", "multi_krum", "geometric_med
 NNM_MODES = ("coordinate_median", "trimmed_mean", "krum", "multi_krum", "geometric_median", "bulyan")
 ROBUST_MAXP = 16                    # workers the fused coordinate-wise / Krum / Bulyan kernels take (TRIM_MAXP, KRUM_MAXP)
 SIGN_VOTE_MAXP = 32                 # workers the fused sign vote takes: the adversary bitmaps are 32-bit (DRC_MAX_WORKERS)
-ERR_MODES = ("rev_grad", "constant", "random", "omniscient", "alie", "minmax", "none")
+ERR_MODES = ("rev_grad", "constant", "random", "omniscient", "alie", "minmax", "ipm", "mimic", "none")
 TRANSPORTS = ("nvl", "nccl", "nccl_flat", "gloo")
 SCOPES = ("tensor", "model")        # --rule-scope / --attack-scope: distances per parameter tensor, or over the whole model
 # the --mode values whose rule measures distances between rows (every --approach nnm mode does, through its neighbourhoods)
@@ -94,6 +94,8 @@ class JobConfig:
     attack_scope: str = "tensor"    # --err-mode minmax: one gamma per parameter tensor, or one over the whole model
     bucketing: int = 0              # worker buckets of s: the robust rule runs on the means of ceil(P / s) random buckets (0: off)
     dirichlet_alpha: Optional[float] = None  # heterogeneous data: each holder's shard has Dirichlet(alpha) class shares (None: IID)
+    attack_eps: Optional[float] = None  # --err-mode ipm: the liars send -eps * mu (None: codes.adversary.IPM_EPS)
+    mimic_warmup: Optional[int] = None  # --err-mode mimic: steps that learn the direction (None: codes.adversary.MIMIC_WARMUP)
 
     # ---- derived --------------------------------------------------------------------------
     def resolve(self, world_size: int) -> "JobConfig":
@@ -147,10 +149,21 @@ class JobConfig:
         return self
 
     def _check_ps_attack(self) -> None:
-        """--err-mode alie | minmax: the PS replaces the liars' slots with a row built from the honest slots."""
+        """--err-mode alie | minmax | ipm | mimic: the PS replaces the liars' slots with a row built from the honest slots."""
         from .codes.adversary import PS_ATTACKS, alie_s
         if self.attack_z is not None and self.err_mode != "alie":
             raise ValueError(f"--attack-z sets ALIE's z: it needs --err-mode alie (got --err-mode {self.err_mode})")
+        if self.attack_eps is not None and self.err_mode != "ipm":
+            raise ValueError(f"--attack-eps sets IPM's eps: it needs --err-mode ipm (got --err-mode {self.err_mode})")
+        if self.attack_eps is not None and not (math.isfinite(self.attack_eps) and self.attack_eps > 0):
+            raise ValueError(f"--attack-eps must be a finite eps > 0 (got {self.attack_eps}): the liars send -eps times the "
+                             f"honest mean")
+        if self.mimic_warmup is not None and self.err_mode != "mimic":
+            raise ValueError(f"--mimic-warmup sets how many steps mimic learns its direction: it needs --err-mode mimic (got "
+                             f"--err-mode {self.err_mode})")
+        if self.mimic_warmup is not None and self.mimic_warmup < 0:
+            raise ValueError(f"--mimic-warmup must be >= 0 steps (got {self.mimic_warmup}; 0 mimics along the random starting "
+                             f"direction)")
         if self.err_mode not in PS_ATTACKS:
             return
         m = self.err_mode
@@ -222,7 +235,7 @@ class JobConfig:
         if self.approach != "baseline":
             raise ValueError(f"--mode sign_vote votes over the signs of the P workers' rows: use --approach baseline (got "
                              f"--approach {self.approach})")
-        if self.err_mode in ("omniscient", "alie", "minmax"):
+        if self.err_mode in ("omniscient", "alie", "minmax", "ipm", "mimic"):
             raise ValueError(f"--err-mode {self.err_mode} builds a real-valued row from the honest workers' fp32 slots, and the sign "
                              f"wire has none: use --err-mode rev_grad | constant | random | none with --mode sign_vote")
         if self.compress:
@@ -303,6 +316,18 @@ class JobConfig:
         if self.approach == "cyclic":
             raise ValueError("--dirichlet-alpha gives every data holder its own shard; under --approach cyclic the workers split "
                              "one global batch, so there is no holder to give it to")
+
+    @property
+    def ipm_eps(self) -> float:
+        """eps of the IPM attack: --attack-eps, else the repository's default (codes.adversary.IPM_EPS)."""
+        from .codes.adversary import IPM_EPS
+        return float(self.attack_eps) if self.attack_eps is not None else IPM_EPS
+
+    @property
+    def mimic_w(self) -> int:
+        """Mimic's warm-up steps W: --mimic-warmup, else the repository's default (codes.adversary.MIMIC_WARMUP)."""
+        from .codes.adversary import MIMIC_WARMUP
+        return int(self.mimic_warmup) if self.mimic_warmup is not None else MIMIC_WARMUP
 
     @property
     def alie_z(self) -> float:
@@ -433,10 +458,17 @@ def add_fit_args(parser: argparse.ArgumentParser) -> argparse.ArgumentParser:
     a("--dataset", type=str, default=d.dataset)
     a("--comm-type", type=str, default=d.comm_type)
     a("--err-mode", type=str, default=d.err_mode,
-      help="rev_grad | constant | random | omniscient | alie | minmax | none.  alie (A Little Is Enough) and minmax (min-max, "
-           "inverse-std direction) are applied by the PS per tensor from the honest workers' mean and standard deviation")
+      help="rev_grad | constant | random | omniscient | alie | minmax | ipm | mimic | none.  alie (A Little Is Enough) and minmax "
+           "(min-max, inverse-std direction) are applied by the PS per tensor from the honest workers' mean and standard "
+           "deviation; ipm (inner-product manipulation): the liars send -eps times the honest mean; mimic: every liar sends a "
+           "copy of the honest worker furthest along a direction the PS learns over the first --mimic-warmup steps")
     a("--attack-z", type=float, default=None,
       help="--err-mode alie: the liars send mu - z * sigma (default: z_max = Phi^-1((P - s) / P), s = floor(P/2 + 1) - f)")
+    a("--attack-eps", type=float, default=None,
+      help="--err-mode ipm: the liars send -eps * mu, mu the honest mean (default 0.1, this repository's choice)")
+    a("--mimic-warmup", type=int, default=None,
+      help="--err-mode mimic: the first W steps learn the top principal direction of the honest gradients by an online power "
+           "iteration (default 20, this repository's choice; 0: a fixed random direction)")
     a("--worker-momentum", type=float, default=d.worker_momentum,
       help="beta of worker-side momentum (0 = off): every worker keeps m <- beta m + (1 - beta) g and pushes m instead of its "
            "gradient, which shrinks the honest workers' spread before the robust rule sees it (Karimireddy et al. 2021, El "

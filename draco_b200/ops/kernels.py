@@ -145,12 +145,16 @@ def ps_attack(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, mode
               step_ptr: Addr, z: float = 0.0, ws: Optional[AttackWorkspace] = None, tile_range: Optional[tuple] = None,
               tensor_range: Optional[tuple] = None, grid: Optional[int] = None) -> int:
     """Overwrite the liar slots of the step (``adv_bitmap[*step_ptr % adv_len]``) of ``grad_in`` [P, slot_stride] with the ALIE
-    (``mode`` 5, ``z``) or min-max (``mode`` 6, workspace ``ws``) row of every tensor, built from the honest slots
-    (csrc/cuda/attack.cu).  ``tile_range`` / ``tensor_range``: one bucket (whole tensors).  Returns the kernels launched."""
+    (``mode`` 5, ``z``), min-max (``mode`` 6, workspace ``ws``) or IPM (``mode`` 7, ``z`` = eps) row of every tensor, built from
+    the honest slots (csrc/cuda/attack.cu).  ``tile_range`` / ``tensor_range``: one bucket (whole tensors).  Returns the
+    kernels launched."""
     a, g = _attack_args(layout, grad_in, slot_stride, P, mode, adv_bitmap, adv_len, step_ptr, z, ws, tile_range, grid)
     if tensor_range is not None:
         a.t_begin, a.t_end = int(tensor_range[0]), int(tensor_range[1])
     lib = N.cuda()
+    if mode == 7:
+        N.check(lib.drc_attack_ipm(C.byref(a), g, _stream()), "attack_ipm")
+        return 1
     N.check(lib.drc_attack_stats(C.byref(a), g, _stream()), "attack_stats")
     if mode == 5:
         return 1
@@ -163,8 +167,8 @@ def _attack_args(layout, grad_in, slot_stride, P, mode, adv_bitmap, adv_len, ste
     """The ``AttackArgs`` both attack launchers share, and the grid of the tile kernels."""
     if not 1 <= P <= ATTACK_MAXP:
         raise ValueError(f"the PS-side attacks take 1..{ATTACK_MAXP} worker slots, got {P}")
-    if mode not in (5, 6):
-        raise ValueError(f"attack mode must be 5 (alie) or 6 (minmax), got {mode}")
+    if mode not in (5, 6, 7):
+        raise ValueError(f"attack mode must be 5 (alie), 6 (minmax) or 7 (ipm), got {mode}")
     if mode == 6 and ws is None:
         raise ValueError("the min-max attack needs an AttackWorkspace")
     dev = torch.device("cuda", torch.cuda.current_device())
@@ -201,6 +205,45 @@ def ps_attack_model(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int
     N.check(lib.drc_attack_solve_model(C.byref(a), _stream()), "attack_solve_model")
     N.check(lib.drc_attack_write(C.byref(a), g, _stream()), "attack_write")
     return 4
+
+
+class MimicState:
+    """The mimic attack's PS state and scratch (csrc/cuda/mimic.cu): the fp32 arenas ``m`` (running mean of the honest means,
+    +0 at the start) and ``z`` (the unit direction, ``z0`` at the start), the fp64 arena ``u``, the per-tile and per-tensor
+    fp64 partials, the w_i and the step's target slot."""
+
+    def __init__(self, layout: ArenaLayout, P: int, device, z0: torch.Tensor):
+        if not 1 <= P <= ATTACK_MAXP:
+            raise ValueError(f"the mimic attack takes 1..{ATTACK_MAXP} worker slots, got {P}")
+        self.m = layout.new_arena(device)
+        self.z = z0.to(device=device, dtype=torch.float32).clone()
+        _check_buffer("MimicState: z0", self.z, torch.float32, (layout.total,))
+        self.u = torch.zeros(layout.total, dtype=torch.float64, device=device)
+        self.partials = torch.zeros(layout.ntiles, P + 1, dtype=torch.float64, device=device)
+        self.fold = torch.zeros(layout.ntensors, P + 1, dtype=torch.float64, device=device)
+        self.upart = torch.zeros(layout.ntiles, dtype=torch.float64, device=device)
+        self.ufold = torch.zeros(layout.ntensors, dtype=torch.float64, device=device)
+        self.w = torch.zeros(P, dtype=torch.float64, device=device)
+        self.target = torch.zeros(1, dtype=torch.int32, device=device)
+
+
+def mimic_step(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, *, adv_bitmap: Addr, adv_len: int, step_ptr: Addr,
+               warmup: int, st: MimicState, grid: Optional[int] = None) -> int:
+    """One step of the mimic attack over the whole arena (codes/adversary.py ``mimic_step``): every liar slot of the step becomes
+    a copy of the honest slot with the largest <x_i, z>, and while ``*step_ptr - 1 < warmup`` the state ``st`` advances.  Six
+    kernels, the last two warm-up only (they return on the device after it).  Returns the kernels launched."""
+    if warmup < 0:
+        raise ValueError(f"mimic warm-up must be >= 0, got {warmup}")
+    dev = torch.device("cuda", torch.cuda.current_device())
+    a = N.MimicArgs()
+    a.grad_in, a.slot_stride, a.P, a.warmup = addr(grad_in), slot_stride, P, int(warmup)
+    a.tv = layout.tile_view(dev)
+    a.adv_bitmap, a.adv_len, a.step_ptr = addr(adv_bitmap), int(adv_len) if adv_bitmap is not None else 0, addr(step_ptr)
+    a.m, a.z, a.u = st.m.data_ptr(), st.z.data_ptr(), st.u.data_ptr()
+    a.partials, a.fold, a.upart, a.ufold = st.partials.data_ptr(), st.fold.data_ptr(), st.upart.data_ptr(), st.ufold.data_ptr()
+    a.w, a.target = st.w.data_ptr(), st.target.data_ptr()
+    N.check(N.cuda().drc_mimic_step(C.byref(a), grid or stream_grid(layout), _stream()), "mimic_step")
+    return 6
 
 
 # ------------------------------------------------------------------------------------------------ vote (K3)

@@ -162,10 +162,23 @@ class CollectiveEngine:
             self.slots[w - 1].copy_(mean * self.cfg.attack_magnitude)
 
     def _ps_attack(self, step: int) -> None:
-        """--err-mode alie | minmax: every liar slot gets the attack row of each tensor, built in fp64 from the honest slots."""
+        """--err-mode alie | minmax | ipm: every liar slot gets the attack row of each tensor, built in fp64 from the honest
+        slots.  mimic: the PS's ``TorchPS.mimic_attack``, whose state advances in warm-up steps."""
         liars = [w - 1 for w in range(1, self.P + 1) if self.schedule.is_adversary(w, step)]
         honest = [w for w in range(self.P) if w not in liars]
+        if self.cfg.err_mode == "mimic":
+            self.ps.mimic_attack(self.slots, liars, step - 1)
+            return
         if not liars or not honest:
+            return
+        if self.cfg.err_mode == "ipm":
+            eps = self.cfg.ipm_eps
+            for s in self.layout.specs:
+                H = self.slots[honest, s.offset: s.offset + s.numel].double()
+                mu = torch.zeros_like(H[0])                 # from +0, in slot order, as the kernel sums
+                for h in H:
+                    mu = mu + h
+                self.slots[liars, s.offset: s.offset + s.numel] = (-eps * (mu / len(honest))).to(self.slots.dtype)
             return
         z = self.cfg.alie_z if self.cfg.err_mode == "alie" else 0.0
         specs = self.layout.specs

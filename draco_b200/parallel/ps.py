@@ -19,7 +19,7 @@ import numpy as np
 import torch
 
 from .. import _native as N
-from ..codes.adversary import ATTACK_ALIE, ATTACK_MINMAX, PS_ATTACKS, attack_code
+from ..codes.adversary import ATTACK_ALIE, ATTACK_IPM, ATTACK_MIMIC, ATTACK_MINMAX, PS_ATTACKS, attack_code, mimic_z0
 from ..codes.bucketing import bucket_schedule, wbuckets
 from ..codes.cyclic import CyclicCode, search_w
 from ..codes.oracle import (_bulyan_rounds, _krum_scores_d2, _weiszfeld_weights, centered_clip_weight, model_d2,
@@ -60,7 +60,8 @@ NNM_RULES = {"coordinate_median": "nnm_median", "trimmed_mean": "nnm_trimmed_mea
 
 # rules the fused PS applies bucket by bucket while the workers still push (nothing in them reaches beyond the bucket's
 # tensors: buckets hold whole tensors, and centered clipping's centre is known before the step starts).  Only at the default
-# scopes: a whole-model distance, or min-max's whole-model gamma, needs every bucket first (RulePlan.pipelined)
+# scopes: a whole-model distance, or min-max's whole-model gamma, needs every bucket first (RulePlan.pipelined); so does the
+# mimic attack, whose target comes from whole-model sums
 PIPELINED_RULES = ("mean", "vote", "median", "trimmed_mean", "detox_median", "detox_trimmed_mean", "centered_clip",
                    "detox_centered_clip", "sign_vote")
 
@@ -87,7 +88,8 @@ class RulePlan:
     m: int              # Krum / multi-Krum: rows averaged
     theta: int          # Bulyan: rows selected
     opt_mode: str       # the optimizer's mode string
-    pipelined: bool     # the fused PS may apply it bucket by bucket: a PIPELINED_RULES rule with both scopes "tensor"
+    pipelined: bool     # the fused PS may apply it bucket by bucket: a PIPELINED_RULES rule with both scopes "tensor", and no
+                        # --err-mode mimic
     scope: str          # --rule-scope: tensor | model (one choice over the whole model for every tensor)
     attack_scope: str   # --attack-scope: tensor | model (min-max: one gamma over the whole model)
 
@@ -109,8 +111,8 @@ def rule_plan(cfg: JobConfig) -> RulePlan:
     m = {"krum": 1, "multi_krum": rows - f}.get(base, 0)
     scope, attack_scope = cfg.rule_scope, cfg.attack_scope
     return RulePlan(rule, source, base, rows, f, trim, m, rows - 2 * f if base == "bulyan" else 0, _OPT_MODE[base],
-                    rule.removeprefix("wbucket_") in PIPELINED_RULES and scope == "tensor" and attack_scope == "tensor", scope,
-                    attack_scope)
+                    rule.removeprefix("wbucket_") in PIPELINED_RULES and scope == "tensor" and attack_scope == "tensor"
+                    and cfg.err_mode != "mimic", scope, attack_scope)
 
 
 def hyperparams_tensor(cfg: JobConfig, device) -> torch.Tensor:
@@ -145,10 +147,17 @@ class FusedPS:
         # the sign wire packs 32 coordinates into one uint32 word (push_encode(sign=True)); the stride is then in words
         self.slot_stride = layout.total // 32 if plan.base == "sign_vote" else layout.total
         self.rule = plan.rule
-        # --err-mode alie | minmax: the liar slots of each bucket are overwritten after its flags and before its decode
+        # --err-mode alie | minmax | ipm: the liar slots of each bucket are overwritten after its flags and before its decode;
+        # mimic: once, after the last bucket
         self.attack = attack_code(cfg.err_mode) if cfg.err_mode in PS_ATTACKS and adv_bitmap is not None else 0
         self.adv_bitmap, self.adv_len = adv_bitmap, adv_len
-        self.attack_z = cfg.alie_z if self.attack == ATTACK_ALIE else 0.0
+        # ALIE's z (z_max is only defined, and only read, under alie) or IPM's eps
+        self.attack_z = cfg.alie_z if self.attack == ATTACK_ALIE else cfg.ipm_eps if self.attack == ATTACK_IPM else 0.0
+        # mimic's state (checkpointed as opt_state["mimic_m"] / ["mimic_z"]) exists in every --err-mode mimic job
+        self.mimic = None
+        if cfg.err_mode == "mimic":
+            z0 = mimic_z0([(sp.offset, sp.numel) for sp in layout.specs], layout.total)
+            self.mimic = K.MimicState(layout, self.P, device, torch.from_numpy(z0))
         self.attack_ws = K.AttackWorkspace(layout, self.P, device) if self.attack == ATTACK_MINMAX else None
         # --attack-scope model: min-max's per-tensor sums, folded, then one solve over the whole arena
         self.attack_fold = (K.attack_fold_buffer(layout, self.P, device)
@@ -216,6 +225,8 @@ class FusedPS:
         state = {"exp_avg_sq": self.exp_avg_sq, "max_exp_avg_sq": self.max_exp_avg_sq}
         if self.plan.base == "centered_clip":
             state["cc_center"] = self.cc_center
+        if self.mimic is not None:
+            state["mimic_m"], state["mimic_z"] = self.mimic.m, self.mimic.z
         return state
 
     def enqueue_step(self, step_ptr: torch.Tensor, *, mc_params: Optional[int], dst: Sequence[int], flags: Sequence[int],
@@ -243,7 +254,10 @@ class FusedPS:
             last = bi == len(ranges) - 1
             if pipelined:
                 n += wait_bucket(bi)
-            if self.attack_fold is not None:
+            if self.attack == ATTACK_MIMIC:
+                n += K.mimic_step(L, self.grad_in, self.slot_stride, self.P, adv_bitmap=self.adv_bitmap, adv_len=self.adv_len,
+                                  step_ptr=step_ptr, warmup=self.cfg.mimic_w, st=self.mimic)
+            elif self.attack_fold is not None:
                 n += K.ps_attack_model(L, self.grad_in, self.slot_stride, self.P, adv_bitmap=self.adv_bitmap, adv_len=self.adv_len,
                                        step_ptr=step_ptr, ws=self.attack_ws, fold=self.attack_fold)
             elif self.attack:
@@ -390,6 +404,12 @@ class TorchPS:
                                          dampening=cfg.dampening, nesterov=cfg.nesterov)
         # centered clipping's centre: last step's aggregate, +0 at the start (PS state, checkpointed as opt_state["cc_center"])
         self.cc_center = layout.new_arena(device) if self.plan.base == "centered_clip" else None
+        # --err-mode mimic: the running mean and the direction (opt_state["mimic_m"] / ["mimic_z"]), see ``mimic_attack``
+        self.mimic_m = self.mimic_z = None
+        if cfg.err_mode == "mimic":
+            self.mimic_m = layout.new_arena(device)
+            self.mimic_z = torch.from_numpy(mimic_z0([(sp.offset, sp.numel) for sp in layout.specs], layout.total)).to(device)
+        self.mimic_target = -1
         # --bucketing: the permutation of every step (row step % len, as the fused PS reads it)
         self.wb_schedule = bucket_schedule(self.P, cfg.max_steps, cfg.seed) if self.plan.source == "wbucket" else None
         if self.plan.base == "cyclic":
@@ -435,6 +455,8 @@ class TorchPS:
                                                           "max_exp_avg_sq": self._gather("max_exp_avg_sq")}
         if self.cc_center is not None:
             state["cc_center"] = self.cc_center.clone()
+        if self.mimic_m is not None:
+            state["mimic_m"], state["mimic_z"] = self.mimic_m.clone(), self.mimic_z.clone()
         return state
 
     def load_opt_state(self, arenas: Dict[str, torch.Tensor], step: int) -> None:
@@ -444,6 +466,10 @@ class TorchPS:
         center = arenas.pop("cc_center", None)
         if self.cc_center is not None and center is not None:
             self.cc_center.copy_(center)
+        for key, dst in (("mimic_m", self.mimic_m), ("mimic_z", self.mimic_z)):
+            saved = arenas.pop(key, None)
+            if dst is not None and saved is not None:
+                dst.copy_(saved)
         if self.cfg.optimizer != "adam":
             return
         for v, spec in zip(self._views, self.layout.specs):
@@ -454,6 +480,56 @@ class TorchPS:
                 if arena is not None:
                     st[key] = arena[spec.offset: spec.offset + spec.numel].clone()
             st.setdefault("exp_avg_sq", torch.zeros_like(v))
+
+    # --- the mimic attack -----------------------------------------------------------------------
+    def mimic_attack(self, slots: torch.Tensor, liars: List[int], t: int) -> None:
+        """``--err-mode mimic`` on the PS's slots [P, D] (``codes.adversary.mimic_step``, in fp64 torch ops on the slots'
+        device): every liar slot (0-based) becomes a copy of the honest slot with the largest <x_i, z>, and while t < W (t =
+        step - 1) the running mean and the direction advance.  Whole-model sums are the per-tensor fp64 sums added in
+        ascending tensor order."""
+        honest = [w for w in range(self.P) if w not in liars]
+        if not honest:
+            return
+        specs = self.layout.specs
+        z = self.mimic_z
+
+        def model_dot(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:       # [..., D] x [D] -> [...]
+            acc = None
+            for sp in specs:
+                d = (a[..., sp.offset: sp.offset + sp.numel].double() * b[sp.offset: sp.offset + sp.numel].double()).sum(-1)
+                acc = d if acc is None else acc + d
+            return acc
+
+        X = slots[honest]
+        s = model_dot(X, z).cpu().numpy()
+        k = honest[int(np.argmax(s))]
+        self.mimic_target = k
+        for sp in specs:
+            slots[liars, sp.offset: sp.offset + sp.numel] = slots[k, sp.offset: sp.offset + sp.numel]
+        if t >= self.cfg.mimic_w:
+            return
+        n = len(honest)
+        u = torch.zeros(self.layout.total, dtype=torch.float64, device=slots.device)
+        for sp in specs:
+            sl = slice(sp.offset, sp.offset + sp.numel)
+            c = torch.zeros(sp.numel, dtype=torch.float64, device=slots.device)
+            for i in range(n):
+                c = c + X[i, sl].double()
+            self.mimic_m[sl] = ((t * self.mimic_m[sl].double() + c / n) / (t + 1)).float()
+        mz = float(model_dot(self.mimic_m, z))
+        w = [float(si) - mz for si in s]
+        for sp in specs:
+            sl = slice(sp.offset, sp.offset + sp.numel)
+            acc = t * z[sl].double()
+            m64 = self.mimic_m[sl].double()
+            for i in range(n):
+                acc = acc + w[i] * (X[i, sl].double() - m64)
+            u[sl] = acc
+        nrm = math.sqrt(float(model_dot(u, u)))
+        if nrm != 0.0:
+            for sp in specs:
+                sl = slice(sp.offset, sp.offset + sp.numel)
+                z[sl] = (u[sl] / nrm).float()
 
     # --- per-tensor rules -----------------------------------------------------------------------
     def _vote_tensor(self, rows: List[torch.Tensor]) -> int:

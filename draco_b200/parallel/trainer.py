@@ -21,8 +21,8 @@ import torch.distributed as dist
 
 from ..config import JobConfig
 from ..data import TensorDataset, class_histograms, load_dataset
-from ..utils.checkpoint import (arena_tensors, check_cc_center, check_worker_momentum, checkpoint_path, load_checkpoint,
-                                model_buffers, restore_into, restore_worker_momentum, save_checkpoint)
+from ..utils.checkpoint import (arena_tensors, check_cc_center, check_mimic_state, check_worker_momentum, checkpoint_path,
+                                load_checkpoint, model_buffers, restore_into, restore_worker_momentum, save_checkpoint)
 from ..utils.metrics import MetricsLogger
 
 
@@ -205,6 +205,7 @@ class Trainer:
         blob = load_checkpoint(checkpoint_path(self.cfg.train_dir, step))
         check_worker_momentum(blob, self.cfg.worker_momentum)
         check_cc_center(blob, self.cfg.mode == "centered_clip")
+        check_mimic_state(blob, self.cfg.err_mode == "mimic")
         eng = self.engine
         if self.cfg.worker_momentum > 0:
             restore_worker_momentum(blob, eng.layout, eng.worker_momentum)       # every process: its own local workers

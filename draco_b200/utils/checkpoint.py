@@ -10,8 +10,9 @@ the momentum buffers, the step, the BatchNorm statistics of the evaluating worke
 its own BN statistics would be meaningless -- the reason the reference refuses to save ResNets on the PS) and the job
 config.  Resume works for every approach and restores optimizer state.  With ``--worker-momentum`` the blob also holds
 every logical worker's momentum (``"worker_momentum": {w: {tensor name: fp32 tensor}}``); the key is absent otherwise.  Under
-``--mode centered_clip`` the PS's centre travels with the optimizer arenas as ``opt_state["cc_center"]``; other jobs have no
-such entry.
+``--mode centered_clip`` the PS's centre travels with the optimizer arenas as ``opt_state["cc_center"]``, and under
+``--err-mode mimic`` the attack's running mean and direction as ``opt_state["mimic_m"]`` and ``["mimic_z"]``; other jobs have
+no such entries.
 """
 from __future__ import annotations
 
@@ -81,6 +82,18 @@ def check_cc_center(blob: dict, centered_clip: bool) -> None:
     if not centered_clip and has:
         raise ValueError("the checkpoint holds centered clipping's centre (it was written with --mode centered_clip): resume it "
                          "with the same --mode, or the centre would be dropped")
+
+
+def check_mimic_state(blob: dict, mimic: bool) -> None:
+    """A job resumes only from a checkpoint of the same kind: with the mimic attack's running mean and direction iff the job
+    runs --err-mode mimic."""
+    has = "mimic_m" in (blob.get("opt_state") or {}) and "mimic_z" in (blob.get("opt_state") or {})
+    if mimic and not has:
+        raise ValueError("--err-mode mimic: the checkpoint holds no mimic state (it was written by a job with another "
+                         "--err-mode), so the attack's direction and running mean cannot be restored")
+    if not mimic and "mimic_m" in (blob.get("opt_state") or {}):
+        raise ValueError("the checkpoint holds the mimic attack's state (it was written with --err-mode mimic): resume it with "
+                         "the same --err-mode, or the state would be dropped")
 
 
 def restore_worker_momentum(blob: dict, layout: ArenaLayout, arenas: Dict[int, torch.Tensor]) -> None:
