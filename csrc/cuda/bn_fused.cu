@@ -400,8 +400,10 @@ __global__ void __launch_bounds__(BN_THREADS, 2) bn_bwd_apply_kernel(const BnBwd
     const int c = cv * BN_VEC + i;
     const float istd = a.invstd[c], gs = a.gamma[c] * istd, m1 = a.sums[c], m2 = a.sums[a.C + c], mean = a.mean[c];
     cA[i] = gs;                                        // == the forward's scale
+    // every rounding stated (tests/exact_ref.py restates them): cB is two products and nothing to contract; cC's inner term is
+    // one fma of the rounded m2 * istd, which is the contraction nvcc chose for the unfused spelling
     cB[i] = -gs * m2 * istd;
-    cC[i] = gs * (m2 * istd * mean - m1);
+    cC[i] = __fmul_rn(gs, fmaf(__fmul_rn(m2, istd), mean, -m1));
   }
   const long long r0 = (long long)blockIdx.x * a.rows_per_cta;
   long long r1 = r0 + a.rows_per_cta; if (r1 > a.M) r1 = a.M;
@@ -471,7 +473,7 @@ __global__ void __launch_bounds__(BN_THREADS, 2) bn_bwd_apply_dual_kernel(const 
     const float istd = a.invstd_s[c], gs = a.gamma_s[c] * istd, m1 = a.sums_s[c], m2 = a.sums_s[a.C + c], mean = a.mean_s[c];
     bn_smem[c] = gs;
     bn_smem[a.C + c] = -gs * m2 * istd;
-    bn_smem[2 * a.C + c] = gs * (m2 * istd * mean - m1);
+    bn_smem[2 * a.C + c] = __fmul_rn(gs, fmaf(__fmul_rn(m2, istd), mean, -m1));
   }
   float cA[BN_VEC], cB[BN_VEC], cC[BN_VEC];
 #pragma unroll
@@ -480,7 +482,7 @@ __global__ void __launch_bounds__(BN_THREADS, 2) bn_bwd_apply_dual_kernel(const 
     const float istd = a.invstd[c], gs = a.gamma[c] * istd, m1 = a.sums[c], m2 = a.sums[a.C + c], mean = a.mean[c];
     cA[i] = gs;
     cB[i] = -gs * m2 * istd;
-    cC[i] = gs * (m2 * istd * mean - m1);
+    cC[i] = __fmul_rn(gs, fmaf(__fmul_rn(m2, istd), mean, -m1));
   }
   __syncthreads();
   const float* sA = bn_smem + cv * BN_VEC;

@@ -1,4 +1,4 @@
-"""Exact and component-wise references for the tensor-core GEMM / convolution kernels and the BatchNorm statistics.
+"""Exact and component-wise references for the tensor-core GEMM / convolution kernels and the BatchNorm kernels.
 
 Integer operands.  Operands drawn from {-1, 0, +1} make every bf16 x bf16 product exact and every partial sum an integer; as
 long as no partial sum exceeds 2^24 in magnitude, every fp32 sum of them is exact in ANY order, on any tile, split-K or cluster
@@ -24,7 +24,10 @@ from __future__ import annotations
 
 import math
 
+import numpy as np
 import torch
+
+from draco_b200.codes.oracle import fma_f32
 
 FP32_EXACT = 2 ** 24          # every integer of magnitude <= 2^24 is an fp32
 
@@ -246,3 +249,121 @@ def ulps_f32(got: torch.Tensor, ref: torch.Tensor) -> float:
     """max |got - ref| in units of the fp32 spacing at ref."""
     g, r = got.double().to(ref.device), ref.double()
     return float(((g - r).abs() / ulp_f32(r)).max())
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# BatchNorm apply and backward (csrc/cuda/bn_fused.cu), restated operation by operation in fp32
+# ---------------------------------------------------------------------------------------------------------------------
+# Activations are [M, C] (one NHWC pixel row per row), per-channel vectors [C]; any float dtype is read as its fp32 value.
+# rn32(a op b) is the fp64 result rounded once to fp32: a product of two fp32 values is exact in fp64, and a sum rounded
+# first to fp64 then to fp32 equals the fp32 sum (53 >= 2 * 24 + 2).  fma is codes.oracle.fma_f32 (one rounding), bf16 is
+# torch's fp32 -> bf16 conversion (round to nearest even, NaN stays NaN), as __float2bfloat16_rn.
+def _np32(t) -> np.ndarray:
+    return t.detach().cpu().float().numpy() if isinstance(t, torch.Tensor) else np.asarray(t, dtype=np.float32)
+
+
+def _mul32(a, b) -> np.ndarray:
+    with np.errstate(all="ignore"):
+        return (np.asarray(a, np.float32).astype(np.float64) * np.asarray(b, np.float32).astype(np.float64)).astype(np.float32)
+
+
+def _add32(a, b) -> np.ndarray:
+    with np.errstate(all="ignore"):
+        return (np.asarray(a, np.float32).astype(np.float64) + np.asarray(b, np.float32).astype(np.float64)).astype(np.float32)
+
+
+def _fma32(a, b, c) -> np.ndarray:
+    with np.errstate(all="ignore"):
+        return fma_f32(a, b, c)
+
+
+def _bf16(f: np.ndarray) -> torch.Tensor:
+    return torch.from_numpy(np.ascontiguousarray(f, dtype=np.float32)).to(torch.bfloat16)
+
+
+def _scale_shift(gamma, beta, mean, invstd):
+    """The forward's per-channel coefficients: sc = rn32(gamma * invstd), sh = fma(-mean, sc, beta)."""
+    sc = _mul32(_np32(gamma), _np32(invstd))
+    return sc, _fma32(-_np32(mean), sc, _np32(beta))
+
+
+def bn_apply_ref(x, res, gamma, beta, mean, invstd, relu: bool, pair=None):
+    """bn_apply_kernel: y = bf16(relu?(fma(x, sc, sh) [+ r])) and the ReLU bits keep = (y > 0), per element of [M, C]:
+
+        sc = rn32(gamma * invstd);  sh = fma(-mean, sc, beta);  f = fma(x, sc, sh)
+        r  = res, or with ``pair = (xs, gamma_s, beta_s, mean_s, invstd_s)`` the shortcut layer's bf16(fma(xs, sc_s, sh_s))
+        f  = rn32(f + r);  relu: f = fmaxf(f, 0) (a NaN becomes 0);  y = bf16(f)
+
+    Returns (y bf16 [M, C], keep bool [M, C])."""
+    sc, sh = _scale_shift(gamma, beta, mean, invstd)
+    f = _fma32(_np32(x), sc, sh)
+    if pair is not None:
+        xs, gamma_s, beta_s, mean_s, invstd_s = pair
+        sc_s, sh_s = _scale_shift(gamma_s, beta_s, mean_s, invstd_s)
+        f = _add32(f, _np32(_bf16(_fma32(_np32(xs), sc_s, sh_s))))
+    elif res is not None:
+        f = _add32(f, _np32(res))
+    if relu:
+        f = np.fmax(f, np.float32(0.0))
+    y = _bf16(f)
+    return y, y.float() > 0
+
+
+def bn_bwd_coeffs_ref(gamma, invstd, mean, sums):
+    """bn_bwd_apply_kernel's per-channel coefficients from sums = [m1 = mean(dz), m2 = mean(dz * xhat)] ([2C] or [2, C]):
+
+        cA = gs = rn32(gamma * invstd);  cB = -rn32(rn32(gs * m2) * invstd);  cC = rn32(gs * fma(rn32(m2 * invstd), mean, -m1))
+
+    so that dx = cA dz + cB x + cC = gs (dz - m1 - xhat m2).  Returns fp32 tensors (cA, cB, cC)."""
+    s = _np32(sums).reshape(2, -1)
+    m1, m2, istd = s[0], s[1], _np32(invstd)
+    gs = _mul32(_np32(gamma), istd)
+    cB = -_mul32(_mul32(gs, m2), istd)
+    cC = _mul32(gs, _fma32(_mul32(m2, istd), _np32(mean), -m1))
+    return tuple(torch.from_numpy(v) for v in (gs, cB, cC))
+
+
+def bn_bwd_apply_ref(dy, keep, x, coeffs):
+    """bn_bwd_apply_kernel / bn_bwd_apply_dual_kernel / drc_bn_bwd_apply, per element of [M, C]:
+
+        dz = keep ? dy : 0;  dx = bf16(fma(cA, dz, fma(cB, x, cC)));  dres = bf16(dz) (exact)
+
+    ``keep`` None keeps every element (mask mode 0).  Returns (dx bf16, dres bf16)."""
+    dz = _np32(dy)
+    if keep is not None:
+        dz = np.where(keep.cpu().numpy(), dz, np.float32(0.0))
+    cA, cB, cC = (_np32(c) for c in coeffs)
+    return _bf16(_fma32(cA, dz, _fma32(cB, _np32(x), cC))), _bf16(dz)
+
+
+def bn_bwd_sums_ref(dz, x, mean, invstd):
+    """bn_bwd_reduce_kernel's sums over the rows of [M, C], for the masked gradient dz:
+
+        xhat = rn32(rn32(x - mean) * invstd);  dbeta = sum dz;  dgamma = sum dz * xhat;
+        sums = [rn32(dbeta * rn32(1/M)), rn32(dgamma * rn32(1/M))]
+
+    dbeta and dgamma are returned EXACT (fp64 sums of fp32 terms).  The kernel's fp32 sums equal them in any order when every
+    partial sum is an fp32 value: integer dz with xhat on a grid of 2^-k (an integer mean and invstd = 2^-k) whose absolute
+    sums stay below 2^(24 - k).  ``assert_exact_domain`` checks the absolute sums against 2^24; the caller keeps k small.
+    For the dual reduce call it again with the shortcut input xs, mean_s, invstd_s (its dbeta is the same).
+    Returns (dbeta fp64 [C], dgamma fp64 [C], sums fp32 [2C])."""
+    d = _np32(dz).astype(np.float64)
+    xhat = _mul32(_add32(_np32(x), -_np32(mean)), _np32(invstd)).astype(np.float64)
+    assert_exact_domain(torch.from_numpy(np.abs(d).sum(0)), torch.from_numpy(np.abs(d * xhat).sum(0)))
+    dbeta, dgamma = d.sum(0), (d * xhat).sum(0)
+    M = d.shape[0]
+    inv_m = np.float64(np.float32(1.0) / np.float32(M))
+    sums = np.concatenate([dbeta * inv_m, dgamma * inv_m]).astype(np.float32)
+    return torch.from_numpy(dbeta), torch.from_numpy(dgamma), torch.from_numpy(sums)
+
+
+def unpack_relu_bits(mask: torch.Tensor, shape) -> torch.Tensor:
+    """The forward's ReLU bits (bit i of byte (row, cv) is channel 8 cv + i of that row) as a bool tensor: [M, C] for
+    shape (M, C), NCHW for shape (n, c, h, w)."""
+    c = shape[1]
+    m = mask.reshape(-1, c // 8).long()
+    bits = torch.stack([(m >> i) & 1 for i in range(8)], dim=-1).reshape(-1, c).bool()
+    if len(shape) == 2:
+        return bits
+    n, _, h, w = shape
+    return bits.reshape(n, h, w, c).permute(0, 3, 1, 2)

@@ -4,6 +4,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+import exact_ref as X
+
 pytestmark = pytest.mark.gpu
 
 DEV = torch.device("cuda", 0)
@@ -38,13 +40,6 @@ def _fwd_with_mask(x, res, scale, shift):
     return y, mask
 
 
-def _unpack(mask, shape):
-    n, c, h, w = shape
-    m = mask.view(n * h * w, c // 8).long()
-    bits = torch.stack([(m >> i) & 1 for i in range(8)], dim=-1).reshape(n, h, w, c)
-    return bits.permute(0, 3, 1, 2).bool()
-
-
 @pytest.mark.parametrize("shape", [(2, 8, 3, 5), (4, 64, 5, 5), (3, 512, 3, 3), (2, 2048, 1, 3), (3, 8, 5, 7), (7, 64, 9, 11)])
 @pytest.mark.parametrize("with_res", [False, True])
 def test_relu_bits_equal_stored_output_positive(shape, with_res):
@@ -71,7 +66,7 @@ def test_relu_bits_equal_stored_output_positive(shape, with_res):
         res = torch.where(torch.arange(k, device=DEV).view(shape) % 3 == 0, -x.float(), res)
         res = _cl(res.to(torch.bfloat16))
     y, mask = _fwd_with_mask(x, res, scale, shift)
-    assert torch.equal(_unpack(mask, shape), y.float() > 0)
+    assert torch.equal(X.unpack_relu_bits(mask, shape), y.float() > 0)
     assert not torch.isnan(y.float()).any()
 
 

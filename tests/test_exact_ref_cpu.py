@@ -1,6 +1,7 @@
 """The checkers of tests/exact_ref.py have teeth: fed mutated fp64 "kernel outputs" of a convolution, each mutation a kernel could
 plausibly make is flagged, while the global metric of the older tests (max |out - ref| / max |ref| < 1.5e-2) lets the truncating
-store and the one-ulp element through.  Also cross-checks the fp64 tap-decomposition references against torch's fp64 convolution."""
+store and the one-ulp element through.  Also cross-checks the fp64 tap-decomposition references against torch's fp64 convolution,
+and the fp32 BatchNorm restatements against fp64 autograd of batch_norm (+ residual, + ReLU), with their own mutations."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -168,3 +169,181 @@ def test_batchnorm_statistics_reference_sees_one_masked_row():
     v64 = yd.var((0, 2, 3), unbiased=False)
     assert float(((var - v64).abs() / v64).max()) < 1e-5
     assert X.ulps_f32(rm, 0.1 * yd.mean((0, 2, 3))) <= 2
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# BatchNorm apply and backward references (exact_ref.bn_*_ref)
+# ------------------------------------------------------------------------------------------------------------------------------
+U32 = 2.0 ** -24                                                          # unit roundoff of fp32
+
+
+def _bn_real(M, c, seed, with_res):
+    """bf16 activations [M, C] with one channel at a large mean / std ratio, fp32 parameters, the fp64 batch statistics and
+    their fp32 roundings (what a convolution epilogue hands over)."""
+    g = _gen(seed)
+    off = torch.randn(c, generator=g, dtype=torch.float64) * 0.5
+    off[1] = 60.0
+    x = (torch.randn(M, c, generator=g, dtype=torch.float64) * 1.7 + off).to(torch.bfloat16)
+    res = torch.randn(M, c, generator=g, dtype=torch.float64).to(torch.bfloat16) if with_res else None
+    dy = torch.randn(M, c, generator=g, dtype=torch.float64).to(torch.bfloat16)
+    gamma = (torch.rand(c, generator=g, dtype=torch.float64) + 0.5).float()
+    beta = (torch.rand(c, generator=g, dtype=torch.float64) - 0.5).float()
+    xd = x.double()
+    mean64 = xd.mean(0)
+    istd64 = 1.0 / (xd.var(0, unbiased=False) + 1e-5).sqrt()
+    return x, res, dy, gamma, beta, mean64, istd64
+
+
+@pytest.mark.parametrize("M,c", [(63, 5), (50, 7), (9, 3), (231, 16)])
+@pytest.mark.parametrize("with_res", [False, True])
+def test_bn_references_are_batchnorm_and_its_gradient(M, c, with_res):
+    """bn_apply_ref and bn_bwd_apply_ref (fed with bn_bwd_sums_ref) against fp64 autograd of relu(batch_norm(x) + res).
+
+    Per element, with u = 2^-24, gs = gamma * invstd, xhat = (x - mean) * invstd, m1 = mean(dz), m2 = mean(dz * xhat) (all
+    exact fp64) and the fp32 statistics mean(1 + d), invstd(1 + d'), |d|, |d'| <= u:
+
+      |y - y64|   <= ulp_bf16(y) / 2 + 8u (|gs| (|x| + |mean|) + |beta| + |res| + |y64|)
+      |dx - dx64| <= ulp_bf16(dx) / 2 + 8u (|gs| (|dz| + |m1| + |xhat| (|m2| + mean|dz xhat| + |mean| invstd mean|dz|))
+                                            + |gs m2 invstd| (|x| + |mean|))
+
+    Half a bf16 ulp is the final rounding; every fp32 operation and the rounded statistics contribute O(u) relative to the
+    magnitudes they touch (at most 6 roundings per term, 8 leaves slack).  The last term is the cancellation in cB x + cC
+    when |mean| / std is large (channel 1 sits at mean / std ~ 35); the mean|dz xhat| and mean|dz| terms carry xhat's and the
+    mean's fp32 roundings into m2.  Gradients are compared where both ReLU masks agree."""
+    x, res, dy, gamma, beta, mean64, istd64 = _bn_real(M, c, M + c + with_res, with_res)
+    mean32, istd32 = mean64.float(), istd64.float()
+    xd = x.double().requires_grad_(True)
+    rd = res.double().requires_grad_(True) if with_res else None
+    gd, bd = gamma.double().requires_grad_(True), beta.double().requires_grad_(True)
+    y64 = F.batch_norm(xd, None, None, gd, bd, True, 0.1, 1e-5)
+    pre = (y64 + rd) if with_res else y64
+    y64 = F.relu(pre)
+    y64.backward(dy.double())
+
+    y, keep = X.bn_apply_ref(x, res, gamma, beta, mean32, istd32, True)
+    gs = gamma.double() * istd64
+    r_abs = res.double().abs() if with_res else 0.0
+    bound_y = X.ulp_bf16(y) / 2 + 8 * U32 * (gs.abs() * (x.double().abs() + mean64.abs()) + beta.double().abs() + r_abs
+                                            + pre.detach().abs())
+    assert bool(((y.double() - y64.detach()).abs() <= bound_y).all())
+
+    agree = keep == (y64.detach() > 0)
+    assert float(agree.double().mean()) >= 0.99
+    dz = torch.where(keep, dy, torch.zeros_like(dy))
+    dbeta, dgamma, sums = X.bn_bwd_sums_ref(dz, x, mean32, istd32)
+    dx, dres = X.bn_bwd_apply_ref(dy, keep, x, X.bn_bwd_coeffs_ref(gamma, istd32, mean32, sums))
+    assert torch.equal(dres, dz)
+    if with_res:
+        X.assert_equal(dres.float()[agree], rd.grad.float()[agree], "dres")
+    dzd = dz.double()
+    xhat = (x.double() - mean64) * istd64
+    m1, m2 = dzd.mean(0), (dzd * xhat).mean(0)
+    a_dzx, a_dz = (dzd * xhat).abs().mean(0), dzd.abs().mean(0)
+    bound_dx = X.ulp_bf16(dx) / 2 + 8 * U32 * (gs.abs() * (dzd.abs() + m1.abs() + xhat.abs() * (m2.abs() + a_dzx + mean64.abs() * istd64 * a_dz))
+                                              + (gs * m2 * istd64).abs() * (x.double().abs() + mean64.abs()))
+    err = (dx.double() - xd.grad).abs()
+    assert bool((err <= bound_dx)[agree].all()), float((err / bound_dx)[agree].max())
+    # dbeta = sum dz exactly; dgamma within the fp32 roundings of xhat and of the statistics
+    assert torch.allclose(dbeta, bd.grad, rtol=1e-12, atol=1e-12)
+    assert bool(((dgamma - gd.grad).abs() <= 8 * U32 * M * (a_dzx + mean64.abs() * istd64 * a_dz)).all())
+    # sums are the fp32 means the coefficients are formed from
+    assert X.ulps_f32(sums[:c], dbeta / M) <= 1.5 and X.ulps_f32(sums[c:], dgamma / M) <= 1.5
+
+
+def _pack_bits(keep, reverse=False):
+    """ReLU bits as bn_apply_kernel stores them: bit i of byte (row, cv) is channel 8 cv + i (bit 7 - i when ``reverse``)."""
+    k = keep.reshape(keep.shape[0], -1, 8).long()
+    sh = torch.arange(8)
+    return (k << (7 - sh if reverse else sh)).sum(-1).to(torch.uint8).flatten()
+
+
+def _old_accepts(out, ref, tol):
+    """The older tests' global metric: max |out - ref| <= tol * max(1, max |ref|) (a NaN fails it)."""
+    return float((out.double() - ref.double()).abs().max()) <= tol * max(1.0, float(ref.double().abs().max()))
+
+
+def test_bn_exact_checks_flag_every_mutation_the_old_metric_misses():
+    """Mutated restatements of the BatchNorm kernels, each flagged by the exact comparison.  Reduce-level mutations on integer
+    data (x in [-8, 8], integer means, invstd = 1/4: the sums are exact), rounding-level ones on real data with NaN / Inf.
+    The older tests' tolerances (2e-2 on y, 3e-2 on dx and dgamma, 99.5 % of mask bits) accept the listed ones."""
+    g = _gen(21)
+    M, c = 16384 + 5, 64
+    x = torch.randint(-8, 9, (M, c), generator=g).to(torch.bfloat16)
+    mean = torch.randint(-3, 4, (c,), generator=g).float()
+    istd = torch.full((c,), 0.25)
+    # gradients correlated with xhat, as a trained layer's are: dgamma ~ M, dbeta small
+    noise = torch.randint(-1, 2, (M, c), generator=g)
+    dy = torch.where(torch.rand(M, c, generator=g) < 0.7, torch.sign(x.float() - mean), noise.float()).to(torch.bfloat16)
+    gamma = (torch.rand(c, generator=g) + 0.5)
+    beta = (torch.rand(c, generator=g) - 0.5)
+    y, keep = X.bn_apply_ref(x, None, gamma, beta, mean, istd, True)
+    dz = torch.where(keep, dy, torch.zeros_like(dy))
+    dbeta, dgamma, sums = X.bn_bwd_sums_ref(dz, x, mean, istd)
+    co = X.bn_bwd_coeffs_ref(gamma, istd, mean, sums)
+    dx, _ = X.bn_bwd_apply_ref(dy, keep, x, co)
+    accepted = set()
+
+    # one row dropped from the reduction (a remainder-loop bug): last row with a nonzero dz
+    dz_drop = dz.clone()
+    dz_drop[-1] = 0
+    assert bool((dz[-1] != 0).any())
+    _, dgamma_drop, sums_drop = X.bn_bwd_sums_ref(dz_drop, x, mean, istd)
+    assert X.mismatch(dgamma_drop.float(), dgamma.float()) and X.mismatch(sums_drop, sums)
+    if _old_accepts(dgamma_drop, dgamma, 3e-2):
+        accepted.add("one dropped row in the sums")
+    # 1 / (M - 1) in the sums
+    inv = torch.tensor(1.0 / (M - 1), dtype=torch.float32).double()
+    sums_m1 = torch.cat([dbeta * inv, dgamma * inv]).float()
+    assert X.mismatch(sums_m1, sums)
+    dx_m1, _ = X.bn_bwd_apply_ref(dy, keep, x, X.bn_bwd_coeffs_ref(gamma, istd, mean, sums_m1))
+    assert X.mismatch(dx_m1, dx)
+    if _old_accepts(dx_m1, dx, 3e-2):
+        accepted.add("1/(M-1)")
+
+    # real-valued data for the rounding-level mutations
+    xr, res, dyr, gr, br, mean64, istd64 = _bn_real(M, c, 22, True)
+    xr = xr.clone()
+    xr.view(-1)[3::997] = float("nan")
+    xr.view(-1)[5::1009] = float("inf")
+    meanr, istdr = mean64.float(), istd64.float()
+    yr, keepr = X.bn_apply_ref(xr, res, gr, br, meanr, istdr, True)
+    assert not bool(yr.isnan().any())
+    dzr = torch.where(keepr, dyr, torch.zeros_like(dyr)).float()
+    sums_r = torch.cat([dzr.double().mean(0), dzr.double().mean(0) * 0.37 - 0.01]).float()    # any fp32 sums will do
+    cA, cB, cC = X.bn_bwd_coeffs_ref(gr, istdr, meanr, sums_r)
+    xrf = xr.float()
+    dxr, _ = X.bn_bwd_apply_ref(dyr, keepr, xr, (cA, cB, cC))
+    finite = torch.isfinite(dxr.float())
+    # truncating bf16 store
+    exact_pre = torch.from_numpy(X._fma32(cA.numpy(), dzr.numpy(), X._fma32(cB.numpy(), xrf.numpy(), cC.numpy())))
+    dx_rz = X.bf16_rz(exact_pre.double())
+    assert X.mismatch(dx_rz[finite], dxr[finite])
+    if _old_accepts(dx_rz[finite], dxr[finite], 3e-2):
+        accepted.add("truncating bf16 stores")
+    # cB x + cC rounded before the outer fma
+    unfused = (cB.double() * xrf.double()).float().double() + cC.double()
+    dx_unf = X._bf16(X._fma32(cA.numpy(), dzr.numpy(), unfused.float().numpy()))
+    assert X.mismatch(dx_unf, dxr)
+    if _old_accepts(dx_unf[finite], dxr[finite], 3e-2):
+        accepted.add("unfused cB*x + cC")
+    # reversed bit order in the mask
+    assert torch.equal(X.unpack_relu_bits(_pack_bits(keepr), (M, c)), keepr)
+    rev = X.unpack_relu_bits(_pack_bits(keepr, reverse=True), (M, c))
+    assert X.mismatch(rev, keepr)
+    if float((rev == keepr).double().mean()) >= 0.995:
+        accepted.add("reversed mask bits")
+    # the pair's shortcut term formed with the main layer's mean
+    xs = (torch.randn(M, c, generator=g) * 0.8 - 0.4).to(torch.bfloat16)
+    gs_, bs_, ms_, is_ = torch.rand(c, generator=g) + 0.5, torch.rand(c, generator=g) - 0.5, xs.float().mean(0), torch.full((c,), 1.25)
+    yp, _ = X.bn_apply_ref(xr, None, gr, br, meanr, istdr, True, pair=(xs, gs_, bs_, ms_, is_))
+    yp_bad, _ = X.bn_apply_ref(xr, None, gr, br, meanr, istdr, True, pair=(xs, gs_, bs_, meanr, is_))
+    assert X.mismatch(yp_bad, yp)
+    if _old_accepts(yp_bad, yp, 2e-2):
+        accepted.add("pair shortcut with the main mean")
+    # a NaN-propagating ReLU in place of fmaxf
+    y_lin, _ = X.bn_apply_ref(xr, res, gr, br, meanr, istdr, False)
+    y_nan = torch.where(y_lin.isnan(), y_lin, y_lin.clamp_min(0))
+    assert X.mismatch(y_nan, yr)
+    if _old_accepts(y_nan, yr, 2e-2):
+        accepted.add("NaN-propagating ReLU")
+    assert accepted == {"one dropped row in the sums", "1/(M-1)", "truncating bf16 stores", "unfused cB*x + cC"}, accepted
