@@ -359,9 +359,12 @@ __global__ void __launch_bounds__(DRC_THREADS) aggregate_update_kernel(const __g
   const bool first = (step == a.first_step);
   // Adam: step count t = updates so far + 1; bias corrections folded into the step size like the reference
   float adam_step_size = 0.f;
+  // fp32 beta and fp32(1 - beta) with 1 - beta formed in fp64 (HyperParams)
+  const float beta1 = (float)hp.beta1, beta2 = (float)hp.beta2;
+  const float one_minus_beta1 = (float)(1.0 - hp.beta1), one_minus_beta2 = (float)(1.0 - hp.beta2);
   if (hp.optimizer != 0) {
     const double t = (double)(step - a.first_step + 1);
-    const double bc1 = 1.0 - pow((double)hp.beta1, t), bc2 = 1.0 - pow((double)hp.beta2, t);
+    const double bc1 = 1.0 - pow(hp.beta1, t), bc2 = 1.0 - pow(hp.beta2, t);
     adam_step_size = (float)((double)hp.lr * sqrt(bc2) / bc1);
   }
   const int tile_end = a.tile_end > 0 ? a.tile_end : a.tv.ntiles;
@@ -401,10 +404,11 @@ __global__ void __launch_bounds__(DRC_THREADS) aggregate_update_kernel(const __g
         if (v.x == 0.f && v.y == 0.f) continue;             // rows outside the healthy set
         const float4* src = reinterpret_cast<const float4*>(a.grad_in + 2 * (k * a.slot_stride + idx));
         float4 c0 = ld_f4(src), c1 = ld_f4(src + 1);        // (re0,im0,re1,im1) (re2,im2,re3,im3)
-        g.x += v.x * c0.x - v.y * c0.y;
-        g.y += v.x * c0.z - v.y * c0.w;
-        g.z += v.x * c1.x - v.y * c1.y;
-        g.w += v.x * c1.z - v.y * c1.w;
+        // Re(v c) = fma(v.re, c.re, -rn(v.im c.im)), added to the row sum with one rounding
+        g.x = __fadd_rn(g.x, __fmaf_rn(v.x, c0.x, -__fmul_rn(v.y, c0.y)));
+        g.y = __fadd_rn(g.y, __fmaf_rn(v.x, c0.z, -__fmul_rn(v.y, c0.w)));
+        g.z = __fadd_rn(g.z, __fmaf_rn(v.x, c1.x, -__fmul_rn(v.y, c1.y)));
+        g.w = __fadd_rn(g.w, __fmaf_rn(v.x, c1.z, -__fmul_rn(v.y, c1.w)));
       }
     }
     if constexpr (MODE != 5 && MODE != 6 && MODE != 8) { g.x *= a.scale; g.y *= a.scale; g.z *= a.scale; g.w *= a.scale; }
@@ -419,7 +423,7 @@ __global__ void __launch_bounds__(DRC_THREADS) aggregate_update_kernel(const __g
         float d = gp[e];
         if (hp.weight_decay != 0.f) d = fmaf(hp.weight_decay, pp[e], d);
         if (hp.momentum != 0.f) {
-          float b = first ? d : fmaf(hp.momentum, mp[e], (1.f - hp.dampening) * d);
+          float b = first ? d : fmaf(hp.momentum, mp[e], hp.one_minus_dampening * d);
           mp[e] = b;
           d = hp.nesterov ? fmaf(hp.momentum, b, d) : b;
         }
@@ -433,8 +437,8 @@ __global__ void __launch_bounds__(DRC_THREADS) aggregate_update_kernel(const __g
       for (int e = 0; e < 4; ++e) {
         float d = gp[e];
         if (hp.weight_decay != 0.f) d = fmaf(hp.weight_decay, pp[e], d);
-        mp[e] = fmaf(hp.beta1, mp[e], (1.f - hp.beta1) * d);
-        vp[e] = fmaf(hp.beta2, vp[e], (1.f - hp.beta2) * d * d);
+        mp[e] = fmaf(beta1, mp[e], one_minus_beta1 * d);
+        vp[e] = fmaf(beta2, vp[e], one_minus_beta2 * d * d);
         float vv = vp[e];
         if (hp.optimizer == 2) { vmp[e] = fmaxf(vmp[e], vv); vv = vmp[e]; }
         pp[e] = fmaf(-adam_step_size, mp[e] / (sqrtf(vv) + hp.eps), pp[e]);

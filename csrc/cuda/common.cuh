@@ -23,11 +23,18 @@ struct TensorMeta {
 };
 
 struct HyperParams {             // lives in device memory so a captured graph sees updates
-  float lr, momentum, weight_decay, dampening;
+  // 48 bytes, the size the launch plans have always carried.  Every "1 - x" coefficient is formed in fp64 and rounded once to
+  // fp32, as the library optimizers and codes/oracle.py::worker_momentum_coefficients do (fp32 1.f - 0.999f is 1.29e-5 away
+  // from fp32(0.001)): fp32(1 - dampening) on the host, fp32(1 - beta) in the kernel from the fp64 betas, which the Adam bias
+  // corrections 1 - beta^t also take.
+  float lr, momentum, weight_decay;
+  float one_minus_dampening;     // fp32(1 - dampening), 1 - dampening formed in fp64 on the host
   int nesterov;
   int optimizer;                 // 0: SGD-momentum (optim/sgd_modified.py:53-88), 1: Adam, 2: AMSGrad (optim/adam_modified.py:32-92)
-  float beta1, beta2, eps;
-  int pad[3];
+  double beta1;                  // fp64 Adam betas
+  float eps;
+  int pad;
+  double beta2;
 };
 
 // ---------------------------------------------------------------------------------------------

@@ -34,9 +34,9 @@ class TensorMeta(C.Structure):
 
 
 class HyperParams(C.Structure):
-    _fields_ = [("lr", C.c_float), ("momentum", C.c_float), ("weight_decay", C.c_float), ("dampening", C.c_float),
-                ("nesterov", C.c_int), ("optimizer", C.c_int), ("beta1", C.c_float), ("beta2", C.c_float), ("eps", C.c_float),
-                ("pad", C.c_int * 3)]
+    _fields_ = [("lr", C.c_float), ("momentum", C.c_float), ("weight_decay", C.c_float), ("one_minus_dampening", C.c_float),
+                ("nesterov", C.c_int), ("optimizer", C.c_int), ("beta1", C.c_double), ("eps", C.c_float), ("pad", C.c_int),
+                ("beta2", C.c_double)]
 
 
 class TileView(C.Structure):

@@ -6,8 +6,9 @@ is a list indexed like the parameters and ``mode`` names the aggregation that pr
 to decide whether to reshape).  Gradients may be torch tensors or numpy arrays.
 
 These are the library-op optimizers used by the NCCL-baseline and CPU/Gloo transports; on the fused path the same SGD
-arithmetic runs inside ``aggregate_update_kernel`` (csrc/cuda/aggregate_update.cu) -- ``tests/test_kernels_gpu.py``
-checks the two against each other and against ``torch.optim.SGD``.
+arithmetic (and Adam / AMSGrad) runs inside ``aggregate_update_kernel`` (csrc/cuda/aggregate_update.cu) --
+``tests/test_exact_ps_update_gpu.py`` checks it bit for bit against the fp32 restatements of ``tests/exact_ref.py``, and
+``tests/test_exact_ref_cpu.py`` checks those against these optimizers and ``torch.optim.SGD`` / ``Adam`` in fp64.
 """
 from __future__ import annotations
 

@@ -117,8 +117,11 @@ def rule_plan(cfg: JobConfig) -> RulePlan:
 
 def hyperparams_tensor(cfg: JobConfig, device) -> torch.Tensor:
     opt = {"sgd": 0, "adam": 2 if getattr(cfg, "amsgrad", False) else 1}[cfg.optimizer]
-    hp = N.HyperParams(cfg.lr, cfg.momentum, cfg.weight_decay, cfg.dampening, int(cfg.nesterov), opt,
-                       float(cfg.adam_beta1), float(cfg.adam_beta2), float(cfg.adam_eps))
+    # fp32(1 - dampening) with 1 - dampening formed in fp64; the kernel forms fp32(1 - beta) the same way from the fp64 betas
+    # (DESIGN.md section 7)
+    hp = N.HyperParams(lr=cfg.lr, momentum=cfg.momentum, weight_decay=cfg.weight_decay,
+                       one_minus_dampening=1.0 - float(cfg.dampening), nesterov=int(cfg.nesterov), optimizer=opt,
+                       beta1=float(cfg.adam_beta1), eps=float(cfg.adam_eps), beta2=float(cfg.adam_beta2))
     raw = np.frombuffer(bytes(hp), dtype=np.uint8).copy()
     return torch.from_numpy(raw).to(device)
 

@@ -367,3 +367,173 @@ def unpack_relu_bits(mask: torch.Tensor, shape) -> torch.Tensor:
         return bits
     n, _, h, w = shape
     return bits.reshape(n, h, w, c).permute(0, 3, 1, 2)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# PS update (csrc/cuda/aggregate_update.cu: the gradient sources of modes 0 / 1 / 2 and the SGD / Adam / AMSGrad tail),
+# the bf16 parameter cast and the cyclic projection (csrc/cuda/fourier.cu), restated operation by operation
+# ---------------------------------------------------------------------------------------------------------------------
+# Every function takes numpy arrays (or anything np.asarray reads) and returns fp32 numpy arrays.  rn32 is one rounding to
+# fp32 of the exact result: +, -, *, / and sqrt are formed in fp64 and rounded once more to fp32, which is innocuous
+# (53 >= 2 * 24 + 2), subnormals included; fma is codes.oracle.fma_f32.  Nothing here flushes subnormals, like the kernels
+# (built without --use_fast_math).
+def _a32(x) -> np.ndarray:
+    return np.asarray(x, dtype=np.float32)
+
+
+def _div32(a, b) -> np.ndarray:
+    with np.errstate(all="ignore"):
+        return (_a32(a).astype(np.float64) / _a32(b).astype(np.float64)).astype(np.float32)
+
+
+def _sqrt32(a) -> np.ndarray:
+    with np.errstate(all="ignore"):
+        return np.sqrt(_a32(a).astype(np.float64)).astype(np.float32)
+
+
+def one_minus_f32(x: float) -> np.float32:
+    """fp32(1 - x) with 1 - x formed in fp64 and rounded once: the coefficient the update kernel reads from HyperParams."""
+    return np.float32(1.0 - float(x))
+
+
+def update_source_ref(mode: int, rows, scale: float, weights=None, recomb=None) -> np.ndarray:
+    """The aggregated gradient g (``grad_out``) of one tensor.  ``rows``: the K rows that contribute, [K, n] fp32 for modes 0
+    and 2 (row k is worker slot select[k][tensor], or slot k), complex [K, n] (or a pair (re, im)) for mode 1.  Starting from
+    acc = +0 in every mode, for k = 0, 1, ..., K - 1 in ascending order:
+
+        mode 0 (select-sum):   acc = rn32(acc + x_k)
+        mode 2 (weights):      acc = fma(w_k, x_k, acc)                         w = ``weights`` [K] fp32
+        mode 1 (cyclic):       acc = rn32(acc + fma(v.re, c.re, -rn32(v.im * c.im)))   v = ``recomb`` [K] complex64, c = x_k;
+                               a row with v.re == 0 and v.im == 0 is skipped (it is never read)
+
+    then g = rn32(acc * scale): one rounded multiply by the fp32 ``scale`` (1/K, 1/n, 1), not a divide."""
+    sc = np.float32(scale)
+    if mode == 1:
+        re, im = (rows if isinstance(rows, tuple) else (np.real(rows), np.imag(rows)))
+        re, im = _a32(re), _a32(im)
+        v = np.asarray(recomb)
+        vr, vi = _a32(np.real(v)), _a32(np.imag(v))
+        acc = np.zeros(re.shape[1:], np.float32)
+        for k in range(re.shape[0]):
+            if vr[k] == 0 and vi[k] == 0:
+                continue
+            acc = _add32(acc, _fma32(vr[k], re[k], -_mul32(vi[k], im[k])))
+        return _mul32(acc, sc)
+    x = _a32(rows)
+    acc = np.zeros(x.shape[1:], np.float32)
+    for k in range(x.shape[0]):
+        acc = _add32(acc, x[k]) if mode == 0 else _fma32(_a32(weights)[k], x[k], acc)
+    return _mul32(acc, sc)
+
+
+def sgd_tail_ref(g, p, m, *, lr: float, momentum: float, dampening: float, weight_decay: float, nesterov: bool, first: bool):
+    """SGD-momentum (torch.optim.SGD semantics) per element, on fp32 values lr, mu, wd and c = one_minus_f32(dampening):
+
+        d = g;  wd != 0: d = fma(wd, p, d)
+        mu != 0:  b = d on the first step (no dampening), else fma(mu, m, rn32(c * d));  m = b;
+                  d = nesterov ? fma(mu, b, d) : b
+        p = fma(-lr, d, p)
+
+    Returns (p, m); m is returned unchanged when mu == 0."""
+    lr32, mu, wd, c = np.float32(lr), np.float32(momentum), np.float32(weight_decay), one_minus_f32(dampening)
+    d, p, m = _a32(g), _a32(p), _a32(m)
+    if wd != 0:
+        d = _fma32(wd, p, d)
+    if mu != 0:
+        b = d.copy() if first else _fma32(mu, m, _mul32(c, d))
+        m = b
+        d = _fma32(mu, b, d) if nesterov else b
+    return _fma32(-lr32, d, p), m
+
+
+def adam_step_size_ref(lr: float, beta1: float, beta2: float, step: int, first_step: int = 1) -> np.float32:
+    """The folded Adam step size fp32(lr32 * sqrt(1 - beta2^t) / (1 - beta1^t)) formed in fp64 from the fp32 lr and the fp64
+    betas, with t = step - first_step + 1 (the updates so far, plus one).  The kernel's fp64 pow may differ from the host's
+    in the last fp64 bit; one rounding to fp32 absorbs that unless the value sits within a few fp64 ulp of an fp32 midpoint."""
+    t = float(step - first_step + 1)
+    bc1, bc2 = 1.0 - float(beta1) ** t, 1.0 - float(beta2) ** t
+    return np.float32(float(np.float32(lr)) * math.sqrt(bc2) / bc1)
+
+
+def adam_tail_ref(g, p, m, v, vmax, *, step_size, beta1: float, beta2: float, eps: float, weight_decay: float,
+                  amsgrad: bool, c1=None, c2=None):
+    """Adam / AMSGrad per element, on fp32 b1, b2, eps, wd, c1 = one_minus_f32(beta1), c2 = one_minus_f32(beta2) and the
+    fp32 ``step_size`` of ``adam_step_size_ref``:
+
+        d = g;  wd != 0: d = fma(wd, p, d)
+        m = fma(b1, m, rn32(c1 * d));  v = fma(b2, v, rn32(rn32(c2 * d) * d))
+        amsgrad: vmax = fmaxf(vmax, v) (a NaN loses to a number), s = vmax;  else s = v
+        p = fma(-step_size, rn32(m / rn32(sqrt(s) + eps)), p)       (IEEE sqrt and divide)
+
+    Returns (p, m, v, vmax) (vmax unchanged without amsgrad)."""
+    b1, b2, e, wd = np.float32(beta1), np.float32(beta2), np.float32(eps), np.float32(weight_decay)
+    c1 = one_minus_f32(beta1) if c1 is None else np.float32(c1)
+    c2 = one_minus_f32(beta2) if c2 is None else np.float32(c2)
+    d, p, m, v = _a32(g), _a32(p), _a32(m), _a32(v)
+    if wd != 0:
+        d = _fma32(wd, p, d)
+    m = _fma32(b1, m, _mul32(c1, d))
+    v = _fma32(b2, v, _mul32(_mul32(c2, d), d))
+    s = v
+    if amsgrad:
+        vmax = np.fmax(_a32(vmax), v)
+        s = vmax
+    u = _div32(m, _add32(_sqrt32(s), e))
+    return _fma32(-np.float32(step_size), u, p), m, v, (vmax if amsgrad else _a32(vmax))
+
+
+def cast_bf16_ref(x) -> np.ndarray:
+    """cast_params_kernel (__floats2bfloat162_rn): fp32 -> bf16 to nearest, ties to even, on the bit pattern; overflow rounds
+    to +-Inf, subnormals round like normals, +-0 keep their sign, a NaN stays a NaN (its payload is not specified).
+    Returns the bf16 bit patterns as uint16."""
+    u = _a32(x).view(np.uint32).astype(np.uint64)
+    r = ((u + 0x7FFF + ((u >> 16) & 1)) >> 16).astype(np.uint16)
+    nan = np.isnan(_a32(x))
+    return np.where(nan, (u >> 16).astype(np.uint16) | np.uint16(0x0040), r)
+
+
+def cyclic_project_ref(R_re, R_im, f, tile_tensor, valid) -> tuple:
+    """cyclic_project_kernel + cyclic_fold_kernel: E[t][i] = sum over tensor t of R_i[d] f[d] in fp64, in the kernels' order.
+    ``R_re`` / ``R_im``: [n, D] fp32 (D a multiple of 1024), ``f``: [D] fp32, ``tile_tensor``: [ntiles] tensor of each tile,
+    ``valid``: [ntiles] real elements of each tile.  Per tile (1024 elements, 256 threads of 4, 8 warps):
+
+        thread j (active iff 4 j < valid): x_j = ((R[4j] f[4j] + R[4j+1] f[4j+1]) + R[4j+2] f[4j+2]) + R[4j+3] f[4j+3] in fp64
+                 (every fp32 x fp32 product is exact in fp64, so contraction into DFMA cannot change a bit); inactive: 0
+        warp w:  lane values y_l = x_{32w+l}; for o = 16, 8, 4, 2, 1: y_l = y_l + y_{l xor o}; the warp's value is y_0
+        tile:    t = 0;  for w = 0..7: t = t + warp_w                                      (Epart[tile])
+    Per tensor (one warp over its tiles q = 0 .. ntile - 1):
+        lane l:  s_l = 0;  for q = l, l + 32, ...: s_l = s_l + Epart[tile0 + q];  then the same xor butterfly; E = s_0
+    The worker chunks of 8 (DRC_MAX_R) only split the work: every (worker, re / im) has its own sum.
+    Returns (E_re, E_im) fp64 [T, n]."""
+    tile_tensor = np.asarray(tile_tensor)
+    ntiles = tile_tensor.shape[0]
+    f64 = _a32(f).astype(np.float64).reshape(ntiles, 256, 4)
+    active = (np.arange(256)[None, :] * 4) < np.asarray(valid)[:, None]                  # [ntiles, 256]
+
+    def butterfly(y):                                                                    # y [..., 32] -> lane 0's value
+        for o in (16, 8, 4, 2, 1):
+            y = y + y[..., np.arange(32) ^ o]
+        return y[..., 0]
+
+    out = []
+    for Rc in (R_re, R_im):
+        Rd = _a32(Rc).astype(np.float64).reshape(-1, ntiles, 256, 4)
+        pr = Rd * f64[None]
+        x = ((pr[..., 0] + pr[..., 1]) + pr[..., 2]) + pr[..., 3]
+        x = np.where(active[None], x, 0.0)                                              # [n, ntiles, 256]
+        warps = butterfly(x.reshape(x.shape[0], ntiles, 8, 32))                         # [n, ntiles, 8]
+        ep = np.zeros(warps.shape[:2])
+        for w in range(8):
+            ep = ep + warps[..., w]                                                      # [n, ntiles]
+        T = int(tile_tensor.max()) + 1
+        E = np.zeros((T, ep.shape[0]))
+        for t in range(T):
+            tiles = np.nonzero(tile_tensor == t)[0]
+            part = ep[:, tiles]                                                          # [n, ntile]
+            s = np.zeros((ep.shape[0], 32))
+            for q0 in range(0, part.shape[1], 32):
+                blk = part[:, q0:q0 + 32]
+                s[:, :blk.shape[1]] = s[:, :blk.shape[1]] + blk
+            E[t] = butterfly(s)
+        out.append(E)
+    return out[0], out[1]

@@ -2,6 +2,9 @@
 plausibly make is flagged, while the global metric of the older tests (max |out - ref| / max |ref| < 1.5e-2) lets the truncating
 store and the one-ulp element through.  Also cross-checks the fp64 tap-decomposition references against torch's fp64 convolution,
 and the fp32 BatchNorm restatements against fp64 autograd of batch_norm (+ residual, + ReLU), with their own mutations."""
+import math
+
+import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
@@ -347,3 +350,312 @@ def test_bn_exact_checks_flag_every_mutation_the_old_metric_misses():
     if _old_accepts(y_nan, yr, 2e-2):
         accepted.add("NaN-propagating ReLU")
     assert accepted == {"one dropped row in the sums", "1/(M-1)", "truncating bf16 stores", "unfused cB*x + cC"}, accepted
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# PS update restatements (aggregate_update.cu sources and optimizer tail, cast_params, cyclic projection)
+# ---------------------------------------------------------------------------------------------------------------------
+U = 2.0 ** -24            # unit roundoff of fp32
+
+
+def _np(seed):
+    return np.random.default_rng(seed)
+
+
+def _sgd_bound_step(e_p, e_m, p, m, d_in, *, lr, mu, c, wd, nesterov, first):
+    """One step of the first-order error recurrence of ``sgd_tail_ref`` against exact arithmetic, element-wise in fp64.
+    Each rounding contributes at most U times the magnitude it rounds, each fp32 coefficient (lr, mu, wd, c) U times its term:
+
+        e_d = |wd| e_p + 2U (|wd p| + |d|)
+        e_b = e_d (first step)  or  mu e_m + c e_d + 4U (mu |m| + |c d|)
+        e_n = mu e_b + e_d + 2U (mu |b| + |d|)   (Nesterov; else e_n = e_b, and e_n = e_d without momentum)
+        e_p' = e_p + lr e_n + 3U (|p| + lr |n|)
+    Magnitudes are those of the fp64 trajectory; the test doubles the bound for the second-order terms."""
+    d = d_in + wd * p
+    e_d = abs(wd) * e_p + (2 * U * (np.abs(wd * p) + np.abs(d)) if wd else 0.0)
+    if mu:
+        if first:
+            b, e_b = d, e_d
+        else:
+            b = mu * m + c * d
+            e_b = mu * e_m + c * e_d + 4 * U * (mu * np.abs(m) + np.abs(c * d))
+        n, e_n = (mu * b + d, mu * e_b + e_d + 2 * U * (mu * np.abs(b) + np.abs(d))) if nesterov else (b, e_b)
+        m, e_m = b, e_b
+    else:
+        n, e_n = d, e_d
+    return e_p + lr * e_n + 3 * U * (np.abs(p) + lr * np.abs(n)), e_m
+
+
+@pytest.mark.parametrize("mu,damp,wd,nesterov", [(0.0, 0.0, 0.0, False), (0.9, 0.0, 5e-4, True), (0.9, 0.1, 5e-4, False),
+                                                 (0.9, 0.5, 0.0, False)])
+def test_sgd_restatement_tracks_fp64_torch_sgd(mu, damp, wd, nesterov):
+    """200 steps of ``sgd_tail_ref`` in fp32 against torch.optim.SGD in fp64 on the same fp32 gradients: every element of
+    params and momentum stays within twice the bound of ``_sgd_bound_step``."""
+    rng = _np(1)
+    n, lr = 4096, 0.05
+    p32 = rng.standard_normal(n).astype(np.float32)
+    m32 = np.zeros(n, np.float32)
+    p64 = torch.tensor(p32.astype(np.float64), requires_grad=True)
+    opt = torch.optim.SGD([p64], lr=lr, momentum=mu, dampening=damp, weight_decay=wd, nesterov=nesterov)
+    e_p = e_m = np.zeros(n)
+    c = float(X.one_minus_f32(damp))
+    for t in range(200):
+        g = (rng.standard_normal(n) * 0.1).astype(np.float32)
+        pr = p64.detach().numpy().copy()
+        mr = opt.state[p64]["momentum_buffer"].numpy().copy() if t and mu else np.zeros(n)
+        e_p, e_m = _sgd_bound_step(e_p, e_m, pr, mr, g.astype(np.float64), lr=lr, mu=mu, c=c, wd=wd, nesterov=nesterov,
+                                   first=t == 0)
+        p32, m32 = X.sgd_tail_ref(g, p32, m32, lr=lr, momentum=mu, dampening=damp, weight_decay=wd, nesterov=nesterov,
+                                  first=t == 0)
+        p64.grad = torch.from_numpy(g.astype(np.float64))
+        opt.step()
+    err = np.abs(p32 - p64.detach().numpy())
+    assert (err <= 2 * e_p).all(), f"params: worst err/bound {float((err / (2 * e_p)).max()):.3f}"
+    if mu:
+        err_m = np.abs(m32 - opt.state[p64]["momentum_buffer"].numpy())
+        assert (err_m <= 2 * e_m + 1e-300).all(), f"momentum: worst err/bound {float((err_m / (2 * e_m)).max()):.3f}"
+
+
+@pytest.mark.parametrize("amsgrad", [False, True])
+def test_adam_restatement_tracks_fp64_torch_adam(amsgrad):
+    """200 steps of ``adam_tail_ref`` in fp32 against torch.optim.Adam in fp64.  torch adds eps after dividing sqrt(v) by
+    sqrt(1 - beta2^t); the kernel (like the reference's AdamModified) folds the corrections into the step size and adds eps to
+    sqrt(v) itself, so eps = 1e-30 here makes the two formulas agree to far below fp32 resolution.  Per element and step, with
+    e_d as for SGD, r = m / (sqrt(s) + eps) and a = the step size (all magnitudes from the fp64 trajectory):
+
+        e_m = b1 e_m + c1 e_d + 4U (b1 |m| + c1 |d|)
+        e_v = b2 e_v + c2 (2 |d| e_d + e_d^2) + 5U (b2 v + c2 d^2);   AMSGrad: e_s = max(e_s, e_v)
+        e_sqrt = min(e_s / (2 sqrt(s)), sqrt(e_s)) + U sqrt(s);   e_r = e_m / sqrt(s) + |r| e_sqrt / sqrt(s) + U |r|
+        e_p' = e_p + a e_r + 2U a |r| + 2U (|p| + a |r|)
+    and every element of params, m, v (and vmax) stays within twice that bound."""
+    rng = _np(2)
+    n, lr, b1, b2, wd = 4096, 1e-3, 0.9, 0.999, 1e-4
+    p32 = rng.standard_normal(n).astype(np.float32)
+    m32, v32, vm32 = (np.zeros(n, np.float32) for _ in range(3))
+    p64 = torch.tensor(p32.astype(np.float64), requires_grad=True)
+    opt = torch.optim.Adam([p64], lr=lr, betas=(b1, b2), eps=1e-30, weight_decay=wd, amsgrad=amsgrad)
+    e_p, e_m, e_v, e_s = (np.zeros(n) for _ in range(4))
+    c1, c2 = float(X.one_minus_f32(b1)), float(X.one_minus_f32(b2))
+    m = v = vm = np.zeros(n)
+    for t in range(1, 201):
+        g = (rng.standard_normal(n) * 0.1 * (1 + (t % 7))).astype(np.float32)
+        p = p64.detach().numpy().copy()
+        d = g.astype(np.float64) + wd * p
+        e_d = wd * e_p + 2 * U * (np.abs(wd * p) + np.abs(d))
+        e_m = b1 * e_m + c1 * e_d + 4 * U * (b1 * np.abs(m) + c1 * np.abs(d))
+        e_v = b2 * e_v + c2 * (2 * np.abs(d) * e_d + e_d ** 2) + 5 * U * (b2 * v + c2 * d * d)
+        m, v = b1 * m + (1 - b1) * d, b2 * v + (1 - b2) * d * d
+        vm = np.maximum(vm, v)
+        s = vm if amsgrad else v
+        e_s = np.maximum(e_s, e_v) if amsgrad else e_v
+        rs = np.sqrt(s)
+        e_sqrt = np.minimum(e_s / (2 * rs), np.sqrt(e_s)) + U * rs
+        r = m / rs
+        e_r = e_m / rs + np.abs(r) * e_sqrt / rs + U * np.abs(r)
+        a = lr * math.sqrt(1 - b2 ** t) / (1 - b1 ** t)
+        e_p = e_p + a * e_r + 2 * U * a * np.abs(r) + 2 * U * (np.abs(p) + a * np.abs(r))
+        step = X.adam_step_size_ref(lr, b1, b2, t)
+        p32, m32, v32, vm32 = X.adam_tail_ref(g, p32, m32, v32, vm32, step_size=step, beta1=b1, beta2=b2, eps=1e-30,
+                                              weight_decay=wd, amsgrad=amsgrad)
+        p64.grad = torch.from_numpy(g.astype(np.float64))
+        opt.step()
+    st = opt.state[p64]
+    for name, got, want, bound in (("params", p32, p64.detach().numpy(), e_p), ("exp_avg", m32, st["exp_avg"].numpy(), e_m),
+                                   ("exp_avg_sq", v32, st["exp_avg_sq"].numpy(), e_v)) + (
+            (("max_exp_avg_sq", vm32, st["max_exp_avg_sq"].numpy(), e_s),) if amsgrad else ()):
+        err = np.abs(got.astype(np.float64) - want)
+        assert (err <= 2 * bound).all(), f"{name}: worst err/bound {float((err / (2 * bound)).max()):.3f}"
+
+
+def _ulps(got, want, scale=None) -> float:
+    """max |got - want| in fp32 ulps of ``scale`` (default: of want)."""
+    want = np.asarray(want, dtype=np.float64)
+    ulp = X.ulp_f32(torch.from_numpy(want if scale is None else np.asarray(scale, np.float64))).numpy()
+    return float((np.abs(np.asarray(got, np.float64) - want) / ulp).max())
+
+
+@pytest.mark.parametrize("amsgrad", [False, True])
+def test_restatements_match_library_optimizers_on_identical_aggregates(amsgrad):
+    """One step of the restatements and of SGDModified / AdamModified (the library PS, fp32 tensors) from the same state and
+    the same aggregate, at a fresh state (t = 1, v = 0) and at t = 2, 3, 10: params, momentum, exp_avg_sq and max_exp_avg_sq
+    agree within 4 fp32 ulp of the magnitudes they are formed from (the library rounds b1 m and c1 d apart where the kernel
+    fuses them, so a sum that cancels differs in more of its own ulps).  The library forms 1 - beta in fp64 and rounds it once, and takes the fp64 betas in the bias
+    corrections; a kernel that forms them in fp32 misses by about 100 ulp in v at t = 1."""
+    from draco_b200.optim import AdamModified, SGDModified
+    rng = _np(3)
+    n = 8192
+    p0 = (rng.standard_normal(n) * 1e-4).astype(np.float32)          # small params: the step itself is visible to the ulp
+    for t in (1, 2, 3, 10):
+        g = (rng.standard_normal(n) * 0.1).astype(np.float32)
+        m0 = (rng.standard_normal(n) * 0.01).astype(np.float32) if t > 1 else np.zeros(n, np.float32)
+        v0 = (rng.random(n) * 1e-3).astype(np.float32) if t > 1 else np.zeros(n, np.float32)
+        vm0 = (v0 * rng.choice([0.5, 2.0], n)).astype(np.float32)
+        pt = torch.from_numpy(p0.copy())
+        opt = AdamModified([pt], lr=1e-3, weight_decay=1e-4, amsgrad=amsgrad)
+        opt.step([torch.zeros(n)])                                      # create the state, then overwrite it
+        st = opt.state[pt]
+        pt.copy_(torch.from_numpy(p0))
+        st["step"], st["exp_avg"], st["exp_avg_sq"] = t - 1, torch.from_numpy(m0.copy()), torch.from_numpy(v0.copy())
+        if amsgrad:
+            st["max_exp_avg_sq"] = torch.from_numpy(vm0.copy())
+        opt.step([torch.from_numpy(g)])
+        p, m, v, vm = X.adam_tail_ref(g, p0, m0, v0, vm0, step_size=X.adam_step_size_ref(1e-3, 0.9, 0.999, t), beta1=0.9,
+                                      beta2=0.999, eps=1e-8, weight_decay=1e-4, amsgrad=amsgrad)
+        # ulps of the magnitudes each result is formed from (m and p may cancel): M = |b1 m| + |c1 d|, V = b2 v + c2 d^2,
+        # P = |p| + a M / (sqrt(s) + eps)
+        d = np.abs(g.astype(np.float64) + 1e-4 * p0)
+        M = 0.9 * np.abs(m0) + 0.1 * d
+        V = 0.999 * v0 + 1e-3 * d * d
+        s_ = np.maximum(V, vm0) if amsgrad else V
+        P = np.abs(p0) + float(X.adam_step_size_ref(1e-3, 0.9, 0.999, t)) * M / (np.sqrt(s_) + 1e-8)
+        for name, got, want, mag in (("params", p, pt, P), ("exp_avg", m, st["exp_avg"], M),
+                                     ("exp_avg_sq", v, st["exp_avg_sq"], V)) + (
+                (("max_exp_avg_sq", vm, st["max_exp_avg_sq"], np.maximum(V, vm0)),) if amsgrad else ()):
+            assert _ulps(got, want.numpy(), mag) <= 4, f"t={t} {name}: {_ulps(got, want.numpy(), mag)} ulp"
+    for damp, nest in ((0.0, True), (0.1, False), (0.3, False)):
+        g = (rng.standard_normal(n) * 0.1).astype(np.float32)
+        pt = torch.from_numpy(p0.copy())
+        opt = SGDModified([pt], lr=0.05, momentum=0.9, dampening=damp, weight_decay=5e-4, nesterov=nest)
+        m0 = np.zeros(n, np.float32)
+        for first in (True, False):
+            p_prev = pt.numpy().copy()
+            opt.step([torch.from_numpy(g)])
+            p, m0 = X.sgd_tail_ref(g, p_prev, m0, lr=0.05, momentum=0.9, dampening=damp, weight_decay=5e-4, nesterov=nest,
+                                   first=first)
+            mom = opt.state[pt]["momentum_buffer"].numpy()
+            Mg = np.abs(g) + 5e-4 * np.abs(p_prev) + 0.9 * np.abs(mom)              # the magnitudes m and p are formed from
+            assert _ulps(m0, mom, Mg) <= 4 and _ulps(p, pt.numpy(), np.abs(p_prev) + 0.05 * 1.9 * Mg) <= 4, (damp, first)
+
+
+def _old_close(got, want, atol) -> bool:
+    """The older GPU tests' check: allclose with an absolute tolerance (NaN where both are NaN counts as equal)."""
+    return bool(torch.allclose(torch.from_numpy(np.asarray(got, np.float64)), torch.from_numpy(np.asarray(want, np.float64)),
+                               atol=atol, rtol=0, equal_nan=True))
+
+
+def _differs(a, b) -> bool:
+    return bool(X.mismatch(torch.from_numpy(np.asarray(a, np.float32)), torch.from_numpy(np.asarray(b, np.float32))))
+
+
+def test_ps_update_exact_checks_flag_every_mutant():
+    """Mutated restatements of the update kernel's sources, optimizer tail and cast, each flagged by the exact comparison.
+    The older tests' tolerances (atol 1e-5 on params, 1e-6 on the aggregate, 5e-5 on the cyclic decode, torch.equal on the
+    cast) accept the ones listed at the end on this data (params of 1e-4, steps of 1e-3): weight decay after momentum, the fp32
+    1 - beta of the kernel before the fix, mode 0 dividing by K and an unfused mode 1.  The others move params by more than
+    1e-5 here, though at other scales (smaller lr, larger params) the old tolerances would take them too."""
+    rng = _np(4)
+    n = 8192
+    g = (rng.standard_normal(n) * 0.1).astype(np.float32)
+    p0 = (rng.standard_normal(n) * 1e-4).astype(np.float32)
+    m0 = (rng.standard_normal(n) * 0.01).astype(np.float32)
+    v0 = (rng.random(n) * 1e-3).astype(np.float32)
+    accepted = set()
+
+    def note(name, got, want, atol):
+        assert _differs(got, want), f"mutant '{name}' is not flagged"
+        if atol is not None and _old_close(got, want, atol):
+            accepted.add(name)
+
+    # ---- SGD
+    hp = dict(lr=0.05, momentum=0.9, weight_decay=5e-4)
+    p_ok, _ = X.sgd_tail_ref(g, p0, m0, dampening=0.0, nesterov=True, first=False, **hp)
+    p_mut, _ = X.sgd_tail_ref(g, p0, m0, dampening=0.0, nesterov=False, first=False, **hp)
+    note("Nesterov dropped", p_mut, p_ok, 1e-5)
+    p_ok, m_ok = X.sgd_tail_ref(g, p0, m0, dampening=0.1, nesterov=False, first=True, **hp)
+    d = X._fma32(np.float32(5e-4), p0, g)
+    b = X._mul32(X.one_minus_f32(0.1), d)                                           # dampening applied on the first step
+    note("dampening on the first step", X._fma32(-np.float32(0.05), b, p0), p_ok, 1e-5)
+    p_ok, m_ok = X.sgd_tail_ref(g, p0, m0, dampening=0.0, nesterov=False, first=False, **hp)
+    b = X._fma32(np.float32(0.9), m0, g)                                            # weight decay after momentum
+    note("weight decay after momentum", X._fma32(-np.float32(0.05), X._fma32(np.float32(5e-4), p0, b), p0), p_ok, 1e-5)
+    # ---- Adam / AMSGrad
+    ad = dict(beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=1e-4)
+    vm0 = (v0 * rng.choice([0.5, 2.0], n)).astype(np.float32)
+    step3 = X.adam_step_size_ref(1e-3, 0.9, 0.999, 3)
+    ok = X.adam_tail_ref(g, p0, m0, v0, vm0, step_size=step3, amsgrad=True, **ad)
+    dd = X._fma32(np.float32(1e-4), p0, g)
+    mm = X._fma32(np.float32(0.9), m0, X._mul32(X.one_minus_f32(0.9), dd))
+    vmax_early = np.fmax(vm0, v0)                                                   # the max taken before the v update
+    u = X._div32(mm, X._add32(X._sqrt32(vmax_early), np.float32(1e-8)))
+    note("AMSGrad max before the v update", X._fma32(-step3, u, p0), ok[0], 1e-5)
+    vv = ok[2]
+    u = X._div32(ok[1], X._sqrt32(X._add32(vv, np.float32(1e-8))))                  # eps inside the sqrt
+    ok_adam = X.adam_tail_ref(g, p0, m0, v0, vm0, step_size=step3, amsgrad=False, **ad)
+    note("eps inside the sqrt", X._fma32(-step3, u, p0), ok_adam[0], 1e-5)
+    note("bias correction at t - 1", X.adam_tail_ref(g, p0, m0, v0, vm0, step_size=X.adam_step_size_ref(1e-3, 0.9, 0.999, 4),
+                                                     amsgrad=False, **ad)[0], ok_adam[0], 1e-5)
+    # fp32 1 - beta and fp32 betas in the bias corrections (the kernel before the fix), at a fresh state
+    z = np.zeros(n, np.float32)
+    fresh = X.adam_tail_ref(g, p0, z, z, z, step_size=X.adam_step_size_ref(1e-3, 0.9, 0.999, 1), amsgrad=False, **ad)
+    b1f, b2f = np.float32(0.9), np.float32(0.999)
+    step_f32b = np.float32(float(np.float32(1e-3)) * math.sqrt(1 - float(b2f)) / (1 - float(b1f)))
+    mut = X.adam_tail_ref(g, p0, z, z, z, step_size=step_f32b, amsgrad=False, c1=np.float32(1) - b1f, c2=np.float32(1) - b2f, **ad)
+    assert _differs(mut[2], fresh[2]) and _differs(mut[0], fresh[0])
+    note("fp32 1 - beta", mut[0], fresh[0], 1e-5)
+    # ---- sources
+    for Kr in (3, 7):
+        rows = (rng.standard_normal((Kr, n)) * 0.1).astype(np.float32)
+        sc = np.float32(1.0 / Kr)
+        ok = X.update_source_ref(0, rows, sc)
+        acc = rows[0]
+        for k in range(1, Kr):
+            acc = X._add32(acc, rows[k])
+        note("mode 0 dividing by K", X._div32(acc, np.float32(Kr)), ok, 1e-6)
+    nr = 7
+    cre, cim = (rng.standard_normal((nr, n)).astype(np.float32) for _ in range(2))
+    v = (rng.standard_normal(nr) + 1j * rng.standard_normal(nr)).astype(np.complex64)
+    v[2] = 0
+    ok = X.update_source_ref(1, (cre, cim), np.float32(1 / nr), recomb=v)
+    acc = np.zeros(n, np.float32)
+    for k in range(nr):
+        if v[k] != 0:
+            acc = X._add32(acc, X._add32(X._mul32(v[k].real, cre[k]), -X._mul32(v[k].imag, cim[k])))
+    note("mode 1 unfused", X._mul32(acc, np.float32(1 / nr)), ok, 5e-5)
+    # ---- cast: truncation in place of round-to-nearest-even
+    x = (rng.standard_normal(n) * 3).astype(np.float32)
+    trunc = (x.view(np.uint32) >> 16).astype(np.uint16)
+    assert (trunc != X.cast_bf16_ref(x)).any()
+    rne = torch.from_numpy(X.cast_bf16_ref(x).view(np.int16)).view(torch.bfloat16)
+    if torch.equal(torch.from_numpy(trunc.view(np.int16)).view(torch.bfloat16), rne):
+        accepted.add("truncating bf16 cast")
+    print("mutants the older tolerances accept:", sorted(accepted))
+    assert accepted == {"weight decay after momentum", "fp32 1 - beta", "mode 0 dividing by K", "mode 1 unfused"}, accepted
+
+
+def test_update_source_and_cast_restatements_on_edges():
+    """The sources on +-0, subnormals and NaN / Inf rows, and the cast on ties, subnormals, overflow and zeros, against
+    independent formulations: torch's fp32 -> bf16 conversion and sums accumulated one fp32 add at a time."""
+    x = np.array([1.0, 1 + 2 ** -8, 1 + 3 * 2 ** -8, -(1 + 2 ** -8), 3.3961e38, 3.4e38, -3.4e38, 1e-40, -1e-40, 2 ** -133,
+                  3 * 2 ** -134, -0.0, 0.0, np.inf, -np.inf, np.nan], np.float32)
+    r = X.cast_bf16_ref(x)
+    t = torch.from_numpy(x).to(torch.bfloat16).view(torch.int16).numpy().view(np.uint16)
+    fin = ~np.isnan(x)
+    assert (r[fin] == t[fin]).all() and np.isnan(torch.from_numpy(r.view(np.int16)).view(torch.bfloat16).float().numpy()[~fin]).all()
+    rng = _np(5)
+    x = torch.from_numpy((rng.standard_normal(100000) * 100).astype(np.float32))
+    assert (X.cast_bf16_ref(x.numpy()) == x.to(torch.bfloat16).view(torch.int16).numpy().view(np.uint16)).all()
+    rows = np.array([[-0.0, -0.0, 1e-45, np.inf, np.nan, 3e38], [-0.0, 0.0, 1e-45, -np.inf, 1.0, 3e38]], np.float32)
+    g = X.update_source_ref(0, rows, 0.5)
+    assert np.signbit(g[0]) == False and g[1] == 0 and g[2] == np.float32(1e-45)        # -0 + -0 from +0 is +0; 2 ulp * 0.5
+    assert np.isnan(g[3]) and np.isnan(g[4]) and g[5] == np.inf                         # Inf - Inf, NaN, overflow
+    w = X.update_source_ref(2, rows, 1.0, weights=np.array([0.5, 0.5], np.float32))
+    # fma(0.5, 2^-149, 0) is a tie between 0 and 2^-149 and rounds to the even 0, twice; fma(0.5, 3e38, 1.5e38) does not overflow
+    assert w[2] == 0 and w[5] == np.float32(3e38)
+
+
+def test_cyclic_project_reference_is_the_fp64_projection():
+    """``cyclic_project_ref`` sums the same products as an fp64 dot product, only in the kernels' order: within 1e-12."""
+    rng = _np(6)
+    ntiles, n = 70, 5
+    tile_tensor = np.repeat(np.arange(4), [3, 1, 33, 33])
+    numel = [2500, 20, 33 * 1024 - 7, 32 * 1024 + 1]
+    valid = np.concatenate([np.clip(nl - 1024 * np.arange(c), 0, 1024) for nl, c in zip(numel, [3, 1, 33, 33])])
+    mask = (np.arange(1024)[None, :] < valid[:, None]).reshape(-1)
+    Rr, Ri = ((rng.standard_normal((n, ntiles * 1024)) * mask).astype(np.float32) for _ in range(2))
+    f = ((rng.standard_normal(ntiles * 1024) + 1) * mask).astype(np.float32)
+    Er, Ei = X.cyclic_project_ref(Rr, Ri, f, tile_tensor, valid)
+    for t in range(4):
+        sl = np.repeat(tile_tensor == t, 1024)
+        for E, R in ((Er, Rr), (Ei, Ri)):
+            ref = R[:, sl].astype(np.float64) @ f[sl].astype(np.float64)
+            assert np.abs(E[t] - ref).max() <= 1e-12 * (np.abs(R[:, sl].astype(np.float64)) @ np.abs(f[sl].astype(np.float64))).max()
