@@ -11,20 +11,18 @@ import math
 from dataclasses import asdict, dataclass
 from typing import Optional
 
+from . import rules
+
 APPROACHES = ("baseline", "maj_vote", "cyclic", "detox", "nnm")
 MODES = ("normal", "geometric_median", "krum", "maj_vote", "coordinate_median", "trimmed_mean", "multi_krum", "bulyan",
          "centered_clip", "sign_vote")
-DETOX_MODES = ("coordinate_median", "trimmed_mean", "multi_krum", "geometric_median", "bulyan", "centered_clip")
-NNM_MODES = ("coordinate_median", "trimmed_mean", "krum", "multi_krum", "geometric_median", "bulyan")
-ROBUST_MAXP = 16                    # workers the fused coordinate-wise / Krum / Bulyan kernels take (TRIM_MAXP, KRUM_MAXP)
-SIGN_VOTE_MAXP = 32                 # workers the fused sign vote takes: the adversary bitmaps are 32-bit (DRC_MAX_WORKERS)
 ERR_MODES = ("rev_grad", "constant", "random", "omniscient", "alie", "minmax", "ipm", "mimic", "none")
 TRANSPORTS = ("nvl", "nccl", "nccl_flat", "gloo")
 SCOPES = ("tensor", "model")        # --rule-scope / --attack-scope: distances per parameter tensor, or over the whole model
 # the --mode values whose rule measures distances between rows (every --approach nnm mode does, through its neighbourhoods)
 DISTANCE_MODES = ("krum", "multi_krum", "geometric_median", "bulyan", "centered_clip")
-# --bucketing: the rules that run on the worker-bucket means
-BUCKETING_MODES = ("coordinate_median", "trimmed_mean", "krum", "multi_krum", "geometric_median", "centered_clip")
+# the --approach nnm modes: the base rules of the mixed rows
+NNM_MODES = tuple(rules.BASES[b].mode for b in rules.SOURCES["nnm"].bases)
 
 
 @dataclass
@@ -122,16 +120,7 @@ class JobConfig:
         if self.no_cuda:
             self.transport = "gloo"
         self._check_sign_vote()
-        if self.approach == "baseline" and self.mode in ("coordinate_median", "trimmed_mean", "multi_krum", "bulyan"):
-            P = self.num_workers
-            self._check_rule_bounds(f"--mode {self.mode}")
-            if self.transport == "nvl" and P > ROBUST_MAXP:
-                raise ValueError(f"--mode {self.mode} on the nvl transport handles at most {ROBUST_MAXP} workers (got {P}); "
-                                 f"use --transport nccl for more")
-        if self.approach == "detox":
-            self._check_detox()
-        if self.approach == "nnm":
-            self._check_nnm()
+        rules.check(self)
         if self.compress and self.transport == "nvl" and self.err_mode == "omniscient":
             raise ValueError("--err-mode omniscient reads the honest slots in PS memory while they arrive; with --compress-grad "
                              "compress they only exist after the PS unpacked them -- pass --compress-grad None")
@@ -175,9 +164,9 @@ class JobConfig:
         if self.worker_fail >= self.num_workers:
             raise ValueError(f"--err-mode {m} builds the liars' row from the honest workers: it needs worker_fail < num_workers "
                              f"(got {self.worker_fail} of {self.num_workers})")
-        if self.transport == "nvl" and self.num_workers > ROBUST_MAXP:
-            raise ValueError(f"--err-mode {m} on the nvl transport handles at most {ROBUST_MAXP} workers (got {self.num_workers}); "
-                             f"use --transport nccl for more")
+        if self.transport == "nvl" and self.num_workers > rules.ROBUST_MAXP:
+            raise ValueError(f"--err-mode {m} on the nvl transport handles at most {rules.ROBUST_MAXP} workers (got "
+                             f"{self.num_workers}); use --transport nccl for more")
         if m == "alie" and self.attack_z is None and alie_s(self.num_workers, self.worker_fail) < 1:
             raise ValueError(f"--err-mode alie: z_max = Phi^-1((P - s) / P) with s = floor(P/2 + 1) - f is undefined for "
                              f"{self.num_workers} workers and worker_fail {self.worker_fail} (s < 1); pass --attack-z")
@@ -215,18 +204,6 @@ class JobConfig:
         if self.clip_tau is None or not (math.isfinite(self.clip_tau) and self.clip_tau > 0):
             raise ValueError(f"--mode centered_clip needs --clip-tau, a finite radius > 0 (got {self.clip_tau}): tau is in the "
                              f"gradient's own units, per tensor, so no default would mean anything")
-        detox = self.approach == "detox"
-        n, f = (self.num_groups, self.captured_group_bound) if detox else (self.num_workers, self.worker_fail)
-        what = f"{n} groups, b_G = {f}" if detox else f"{n} workers, worker_fail {f}"
-        if 2 * f >= n:
-            raise ValueError(f"--mode centered_clip averages every row around the centre: it needs the honest rows to be a strict "
-                             f"majority, {'groups > 2*b_G' if detox else 'num_workers > 2*worker_fail'} (got {what})")
-        if self.transport == "nvl" and n > ROBUST_MAXP:
-            raise ValueError(f"--mode centered_clip on the nvl transport handles at most {ROBUST_MAXP} rows (got {n}); use "
-                             f"{'a larger --group-size or ' if detox else ''}--transport nccl for more")
-        if self.transport == "nccl_flat":
-            raise ValueError("--transport nccl_flat runs the plain mean and the vote only; use --transport nccl for "
-                             "--mode centered_clip")
 
     def _check_sign_vote(self) -> None:
         """--mode sign_vote: every worker sends one bit per coordinate (its sign) and the PS takes the coordinate-wise majority."""
@@ -241,15 +218,6 @@ class JobConfig:
         if self.compress:
             raise ValueError("--mode sign_vote sends 1-bit words of signs, which the lossless codec cannot shrink: pass "
                              "--compress-grad None")
-        if self.transport == "nccl_flat":
-            raise ValueError("--transport nccl_flat runs the plain mean and the vote only; use --transport nccl for "
-                             "--mode sign_vote")
-        if 2 * self.worker_fail >= self.num_workers:
-            raise ValueError(f"--mode sign_vote needs the honest rows to be a strict majority, num_workers > 2*worker_fail (got "
-                             f"{self.num_workers} workers, worker_fail {self.worker_fail})")
-        if self.transport == "nvl" and self.num_workers > SIGN_VOTE_MAXP:
-            raise ValueError(f"--mode sign_vote on the nvl transport handles at most {SIGN_VOTE_MAXP} workers (got "
-                             f"{self.num_workers}); use --transport nccl for more")
 
     def _check_scope(self) -> None:
         """--rule-scope / --attack-scope model: the rule's distances, or min-max's gamma and Dmax, over the whole model."""
@@ -259,51 +227,19 @@ class JobConfig:
         if self.attack_scope == "model" and self.err_mode != "minmax":
             raise ValueError(f"--attack-scope model sets one gamma for the whole model: it needs --err-mode minmax (got --err-mode "
                              f"{self.err_mode}; alie is coordinate-wise, so the scope would change nothing)")
-        if self.rule_scope == "tensor" and self.attack_scope == "tensor":
-            return
-        if self.transport == "nccl_flat":
-            raise ValueError("--transport nccl_flat runs the plain mean and the vote only; use --transport nccl for "
-                             "--rule-scope model / --attack-scope model")
         if self.rule_scope == "tensor":
             return
         if not (self.approach == "nnm" or (self.approach in ("baseline", "detox") and self.mode in DISTANCE_MODES)):
             raise ValueError(f"--rule-scope model applies to the rules that measure distances between rows (--mode "
                              f"{' | '.join(DISTANCE_MODES)} under baseline or detox, and every --approach nnm mode); --approach "
                              f"{self.approach} --mode {self.mode} is coordinate-wise, so the scope would change nothing")
-        rows = self.num_groups if self.approach == "detox" else self.num_workers
-        if self.transport == "nvl" and self.mode == "geometric_median" and rows > ROBUST_MAXP:
-            raise ValueError(f"--rule-scope model: the geometric median of more than {ROBUST_MAXP} rows on the nvl transport "
-                             f"streams over the slab per tensor (got {rows} rows); use --transport nccl or fewer rows")
 
     def _check_bucketing(self) -> None:
         """--bucketing s: each step the PS permutes the P worker slots at random, averages them in worker buckets of s and runs
         ``--mode`` on the nb = ceil(P / s) bucket means, with the rule's bound over nb rows (one liar spoils one bucket)."""
-        s = self.bucketing
-        if s == 0:
-            return
-        P, f = self.num_workers, self.worker_fail
-        if self.approach != "baseline":
+        if self.bucketing != 0 and self.approach != "baseline":
             raise ValueError(f"--bucketing averages the raw worker rows before the rule: use --approach baseline (got --approach "
                              f"{self.approach})")
-        if self.mode not in BUCKETING_MODES:
-            raise ValueError(f"--bucketing takes --mode {' | '.join(BUCKETING_MODES)} (the rule applied to the bucket means), got "
-                             f"--mode {self.mode}: the mean of bucket means is the mean, Bulyan would need nb >= 4f + 3, and "
-                             f"sign_vote has no fp32 rows")
-        if not 1 <= s <= P:
-            raise ValueError(f"--bucketing s needs 1 <= s <= num_workers (got {s} with {P} workers; 0 turns it off)")
-        if self.transport == "nccl_flat":
-            raise ValueError("--transport nccl_flat runs the plain mean and the vote only; use --transport nccl for --bucketing")
-        if self.transport == "nvl" and P > ROBUST_MAXP:
-            raise ValueError(f"--bucketing on the nvl transport handles at most {ROBUST_MAXP} workers (got {P}); use --transport "
-                             f"nccl for more")
-        nb = -(-P // s)
-        what = f"{P} workers in buckets of {s} give nb = {nb} bucket rows, worker_fail {f}"
-        if self.mode in ("krum", "multi_krum") and nb <= 2 * f + 2:
-            raise ValueError(f"--bucketing --mode {self.mode} needs nb > 2*worker_fail + 2 (Krum's condition over the bucket rows; "
-                             f"{what})")
-        if self.mode not in ("krum", "multi_krum") and 2 * f >= nb:
-            raise ValueError(f"--bucketing --mode {self.mode} needs nb > 2*worker_fail (the honest bucket rows must be a strict "
-                             f"majority; {what})")
 
     def _check_dirichlet(self) -> None:
         """--dirichlet-alpha a: each data holder (a worker, or a repetition group) draws from its own shard, whose class shares
@@ -334,59 +270,6 @@ class JobConfig:
         """z of the ALIE attack: --attack-z, else z_max(num_workers, worker_fail)."""
         from .codes.adversary import alie_z_max
         return float(self.attack_z) if self.attack_z is not None else alie_z_max(self.num_workers, self.worker_fail)
-
-    def _check_rule_bounds(self, label: str) -> None:
-        """The P / f conditions of the robust rule ``--mode`` over the num_workers rows (``label`` names the flags in errors)."""
-        P, f = self.num_workers, self.worker_fail
-        if self.mode in ("coordinate_median", "trimmed_mean") and 2 * f >= P:
-            raise ValueError(f"{label} trims --worker-fail {f} values at each end of every coordinate: it needs "
-                             f"num_workers > 2*worker_fail (got {P} workers)")
-        if self.mode == "multi_krum" and P <= 2 * f + 2:
-            raise ValueError(f"{label} needs num_workers > 2*worker_fail + 2 (Krum's condition; got {P} workers, "
-                             f"worker_fail {f})")
-        if self.mode == "bulyan" and P < 4 * f + 3:
-            raise ValueError(f"{label} needs num_workers >= 4*worker_fail + 3 (Bulyan's condition; got {P} workers, "
-                             f"worker_fail {f})")
-
-    def _check_nnm(self) -> None:
-        """NNM mixes every worker's row with its num_workers - worker_fail - 1 nearest rows, then runs ``--mode`` on the mixed
-        rows with the same P / f conditions as the baseline rule."""
-        if self.mode not in NNM_MODES:
-            raise ValueError(f"--approach nnm takes --mode {' | '.join(NNM_MODES)} (the rule applied to the mixed rows), got "
-                             f"--mode {self.mode}")
-        P, f = self.num_workers, self.worker_fail
-        if not 0 <= f < P:
-            raise ValueError(f"--approach nnm mixes num_workers - worker_fail rows: it needs 0 <= worker_fail < num_workers "
-                             f"(got worker_fail {f}, {P} workers)")
-        self._check_rule_bounds(f"--approach nnm --mode {self.mode}")
-        if self.transport == "nvl" and P > ROBUST_MAXP:
-            raise ValueError(f"--approach nnm on the nvl transport handles at most {ROBUST_MAXP} workers (got {P}); use "
-                             f"--transport nccl for more")
-        if self.transport == "nccl_flat":
-            raise ValueError("--transport nccl_flat runs the plain mean and the vote only; use --transport nccl for "
-                             "--approach nnm")
-
-    def _check_detox(self) -> None:
-        """DETOX runs the robust rule across the G group winners, tolerating b_G captured groups in place of f liars."""
-        if self.mode not in DETOX_MODES:
-            raise ValueError(f"--approach detox takes --mode {' | '.join(DETOX_MODES)} (the rule applied across the group "
-                             f"winners), got --mode {self.mode}")
-        if not 1 <= self.group_size <= self.num_workers:
-            raise ValueError(f"--approach detox needs 1 <= group_size <= num_workers (got group_size {self.group_size}, "
-                             f"{self.num_workers} workers)")
-        G, b = self.num_groups, self.captured_group_bound
-        if self.mode == "multi_krum" and G <= 2 * b + 2:
-            raise ValueError(f"--approach detox --mode multi_krum needs groups > 2*b_G + 2 (Krum's condition over the group "
-                             f"winners; got {G} groups, b_G = worker_fail // ceil(group_size / 2) = {b})")
-        if self.mode == "bulyan" and G < 4 * b + 3:
-            raise ValueError(f"--approach detox --mode bulyan needs groups >= 4*b_G + 3 (Bulyan's condition over the group "
-                             f"winners; got {G} groups, b_G = worker_fail // ceil(group_size / 2) = {b})")
-        if self.mode in ("coordinate_median", "trimmed_mean", "geometric_median") and 2 * b >= G:
-            raise ValueError(f"--approach detox --mode {self.mode} needs groups > 2*b_G (got {G} groups, b_G = worker_fail // "
-                             f"ceil(group_size / 2) = {b} groups the liars can capture)")
-        if self.transport == "nvl" and G > ROBUST_MAXP:
-            raise ValueError(f"--approach detox on the nvl transport handles at most {ROBUST_MAXP} groups (got {G}); use a larger "
-                             f"--group-size or --transport nccl")
 
     @property
     def compress(self) -> bool:

@@ -38,10 +38,11 @@ from ..config import JobConfig
 from ..data import BatchPlan, TensorDataset, dirichlet_shards
 from ..ops import conv as _conv_ops
 from ..ops import kernels as K
+from ..rules import rule_plan
 from ..utils.metrics import PhaseTimer, limit_host_threads, wait_event
 from .arena import ArenaLayout
 from .placement import Placement
-from .ps import FusedPS, build_codes, rule_plan
+from .ps import FusedPS, build_codes
 from .symm import SymmContext
 from .worker import WorkerCompute, make_model
 

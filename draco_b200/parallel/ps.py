@@ -12,7 +12,6 @@ src/master/*.py):
 from __future__ import annotations
 
 import math
-from dataclasses import dataclass
 from typing import Dict, List, Optional, Sequence
 
 import numpy as np
@@ -26,93 +25,8 @@ from ..codes.oracle import (_bulyan_rounds, _krum_scores_d2, _weiszfeld_weights,
                             nnm_neighbours_d2, nnm_pair_d2, wbucket_pair_d2)
 from ..codes.repetition import GroupPlan
 from ..config import JobConfig
+from ..rules import PIPELINED_RULES, rule_plan, select_rule  # noqa: F401  (the rule names, importable here as before)
 from .arena import ArenaLayout
-
-
-def select_rule(cfg: JobConfig) -> str:
-    """Aggregation rule of a job.  Mirrors the reference's dispatch: cyclic approach -> Fourier decode
-    (cyclic_master.py:24); maj_vote approach -> vote only when ``--mode maj_vote``, plain mean for ``--mode normal``
-    (rep_master.py:118-129); baseline approach -> mean / geometric median / Krum by ``--mode`` (baseline_master.py:118-129), plus
-    three rules beyond the reference: coordinate-wise median, coordinate-wise trimmed mean and multi-Krum.  The detox approach
-    (beyond the reference too) votes inside every group and runs ``--mode`` across the group winners: ``detox_*`` rules.  Bulyan
-    (``--mode bulyan``) is beyond the reference as well, and so are centered clipping (``--mode centered_clip``, one step around
-    last step's aggregate) and the nnm approach: nearest-neighbour mixing of the worker rows, then ``--mode`` on the mixed rows
-    (``nnm_*`` rules), and signSGD with majority vote (``--mode sign_vote``), which works on the workers' sign bits."""
-    if cfg.approach == "cyclic":
-        return "cyclic"
-    if cfg.approach == "maj_vote":
-        return "vote" if cfg.mode == "maj_vote" else "mean"
-    if cfg.approach == "detox":
-        return DETOX_RULES[cfg.mode]
-    if cfg.approach == "nnm":
-        return NNM_RULES[cfg.mode]
-    return {"normal": "mean", "geometric_median": "geomedian", "krum": "krum", "coordinate_median": "median",
-            "trimmed_mean": "trimmed_mean", "multi_krum": "multi_krum", "bulyan": "bulyan",
-            "centered_clip": "centered_clip", "sign_vote": "sign_vote"}.get(cfg.mode, "mean")
-
-
-DETOX_RULES = {"coordinate_median": "detox_median", "trimmed_mean": "detox_trimmed_mean", "multi_krum": "detox_multi_krum",
-               "geometric_median": "detox_geomedian", "bulyan": "detox_bulyan",
-               "centered_clip": "detox_centered_clip"}
-NNM_RULES = {"coordinate_median": "nnm_median", "trimmed_mean": "nnm_trimmed_mean", "krum": "nnm_krum",
-             "multi_krum": "nnm_multi_krum", "geometric_median": "nnm_geomedian", "bulyan": "nnm_bulyan"}
-
-
-# rules the fused PS applies bucket by bucket while the workers still push (nothing in them reaches beyond the bucket's
-# tensors: buckets hold whole tensors, and centered clipping's centre is known before the step starts).  Only at the default
-# scopes: a whole-model distance, or min-max's whole-model gamma, needs every bucket first (RulePlan.pipelined); so does the
-# mimic attack, whose target comes from whole-model sums
-PIPELINED_RULES = ("mean", "vote", "median", "trimmed_mean", "detox_median", "detox_trimmed_mean", "centered_clip",
-                   "detox_centered_clip", "sign_vote")
-
-# the base rules FusedPS runs over worker buckets (every --bucketing rule)
-WBUCKET_FUSED_BASES = ("median", "trimmed_mean", "krum", "multi_krum", "geomedian", "centered_clip")
-
-# the optimizer's mode string for each base rule (SGDModified / AdamModified.step(mode=))
-_OPT_MODE = {"mean": "normal", "vote": "maj_vote", "cyclic": "cyclic", "median": "coordinate_median", "trimmed_mean": "trimmed_mean",
-             "krum": "krum", "multi_krum": "multi_krum", "geomedian": "geometric_median", "bulyan": "bulyan",
-             "centered_clip": "centered_clip", "sign_vote": "sign_vote"}
-
-
-@dataclass(frozen=True)
-class RulePlan:
-    """A job's aggregation rule as a row source and a base rule, with every parameter worked out once."""
-    rule: str           # select_rule's name
-    source: str         # raw: the P worker slots | detox: the G group winners of the vote | nnm: the P mixed rows |
-                        # wbucket: the nb = ceil(P / s) worker-bucket means of --bucketing s
-    base: str           # mean | vote | cyclic | median | trimmed_mean | krum | multi_krum | geomedian | bulyan | centered_clip |
-                        # sign_vote
-    rows: int           # rows the base rule runs on: P, G over the group winners, or nb over the worker buckets
-    f: int              # rows it tolerates: worker_fail, or b_G over the group winners
-    trim: int           # median / trimmed mean: values dropped at each end of a coordinate
-    m: int              # Krum / multi-Krum: rows averaged
-    theta: int          # Bulyan: rows selected
-    opt_mode: str       # the optimizer's mode string
-    pipelined: bool     # the fused PS may apply it bucket by bucket: a PIPELINED_RULES rule with both scopes "tensor", and no
-                        # --err-mode mimic
-    scope: str          # --rule-scope: tensor | model (one choice over the whole model for every tensor)
-    attack_scope: str   # --attack-scope: tensor | model (min-max: one gamma over the whole model)
-
-
-def rule_plan(cfg: JobConfig) -> RulePlan:
-    """The row source and base rule of ``select_rule(cfg)``: the vote is the mean of the group winners, ``detox_*`` runs the
-    rule across them (f = b_G), ``nnm_*`` on the mixed rows."""
-    rule = select_rule(cfg)
-    source, base = "raw", rule
-    if rule == "vote" or rule.startswith("detox_"):
-        source, base = "detox", rule.removeprefix("detox_")
-    elif rule.startswith("nnm_"):
-        source, base = "nnm", rule.removeprefix("nnm_")
-    elif cfg.bucketing:                                   # --bucketing s: the rule runs on the nb worker-bucket means
-        source, rule = "wbucket", "wbucket_" + rule
-    rows = {"detox": cfg.num_groups, "wbucket": -(-cfg.num_workers // max(cfg.bucketing, 1))}.get(source, cfg.num_workers)
-    f = cfg.captured_group_bound if source == "detox" else cfg.worker_fail
-    trim = {"median": (rows - 1) // 2, "trimmed_mean": f}.get(base, 0)
-    m = {"krum": 1, "multi_krum": rows - f}.get(base, 0)
-    scope, attack_scope = cfg.rule_scope, cfg.attack_scope
-    return RulePlan(rule, source, base, rows, f, trim, m, rows - 2 * f if base == "bulyan" else 0, _OPT_MODE[base],
-                    rule.removeprefix("wbucket_") in PIPELINED_RULES and scope == "tensor" and attack_scope == "tensor"
-                    and cfg.err_mode != "mimic", scope, attack_scope)
 
 
 def hyperparams_tensor(cfg: JobConfig, device) -> torch.Tensor:
@@ -208,8 +122,6 @@ class FusedPS:
                 kc = min(plan.m * cfg.bucketing, self.P)
                 self.wb_wsel = torch.zeros(kc, T, dtype=torch.int32, device=device)
                 self.w_raw = torch.zeros(T, kc, dtype=torch.float32, device=device)
-        if plan.source == "wbucket" and plan.base not in WBUCKET_FUSED_BASES:
-            raise ValueError(f"FusedPS: no fused worker-bucket build of the {plan.base} rule")
         if plan.base == "cyclic":
             self.code = code
             self.E = torch.zeros(T, self.P, 2, dtype=torch.float64, device=device)

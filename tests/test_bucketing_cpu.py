@@ -319,13 +319,6 @@ def test_fused_ps_distance_rules_over_buckets(monkeypatch, mode, scope):
         assert upd["K"] == min(m * 2, 15) == ps.wb_wsel.shape[0] and calls[names.index("wbucket_fold")][1]["m"] == m
 
 
-def test_fused_ps_refuses_a_bucket_rule_it_has_no_build_for(monkeypatch):
-    import draco_b200.parallel.ps as ps_mod
-    monkeypatch.setattr(ps_mod, "WBUCKET_FUSED_BASES", ("median",))
-    with pytest.raises(ValueError, match="no fused worker-bucket build"):
-        _record(_cfg(mode="trimmed_mean", transport="nvl").resolve(1), monkeypatch, None)
-
-
 def test_vectorised_bucket_table_matches_the_oracle():
     from draco_b200.parallel.ps import _wbucket_table
     rng = np.random.default_rng(3)
