@@ -49,14 +49,6 @@ __device__ __forceinline__ unsigned int liar_mask(const AttackArgs& a) {
 
 __device__ __forceinline__ float lane_of(const float4& v, int k) { return k == 0 ? v.x : k == 1 ? v.y : k == 2 ? v.z : v.w; }
 
-// one float4 row of a liar slot; the tail of a tensor is stored element by element so that padding is never written
-__device__ __forceinline__ void store_row(float* p, const float r[4], int lane_valid) {
-  if (lane_valid >= 4) { st_f4(reinterpret_cast<float4*>(p), make_float4(r[0], r[1], r[2], r[3])); return; }
-  p[0] = r[0];
-  if (lane_valid > 1) p[1] = r[1];
-  if (lane_valid > 2) p[2] = r[2];
-}
-
 // x summed over the CTA into s_part[warp][q] (warp shuffles in a fixed pattern; the warps are folded later, in order)
 __device__ __forceinline__ void warp_partial(double x, double* s_part, int q) {
 #pragma unroll

@@ -245,4 +245,12 @@ extern "C" int drc_cc_model_weights(const CcArgs* args, cudaStream_t stream) {
   cc_model_weights_kernel<<<1, DRC_THREADS, 0, stream>>>(*args);
   return (int)cudaGetLastError();
 }
+// cc_fold_kernel alone: ARC's whole-model norm (arc.cu) folds its per-tile partials [ntiles][n] into dist[T][n] with it
+extern "C" int drc_cc_fold(const CcArgs* args, cudaStream_t stream) {
+  if (args->n < 1 || args->n > CC_MAXP || !args->partials || !args->dist || args->tv.ntensors < 1)
+    return (int)cudaErrorInvalidValue;
+  const int warps = DRC_THREADS / 32;
+  cc_fold_kernel<<<(args->tv.ntensors + warps - 1) / warps, DRC_THREADS, 0, stream>>>(*args);
+  return (int)cudaGetLastError();
+}
 extern "C" int drc_sizeof_CcArgs() { return (int)sizeof(CcArgs); }

@@ -72,6 +72,13 @@ __device__ __forceinline__ void st_f4(float4* p, float4 v) {
   asm volatile("st.global.L1::no_allocate.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z),
                "f"(v.w) : "memory");
 }
+// one float4 of a slot row written in place; the tail of a tensor is stored element by element so that padding is never written
+__device__ __forceinline__ void store_row(float* p, const float r[4], int lane_valid) {
+  if (lane_valid >= 4) { st_f4(reinterpret_cast<float4*>(p), make_float4(r[0], r[1], r[2], r[3])); return; }
+  p[0] = r[0];
+  if (lane_valid > 1) p[1] = r[1];
+  if (lane_valid > 2) p[2] = r[2];
+}
 // NVLS: one store, replicated by the NVSwitch into every GPU bound to the multicast object.
 __device__ __forceinline__ void multimem_st_f4(float4* mc, float4 v) {
   asm volatile("multimem.st.relaxed.sys.global.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(mc), "f"(v.x), "f"(v.y),

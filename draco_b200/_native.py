@@ -173,6 +173,12 @@ class CcArgs(C.Structure):
                 ("t_begin", C.c_int), ("t_end", C.c_int), ("dist", ptr), ("wb_mask", ptr), ("wb_scale", ptr)]
 
 
+class ArcArgs(C.Structure):
+    _fields_ = [("grad_in", ptr), ("slot_stride", i64), ("P", C.c_int), ("k", C.c_int), ("tv", TileView), ("partials", ptr),
+                ("factors", ptr), ("dist", ptr), ("tile_begin", C.c_int), ("tile_end", C.c_int), ("t_begin", C.c_int),
+                ("t_end", C.c_int)]
+
+
 def _maybe_build() -> None:
     if os.environ.get("DRACO_NO_AUTOBUILD"):
         return
@@ -257,6 +263,11 @@ def cuda() -> C.CDLL:
             "drc_cc_dist": [C.POINTER(CcArgs), C.c_int, st],
             "drc_cc_weights": [C.POINTER(CcArgs), st],
             "drc_cc_model_weights": [C.POINTER(CcArgs), st],
+            "drc_cc_fold": [C.POINTER(CcArgs), st],
+            "drc_arc_norm": [C.POINTER(ArcArgs), C.c_int, st],
+            "drc_arc_factors": [C.POINTER(ArcArgs), st],
+            "drc_arc_model_factors": [C.POINTER(ArcArgs), st],
+            "drc_arc_scale": [C.POINTER(ArcArgs), C.c_int, st],
             "drc_wbucket_plan": [C.POINTER(WbucketPlanArgs), st],
             "drc_wbucket_table": [C.POINTER(WbucketArgs), st],
             "drc_wbucket_fold": [C.POINTER(WbucketArgs), st],

@@ -12,6 +12,8 @@ distances.
 ``worker_momentum`` is the one worker-side rule here, and it is fp32 on purpose: every path must produce its exact bits.
 ``centered_clip`` is fp64 where it measures (the distances, the weights) and fp32 where it combines rows, for the same reason.
 ``sign_pack`` / ``sign_vote`` (signSGD with majority vote) are exact integer arithmetic on the signs of fp32 values.
+``arc`` (adaptive robust clipping, a pre-aggregation step on the raw worker slots) measures in fp64 and scales with one fp32
+multiply per element.
 """
 from __future__ import annotations
 
@@ -19,6 +21,8 @@ import math
 from typing import List, Sequence, Tuple
 
 import numpy as np
+
+from ..rules import arc_k  # noqa: F401  (ARC's k, with its semantics below)
 
 
 def boyer_moore_winner(members: Sequence[np.ndarray]) -> int:
@@ -587,3 +591,48 @@ def sign_vote(bits: np.ndarray, P: int, valid) -> np.ndarray:
     n_pos = P - n_neg
     g = np.where(n_pos > n_neg, 1.0, np.where(n_neg > n_pos, -1.0, 0.0)).astype(np.float32)
     return np.where(np.asarray(valid, dtype=bool), g, np.float32(0.0)).astype(np.float32)
+
+
+def arc_row_factors(d, k: int) -> np.ndarray:
+    """ARC's fp32 factors from the fp64 squared norms ``d`` [P]: d_tau is the (k+1)-th largest d_i, a NaN ranking above every
+    number (ties do not matter: only the value is used).  a_i = 1 when !(d_i > d_tau), else fp32(sqrt(d_tau) / sqrt(d_i))
+    formed in fp64.  So a NaN row keeps factor 1, a row holding an Inf gets 0, and with more than k non-finite rows d_tau is
+    non-finite and no row is clipped."""
+    d = [float(x) for x in d]
+    tau = sorted(d, key=lambda x: (not math.isnan(x), -x if not math.isnan(x) else 0.0))[k]
+    return np.array([np.float32(math.sqrt(tau) / math.sqrt(x)) if x > tau else np.float32(1.0) for x in d], dtype=np.float32)
+
+
+def _arc_d2(X: np.ndarray) -> np.ndarray:
+    """fp64 squared norm of every row of one tensor's [P, n] fp32 values (each square exact in fp64)."""
+    X64 = np.asarray(X, dtype=np.float32).astype(np.float64)
+    with np.errstate(invalid="ignore", over="ignore"):
+        return (X64 * X64).sum(axis=1)
+
+
+def arc_factors(slots: np.ndarray, spans: Sequence[Tuple[int, int]], f: int, scope: str = "tensor") -> np.ndarray:
+    """Adaptive robust clipping's factors [T, P] fp32 (Allouah et al., arXiv 2405.14432) over the P arena-laid worker slots
+    ``slots`` [P, D] with the tensors ``spans`` (offset, numel): per tensor from its d_i (``scope="tensor"``), or one row from
+    the whole-model d_i -- the per-tensor d_i summed in ascending tensor order, ``model_d2`` -- in every tensor
+    (``scope="model"``).  k = ``arc_k(P, f)``; see ``arc_row_factors``."""
+    X = np.asarray(slots, dtype=np.float32)
+    k = arc_k(X.shape[0], f)
+    d = [_arc_d2(X[:, off:off + n]) for off, n in spans]
+    if scope == "model":
+        return np.tile(arc_row_factors(model_d2(d), k), (len(spans), 1))
+    return np.stack([arc_row_factors(di, k) for di in d])
+
+
+def arc(slots: np.ndarray, spans: Sequence[Tuple[int, int]], f: int, scope: str = "tensor", factors=None) -> np.ndarray:
+    """Adaptive robust clipping: a copy of ``slots`` in which every tensor of every row with factor a_i < 1 (``arc_factors``, or
+    ``factors``) is multiplied by a_i, one fp32 multiply per element.  Padding and the other rows are left as they are, and
+    with k = 0 nothing changes."""
+    X = np.array(slots, dtype=np.float32, copy=True)
+    if arc_k(X.shape[0], f) == 0:
+        return X
+    a = arc_factors(X, spans, f, scope) if factors is None else np.asarray(factors, dtype=np.float32)
+    with np.errstate(invalid="ignore", over="ignore"):
+        for t, (off, n) in enumerate(spans):
+            for i in np.flatnonzero(a[t] < 1):
+                X[i, off:off + n] = np.multiply(X[i, off:off + n], a[t, i], dtype=np.float32)
+    return X

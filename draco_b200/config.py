@@ -94,6 +94,7 @@ class JobConfig:
     dirichlet_alpha: Optional[float] = None  # heterogeneous data: each holder's shard has Dirichlet(alpha) class shares (None: IID)
     attack_eps: Optional[float] = None  # --err-mode ipm: the liars send -eps * mu (None: codes.adversary.IPM_EPS)
     mimic_warmup: Optional[int] = None  # --err-mode mimic: steps that learn the direction (None: codes.adversary.MIMIC_WARMUP)
+    arc: Optional[str] = None       # adaptive robust clipping of the worker slots before the rule: tensor | model (None: off)
 
     # ---- derived --------------------------------------------------------------------------
     def resolve(self, world_size: int) -> "JobConfig":
@@ -132,6 +133,7 @@ class JobConfig:
         self._check_scope()
         self._check_bucketing()
         self._check_dirichlet()
+        self._check_arc()
         if self.transport == "gloo":
             self.dtype = "fp32"
             self.cuda_graphs = False
@@ -252,6 +254,29 @@ class JobConfig:
         if self.approach == "cyclic":
             raise ValueError("--dirichlet-alpha gives every data holder its own shard; under --approach cyclic the workers split "
                              "one global batch, so there is no holder to give it to")
+
+    def _check_arc(self) -> None:
+        """--arc tensor | model: before the row source and the rule, the PS clips the k = floor(2 f (P - f) / P) worker slots
+        of largest norm to the norm of the next largest (per tensor, or over the whole model)."""
+        if self.arc is None:
+            return
+        if self.arc not in SCOPES:
+            raise ValueError(f"--arc must be one of {SCOPES} (or unset for no clipping), got {self.arc!r}")
+        if self.approach == "cyclic":
+            raise ValueError("--arc scales real gradient rows; the cyclic code's slots hold complex codewords, so it has no "
+                             "meaning there -- use another --approach or drop --arc")
+        if self.mode == "sign_vote":
+            raise ValueError("--arc multiplies a row by a positive factor, which changes none of its signs: --mode sign_vote "
+                             "would vote exactly as without it -- drop --arc")
+        if self.transport == "nccl_flat":
+            raise ValueError("--transport nccl_flat runs the plain mean and the vote on the raw buckets only; use --transport "
+                             "nvl or nccl for --arc")
+        if not 0 <= self.worker_fail <= self.num_workers:
+            raise ValueError(f"--arc clips floor(2 f (P - f) / P) rows with f = --worker-fail: it needs 0 <= worker_fail <= "
+                             f"num_workers (got {self.worker_fail} of {self.num_workers})")
+        if self.transport == "nvl" and self.num_workers > rules.ROBUST_MAXP:
+            raise ValueError(f"--arc on the nvl transport handles at most {rules.ROBUST_MAXP} workers (its norm pass holds the "
+                             f"rows in registers; got {self.num_workers}); use --transport nccl for more")
 
     @property
     def ipm_eps(self) -> float:
@@ -375,6 +400,11 @@ def add_fit_args(parser: argparse.ArgumentParser) -> argparse.ArgumentParser:
       help="heterogeneous data: every data holder (a worker; a group under maj_vote / detox) samples from its own shard, whose "
            "class shares are drawn from Dirichlet(alpha) (small alpha: few classes per holder).  Unset: every worker samples "
            "the whole dataset")
+    a("--arc", type=str, default=None, choices=SCOPES,
+      help="adaptive robust clipping (Allouah et al. 2024; every approach but cyclic, not with --mode sign_vote): before the "
+           "row source and the rule, the PS clips the k = floor(2 f (P - f) / P) worker rows of largest norm (f = --worker-fail) "
+           "to the norm of the next largest.  tensor: one norm per parameter tensor; model: one norm per worker over the whole "
+           "model, as in the paper.  No parameter of its own; with f = 0 it does nothing")
     a("--approach", type=str, default=d.approach,
       help="baseline | maj_vote | cyclic | detox (majority vote inside each repetition group, then --mode across the G group "
            "winners) | nnm (nearest-neighbour mixing: every worker's row is replaced, per tensor, by the mean of its "

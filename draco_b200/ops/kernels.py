@@ -620,6 +620,93 @@ def centered_clip_update(layout: ArenaLayout, grad_in: Addr, slot_stride: int, *
                    tile_range=tile_range, grid=grid)
 
 
+# ------------------------------------------------------------------------------------------------ adaptive robust clipping
+class ArcWorkspace:
+    """ARC's scratch (csrc/cuda/arc.cu): the per-tile fp64 partials [ntiles, P], the fp32 factors [T, P] of the last clip and,
+    with ``model``, the per-tensor fp64 d_i [T, P] the whole-model norm is summed from."""
+
+    def __init__(self, layout: ArenaLayout, P: int, device, model: bool):
+        _check_cc_rows("ArcWorkspace", P)
+        self.partials = torch.zeros(layout.ntiles, P, dtype=torch.float64, device=device)
+        self.factors = torch.ones(layout.ntensors, P, dtype=torch.float32, device=device)
+        self.dist = torch.zeros(layout.ntensors, P, dtype=torch.float64, device=device) if model else None
+
+
+def _arc_args(layout: ArenaLayout, P: int, k: int, ws: ArcWorkspace, grad_in: Addr = None) -> N.ArcArgs:
+    _check_cc_rows("arc", P)
+    if not 0 <= k < P:
+        raise ValueError(f"arc: clips k in 0..P-1 of the P = {P} rows, got k = {k}")
+    _check_buffer("arc: partials", ws.partials, torch.float64, (layout.ntiles, P))
+    _check_buffer("arc: factors", ws.factors, torch.float32, (layout.ntensors, P))
+    a = N.ArcArgs()
+    a.grad_in, a.P, a.k, a.tv = addr(grad_in), P, k, layout.tile_view(ws.factors.device)
+    a.partials, a.factors = ws.partials.data_ptr(), ws.factors.data_ptr()
+    return a
+
+
+def _tile_grid(layout: ArenaLayout, a: N.ArcArgs, tile_range: Optional[tuple], grid: Optional[int]) -> int:
+    ntiles = layout.ntiles
+    if tile_range is not None:
+        a.tile_begin, a.tile_end = int(tile_range[0]), int(tile_range[1])
+        ntiles = a.tile_end - a.tile_begin
+    return grid or max(1, min(ntiles, sm_count() * 8))
+
+
+def arc_norm(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, ws: ArcWorkspace, *,
+             tile_range: Optional[tuple] = None, grid: Optional[int] = None) -> None:
+    """ARC's squared norms: for every tile of ``tile_range`` (one bucket; None: the arena) and each of the P worker slots, the
+    fp64 sum of (double)x^2 over the tile's real elements into ``ws.partials``."""
+    a = _arc_args(layout, P, 0, ws, grad_in)
+    a.slot_stride = slot_stride
+    N.check(N.cuda().drc_arc_norm(C.byref(a), _tile_grid(layout, a, tile_range, grid), _stream()), "arc_norm")
+
+
+def arc_factors(layout: ArenaLayout, P: int, k: int, ws: ArcWorkspace, *, tensor_range: Optional[tuple] = None) -> None:
+    """Fold ``arc_norm``'s partials per tensor in tile order into d_i and write the factors of ``tensor_range`` (None: every
+    tensor) into ``ws.factors`` (codes/oracle.py ``arc_row_factors``)."""
+    a = _arc_args(layout, P, k, ws)
+    if tensor_range is not None:
+        a.t_begin, a.t_end = int(tensor_range[0]), int(tensor_range[1])
+    N.check(N.cuda().drc_arc_factors(C.byref(a), _stream()), "arc_factors")
+
+
+def arc_model_factors(layout: ArenaLayout, P: int, k: int, ws: ArcWorkspace) -> None:
+    """``--arc model``: fold ``arc_norm``'s partials per tensor into ``ws.dist`` (clip.cu's cc_fold_kernel), sum them over the
+    tensors in ascending order and write the one factor row into every row of ``ws.factors``.  Two kernels."""
+    a = _arc_args(layout, P, k, ws)
+    _check_buffer("arc: dist", ws.dist, torch.float64, (layout.ntensors, P))
+    a.dist = ws.dist.data_ptr()
+    f = N.CcArgs()
+    f.n, f.tv, f.partials, f.dist = P, a.tv, ws.partials.data_ptr(), ws.dist.data_ptr()
+    N.check(N.cuda().drc_cc_fold(C.byref(f), _stream()), "cc_fold")
+    N.check(N.cuda().drc_arc_model_factors(C.byref(a), _stream()), "arc_model_factors")
+
+
+def arc_scale(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, ws: ArcWorkspace, *,
+              tile_range: Optional[tuple] = None, grid: Optional[int] = None) -> None:
+    """Multiply in place, over the tiles of ``tile_range``, every slot row whose factor for the tile's tensor is below 1 (one
+    fp32 multiply per real element; padding and the other rows are not touched)."""
+    a = _arc_args(layout, P, 0, ws, grad_in)
+    a.slot_stride = slot_stride
+    N.check(N.cuda().drc_arc_scale(C.byref(a), _tile_grid(layout, a, tile_range, grid), _stream()), "arc_scale")
+
+
+def arc_clip(layout: ArenaLayout, grad_in: Addr, slot_stride: int, P: int, k: int, ws: ArcWorkspace, *,
+             tile_range: Optional[tuple] = None, tensor_range: Optional[tuple] = None, grid: Optional[int] = None) -> int:
+    """Adaptive robust clipping of the P worker slots in place (codes/oracle.py ``arc``): the norms, the factors, the scale.
+    Per tensor over one bucket (``tile_range`` / ``tensor_range``; None: the arena), or, when ``ws`` holds ``dist``, once over
+    the whole model (no ranges).  The factors stay in ``ws.factors``.  Returns the kernels launched."""
+    if ws.dist is not None and (tile_range is not None or tensor_range is not None):
+        raise ValueError("arc_clip: the whole-model norm needs every tile, so it takes no bucket")
+    arc_norm(layout, grad_in, slot_stride, P, ws, tile_range=tile_range, grid=grid)
+    if ws.dist is not None:
+        arc_model_factors(layout, P, k, ws)
+    else:
+        arc_factors(layout, P, k, ws, tensor_range=tensor_range)
+    arc_scale(layout, grad_in, slot_stride, P, ws, tile_range=tile_range, grid=grid)
+    return 4 if ws.dist is not None else 3
+
+
 def stream_push(src: Addr, dst: Addr, nbytes: Addr, nbytes_out: Addr = None, *, step_ptr: Addr, done_counter: Addr, flag: Addr = None,
                 grid: int = 16) -> None:
     """Store ``*nbytes`` bytes (device scalar) of a packed stream into a peer buffer and raise the step-stamped flag

@@ -226,6 +226,8 @@ class FusedEngine:
             if self.cfg.err_mode in PS_ATTACKS and self.adv_bitmap is not None:
                 for w in self.schedule.ranks[step % len(self.schedule.ranks)]:   # slots the PS overwrote with the attack row
                     hv[int(w) - 1] = 0
+            if self.ps.arc_ws is not None:                # slots --arc rescaled this step (a factor below 1 in some tensor)
+                hv[(self.ps.arc_ws.factors < 1).any(0).cpu()] = 0
             bad = [w + 1 for w in range(self.P) if hv[w] and int(got[w]) != int(exp[w])]
             self.checksum_log.append({"step": step, "checked": int(hv.sum()), "bad": bad})
             if bad:

@@ -21,8 +21,8 @@ from .. import _native as N
 from ..codes.adversary import ATTACK_ALIE, ATTACK_IPM, ATTACK_MIMIC, ATTACK_MINMAX, PS_ATTACKS, attack_code, mimic_z0
 from ..codes.bucketing import bucket_schedule, wbuckets
 from ..codes.cyclic import CyclicCode, search_w
-from ..codes.oracle import (_bulyan_rounds, _krum_scores_d2, _weiszfeld_weights, centered_clip_weight, model_d2,
-                            nnm_neighbours_d2, nnm_pair_d2, wbucket_pair_d2)
+from ..codes.oracle import (_bulyan_rounds, _krum_scores_d2, _weiszfeld_weights, arc_factors, arc_k, centered_clip_weight,
+                            model_d2, nnm_neighbours_d2, nnm_pair_d2, wbucket_pair_d2)
 from ..codes.repetition import GroupPlan
 from ..config import JobConfig
 from ..rules import PIPELINED_RULES, rule_plan, select_rule  # noqa: F401  (the rule names, importable here as before)
@@ -76,6 +76,10 @@ class FusedPS:
             z0 = mimic_z0([(sp.offset, sp.numel) for sp in layout.specs], layout.total)
             self.mimic = K.MimicState(layout, self.P, device, torch.from_numpy(z0))
         self.attack_ws = K.AttackWorkspace(layout, self.P, device) if self.attack == ATTACK_MINMAX else None
+        # --arc: the worker slots clipped in place after the attack, per bucket (tensor) or after the last one (model); k = 0
+        # (worker_fail 0) clips nothing, so nothing is allocated or launched
+        self.arc_k = arc_k(self.P, cfg.worker_fail) if cfg.arc else 0
+        self.arc_ws = K.ArcWorkspace(layout, self.P, device, model=cfg.arc == "model") if self.arc_k > 0 else None
         # --attack-scope model: min-max's per-tensor sums, folded, then one solve over the whole arena
         self.attack_fold = (K.attack_fold_buffer(layout, self.P, device)
                             if self.attack == ATTACK_MINMAX and plan.attack_scope == "model" else None)
@@ -179,6 +183,9 @@ class FusedPS:
                 n += K.ps_attack(L, self.grad_in, self.slot_stride, self.P, self.attack, adv_bitmap=self.adv_bitmap,
                                  adv_len=self.adv_len, step_ptr=step_ptr, z=self.attack_z, ws=self.attack_ws,
                                  tile_range=tiles, tensor_range=tensors)
+            if self.arc_ws is not None:                    # --arc model is never pipelined: one pass over the arena
+                n += K.arc_clip(L, self.grad_in, self.slot_stride, self.P, self.arc_k, self.arc_ws, tile_range=tiles,
+                                tensor_range=tensors)
             # row source: `rows` is the table of the worker slots the base rule reads (None: slot i is row i)
             rows = None
             if plan.source == "detox":
@@ -325,6 +332,7 @@ class TorchPS:
             self.mimic_m = layout.new_arena(device)
             self.mimic_z = torch.from_numpy(mimic_z0([(sp.offset, sp.numel) for sp in layout.specs], layout.total)).to(device)
         self.mimic_target = -1
+        self.arc_k = arc_k(self.P, cfg.worker_fail) if cfg.arc else 0
         # --bucketing: the permutation of every step (row step % len, as the fused PS reads it)
         self.wb_schedule = bucket_schedule(self.P, cfg.max_steps, cfg.seed) if self.plan.source == "wbucket" else None
         if self.plan.base == "cyclic":
@@ -445,6 +453,19 @@ class TorchPS:
             for sp in specs:
                 sl = slice(sp.offset, sp.offset + sp.numel)
                 z[sl] = (u[sl] / nrm).float()
+
+    # --- adaptive robust clipping ----------------------------------------------------------------
+    def arc_clip(self, slots: torch.Tensor) -> torch.Tensor:
+        """``--arc``: every tensor of every worker slot with factor a_i < 1 (``oracle.arc_factors`` over the slots) multiplied by
+        a_i in place, one fp32 multiply per element, as the fused PS clips its slab.  Returns the factors [T, P]."""
+        specs = self.layout.specs
+        a = arc_factors(slots.detach().cpu().numpy(), [(sp.offset, sp.numel) for sp in specs], self.cfg.worker_fail,
+                        self.cfg.arc)
+        for t, sp in enumerate(specs):
+            for i in np.flatnonzero(a[t] < 1).tolist():
+                slots[i, sp.offset: sp.offset + sp.numel] *= torch.tensor(a[t, i], dtype=torch.float32, device=slots.device)
+        self.last_info["arc_factors"] = a
+        return torch.from_numpy(a)
 
     # --- per-tensor rules -----------------------------------------------------------------------
     def _vote_tensor(self, rows: List[torch.Tensor]) -> int:
@@ -629,6 +650,8 @@ class TorchPS:
         the mixed rows, or the worker-bucket means of ``step``'s permutation), then the base rule's helper on them."""
         plan = self.plan
         self.last_info = {}
+        if self.arc_k > 0:
+            self.arc_clip(slots)
         if plan.base == "sign_vote":
             return self._sign_vote(slots)
         if plan.scope == "model":

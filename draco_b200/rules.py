@@ -101,9 +101,16 @@ def route(cfg) -> Tuple[str, str]:
 
 # rules the fused PS applies bucket by bucket while the workers still push (buckets hold whole tensors, and centered clipping's
 # centre is known before the step starts); with the worker buckets too.  Not NNM, whose neighbourhoods need whole-tensor
-# distances, and only at the default scopes and without the mimic attack, which need whole-model sums (RulePlan.pipelined)
+# distances, and only at the default scopes and without the mimic attack or a clipping --arc model, which need whole-model sums
+# (RulePlan.pipelined)
 PIPELINED_RULES = ("mean", "vote", "median", "trimmed_mean", "detox_median", "detox_trimmed_mean", "centered_clip",
                    "detox_centered_clip", "sign_vote")
+
+
+def arc_k(P: int, f: int) -> int:
+    """Rows adaptive robust clipping (--arc) clips among the P worker slots: k = floor(2 f (P - f) / P) in integer arithmetic
+    (k >= f when f <= P / 2; k = 0 when f = 0, and --arc is then a no-op)."""
+    return (2 * f * (P - f)) // P
 
 
 def select_rule(cfg) -> str:
@@ -184,7 +191,8 @@ class RulePlan:
     m: int              # Krum / multi-Krum: rows averaged
     theta: int          # Bulyan: rows selected
     opt_mode: str       # the optimizer's mode string
-    pipelined: bool     # the fused PS may apply it bucket by bucket: PIPELINED_RULES, both scopes "tensor", no mimic
+    pipelined: bool     # the fused PS may apply it bucket by bucket: PIPELINED_RULES, both scopes "tensor", no mimic, no
+                        # --arc model that clips (k > 0)
     scope: str          # --rule-scope: tensor | model (one choice over the whole model for every tensor)
     attack_scope: str   # --attack-scope: tensor | model (min-max: one gamma over the whole model)
 
@@ -199,6 +207,6 @@ def rule_plan(cfg) -> RulePlan:
     m = {"krum": 1, "multi_krum": rows - f}.get(base, 0)
     scope, attack_scope = cfg.rule_scope, cfg.attack_scope
     pipelined = (rule.removeprefix("wbucket_") in PIPELINED_RULES and scope == "tensor" and attack_scope == "tensor"
-                 and cfg.err_mode != "mimic")
+                 and cfg.err_mode != "mimic" and not (cfg.arc == "model" and arc_k(cfg.num_workers, cfg.worker_fail) > 0))
     return RulePlan(rule, source, base, rows, f, trim, m, rows - 2 * f if base == "bulyan" else 0, BASES[base].mode, pipelined,
                     scope, attack_scope)
